@@ -55,7 +55,12 @@ def parse():
                     help="BASELINE.json config: 1 = HashGrid 8-level, 1-layer-32 MLP, 256^2 single view (the reference's CPU-runnable case; same runner as 2), "
                          "2 = HashGrid NeRF fwd+bwd (headline), 3 = nglod OctreeGrid SDF sphere trace, 4 = TriplanarGrid NeRF")
     ap.add_argument("--hidden-dim", type=int, default=0, help="configs 1/2: decoder width override (128 = the reference's best published app/nerf setting)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="configs 1/2: after the timed steps, write what the last timed step computed (loss, rendered rgb, updated decoder "
+                         "parameters, a fixed sample of the updated hash table) as DIR/<name>.npy")
     a = ap.parse_args()
+    if a.dump_outputs and a.config in (3, 4):
+        ap.error("--dump-outputs is implemented for configs 1 and 2")
     if a.config == 1 and a.res == 1024:
         a.res = 256
     return a
@@ -344,9 +349,10 @@ def run_ours(args):
     e0.record()
     step_ev[0].record()
     total_samples = 0
+    last_loss = None
     for k in range(args.steps):
         i = args.warmup + k
-        step(i, *dev_rays[i], dev_tgt[i], nxt=dev_rays[i + 1] if k + 1 < args.steps else None)
+        last_loss = step(i, *dev_rays[i], dev_tgt[i], nxt=dev_rays[i + 1] if k + 1 < args.steps else None)
         total_samples += tracer.get_prev_num_samples()
         step_ev[k + 1].record()
     e1.record()
@@ -360,6 +366,8 @@ def run_ours(args):
     stage_ms = {}
     for name, a, b in prof:
         stage_ms.setdefault(name, []).append(a.elapsed_time(b))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_loss, nef, stepper.last_rgb if native else None)
 
     # ---- timed: end to end from host buffers through the public API ----
     copy_stream = torch.cuda.Stream(device=dev)
@@ -436,9 +444,9 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
-    tfl = float(peaks.get("bf16_tflops_sustained", 1400.0))            # kernels timed inside a long step -> sustained figure
-    src = "MEASURED_PEAKS.json (measured)" if peaks else "fallback 6650 GB/s / 1400 TFLOP/s"
+    hbm = float(peaks.get("hbm_gbs", 3350.0))
+    tfl = float(peaks.get("bf16_tflops_sustained", 989.0))
+    src = "MEASURED_PEAKS.json (measured)" if peaks else "H100 SXM data sheet: 3350 GB/s HBM3, 989 TFLOP/s dense fp16 (not reached figures)"
     traffic = {}
     try:
         traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))     # dram bytes per launch from the last ncu --set full capture
@@ -453,7 +461,7 @@ def run_ours(args):
         "table_scatter": ("wb_table_scatter_kernel", "hbm", 2 * L_eff * 8 * 2 * e, "B"),
         # the fused backward kernel moves, per hit sample, the 64 B of saved features in and the read-modify-write of the table entries
         # (2 * L * 8 * F * 4 B): that is its SURVEY 8(d) figure; its decoder FLOPs are reported as a second line below
-        "shade_bwd": (((("wb_mlp_bwd3_tc_kernel<FUSE> (decoder backward + table scatter)" if hidden in (64, 128) else "wb_mlp_bwd_tc_kernel + wb_table_scatter_kernel (one stage)"),
+        "shade_bwd": (((("wb_mlp_bwd_tc_kernel<FUSE> (decoder backward + table scatter)" if hidden == 64 else "wb_mlp_bwd_tc_kernel + wb_table_scatter_kernel (one stage)"),
                         "hbm", 4 * n_lods + 2 * L_eff * 8 * 2 * e, "B")) if args.precision == 1
                       else ("wb_shade_bwd_kernel", "hbm", 2 * L_eff * 8 * 2 * e, "B")),
         "decoder_bwd": ("wb_mlp_bwd_tc_kernel", "tensor", 3 * dec_flop, "FLOP"),     # forward recompute + data grad + weight grad of both decoders
@@ -481,9 +489,9 @@ def run_ours(args):
     if args.precision == 1 and "shade_bwd" in mean_ms:   # the same launch against the tensor roof: recompute + data grad + weight grad of both decoders
         t_s = mean_ms["shade_bwd"] * 1e-3
         ach = S_step * (3 * dec_flop) / t_s / 1e12
-        rooflines.append({"bound": "tensor", "kernel": "wb_mlp_bwd3_tc_kernel<FUSE> (decoder part)", "achieved": ach, "peak": tfl, "unit": "TFLOP/s", "frac": ach / tfl,
-                          "traffic": traffic.get("wb_mlp_bwd3_tc_kernel"), "kernel_ms": mean_ms["shade_bwd"] - 1e-9, "algorithmic_per_sample": f"{3 * dec_flop} FLOP",
-                          "samples_per_launch": S_step, "note": "same launch as the hbm line of this kernel; the decoder rounds alone take 3.7 of its 7.0 ms (profiles/README.md)"})
+        rooflines.append({"bound": "tensor", "kernel": "wb_mlp_bwd_tc_kernel<FUSE> (decoder part)", "achieved": ach, "peak": tfl, "unit": "TFLOP/s", "frac": ach / tfl,
+                          "traffic": traffic.get("wb_mlp_bwd_tc_kernel"), "kernel_ms": mean_ms["shade_bwd"] - 1e-9, "algorithmic_per_sample": f"{3 * dec_flop} FLOP",
+                          "samples_per_launch": S_step, "note": "same launch as the hbm line of this kernel"})
     roofline = dict(max(rooflines, key=lambda r: r["kernel_ms"]))
     roofline["peak_source"] = src
     roofline["note"] = ("dominant kernel by time.  hbm-bound kernels: the 41.7 MB table is L2 resident, so `achieved` is HBM-equivalent gather/scatter "
@@ -510,6 +518,26 @@ def run_ours(args):
     if world > 1:
         dist.destroy_process_group()
 
+
+
+DUMP_TABLE_ROWS = 1 << 18          # fixed sample of hash-table rows in --dump-outputs (the whole table is 2^19 x 16 levels)
+
+
+def dump_outputs(out_dir, loss, nef, rgb):
+    """What the last timed step hands its caller: the loss, the rendered rgb (native step) and the parameters it updated, as float32 /
+    float64 .npy files (< 64 MB in all).  The table is sampled at rows drawn from a fixed seed, so two builds compare entry for entry."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    flat = lambda dec: torch.cat([t.detach().reshape(-1) for l in list(dec.layers) + [dec.lout] for t in (l.weight, l.bias)]).float().cpu().numpy()
+    table = nef.grid.codebook.feats.detach()
+    rows = np.sort(np.random.default_rng(0).choice(table.shape[0], size=min(DUMP_TABLE_ROWS, table.shape[0]), replace=False))
+    arrays = {"loss": np.array([float(loss)], np.float64), "decoder_density": flat(nef.decoder_density), "decoder_color": flat(nef.decoder_color),
+              "grid_table_rows": rows.astype(np.float64), "grid_table_sample": table[torch.from_numpy(rows).to(table.device)].float().cpu().numpy()}
+    if rgb is not None:
+        arrays["rgb"] = rgb.detach().float().cpu().numpy()
+    for name, arr in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), arr)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -579,9 +607,9 @@ def parity_leg(args, O, W, torch, dev, spc_np, onef, pipe, tracer, nef, stepper=
 def _peaks():
     try:
         pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        return float(pk.get("hbm_gbs", 6650.0)), "MEASURED_PEAKS.json (measured)"
+        return float(pk.get("hbm_gbs", 3350.0)), "MEASURED_PEAKS.json (measured)"
     except Exception:
-        return 6650.0, "fallback 6650 GB/s (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet: 3350 GB/s HBM3 (not a reached figure)"
 
 
 def _ncu_facts(roof: dict, key: str) -> dict:
@@ -863,7 +891,7 @@ def run_config4(args):
         per = 4 * 3 * 4 * 4 * 4                                                   # SURVEY 8(d): L * 3 planes * 4 texels * fdim * 4 B = 768 B/sample
         roofs = []
         for st_name, kern, mult in (("shade_fwd", "wb_shade_fwd_tc_kernel<GX>" if args.precision == 1 else "wb_shade_fwd_kernel", 1),
-                                    ("table_scatter", "wb_featx_scatter_kernel", 2), ("decoder_bwd", "wb_mlp_bwd3_tc_kernel", 0)):
+                                    ("table_scatter", "wb_featx_scatter_kernel", 2), ("decoder_bwd", "wb_mlp_bwd_tc_kernel", 0)):
             if st_name in mean and mult:
                 a = S_step * per * mult / (mean[st_name] * 1e-3) / 1e9
                 roofs.append({"bound": "hbm", "kernel": kern, "achieved": a, "peak": hbm, "unit": "GB/s", "frac": a / hbm, "traffic": None,

@@ -1,5 +1,5 @@
 /*
- * wispb200.h -- C ABI of libwispb200.so: the B200 (sm_100a) volumetric render path that drops in behind
+ * wispb200.h -- C ABI of libwispb200.so: the H100 (sm_90a) volumetric render path that drops in behind
  * kaolin-wisp's Pipeline / BaseTracer / BLASGrid / BaseNeuralField API.
  *
  * Conventions (SURVEY.md 8(b)):
@@ -28,7 +28,7 @@ enum wb_status {
     WB_OK = 0,
     WB_ERR_INVALID = -1,            /* bad argument / unsupported configuration */
     WB_ERR_CUDA = -2,               /* a CUDA runtime call failed (message has the cudaError string) */
-    WB_ERR_NODEVICE = -3            /* no sm_100 device: there is NO CPU fallback */
+    WB_ERR_NODEVICE = -3            /* no sm_90 device: there is NO CPU fallback */
 };
 
 const char* wb_last_error(void);

@@ -1,4 +1,4 @@
-"""wisp_b200 -- Blackwell (sm_100a) volumetric render path behind the kaolin-wisp API.
+"""wisp_b200 -- Hopper (sm_90a) volumetric render path behind the kaolin-wisp API.
 
 Import as `wisp_b200` (the directory is named kaolin-wisp_b200 per the repo layout; the top-level `wisp_b200`
 package aliases it).  Host-side classes mirror the reference's names and arguments; all compute goes through

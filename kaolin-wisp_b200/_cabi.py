@@ -2,7 +2,7 @@
 
 The C ABI (include/wispb200.h) takes raw device pointers, sizes and a cudaStream_t; PyTorch is used here only
 as the owner of device memory and streams.  There is NO CPU or eager fallback: if the library is missing, or
-the device is not sm_100, every compute entry point raises.
+the device is not sm_90, every compute entry point raises.
 """
 from __future__ import annotations
 
@@ -97,7 +97,7 @@ def lib() -> C.CDLL:
     global _lib
     if _lib is None:
         global LIB_PATH
-        LIB_PATH = os.environ.get("WISPB200_LIB", LIB_PATH)          # debug builds (tools/tc_timing.py) live beside the product library
+        LIB_PATH = os.environ.get("WISPB200_LIB", LIB_PATH)          # debug builds (build.py with WB_LIB_NAME) live beside the product library
         if not os.path.exists(LIB_PATH):
             raise WispB200Error(
                 f"{LIB_PATH} not found: build it with `python kaolin-wisp_b200/build.py` (or __graft_entry__.build()). "
@@ -122,9 +122,9 @@ def check(rc: int) -> None:
 
 
 def require_device(t: torch.Tensor) -> None:
-    """Every compute call requires a CUDA tensor on an sm_100 device."""
+    """Every compute call requires a CUDA tensor on an sm_90 device."""
     if not t.is_cuda:
-        raise WispB200Error("wisp_b200 kernels need CUDA tensors on a B200 (sm_100a); there is no CPU fallback")
+        raise WispB200Error("wisp_b200 kernels need CUDA tensors on an H100 (sm_90a); there is no CPU fallback")
     idx = t.device.index if t.device.index is not None else torch.cuda.current_device()
     if idx != torch.cuda.current_device():
         raise WispB200Error(f"tensor on cuda:{idx} but the current device is cuda:{torch.cuda.current_device()}: call under torch.cuda.device({idx}) "

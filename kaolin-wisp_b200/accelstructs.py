@@ -1,5 +1,5 @@
 """OctreeAS: host-side mirror of wisp.accelstructs.OctreeAS (wisp/accelstructs/octree_as.py:37-440) whose
-query / raymarch run on the sm_100a kernels behind the C ABI.  Result holders mirror base_as.py:18-84."""
+query / raymarch run on the sm_90a kernels behind the C ABI.  Result holders mirror base_as.py:18-84."""
 from __future__ import annotations
 
 from dataclasses import dataclass

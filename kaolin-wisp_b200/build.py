@@ -1,9 +1,9 @@
-"""Build libwispb200.so (hand-written sm_100a CUDA behind a C ABI) in-tree with nvcc.
+"""Build libwispb200.so (hand-written sm_90a CUDA behind a C ABI) in-tree with nvcc.
 
     python kaolin-wisp_b200/build.py [--force]
 
-The library lands in kaolin-wisp_b200/lib/ (git-ignored, shipped to the GPU box by gpurun).
-nvcc cross-compiles sm_100a without a GPU, so this also runs in the CPU-only build container.
+The library lands in kaolin-wisp_b200/lib/ (git-ignored build output).
+nvcc cross-compiles sm_90a without a GPU, so this also runs on a machine without one.
 """
 from __future__ import annotations
 
@@ -17,9 +17,9 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, os.environ.get("WB_LIB_NAME", "libwispb200.so"))      # WB_LIB_NAME + WB_EXTRA_NVCC_FLAGS: debug variants
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
-FLAGS += os.environ.get("WB_EXTRA_NVCC_FLAGS", "").split()          # debug builds only (e.g. -DWB_TC_TIMING)
+FLAGS += os.environ.get("WB_EXTRA_NVCC_FLAGS", "").split()          # debug builds only
 
 
 def sources():

@@ -1,4 +1,4 @@
-// wb_common.cuh -- shared device/host helpers of libwispb200 (sm_100a only).
+// wb_common.cuh -- shared device/host helpers of libwispb200 (sm_90a only).
 //
 // Numerical contracts (bit-exact parts) are stated once here and mirrored by the CPU oracle
 // (oracle/wisp_oracle.c).  Reference citations are relative to the kaolin-wisp checkout.

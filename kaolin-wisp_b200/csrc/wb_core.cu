@@ -36,7 +36,7 @@ extern "C" int wb_device_check(int device) {
     int major = 0, minor = 0;
     WB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
     WB_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
-    if (major != 10) { wb_set_error("wb_device_check: device %d is sm_%d%d; libwispb200 is built for sm_100a only", device, major, minor); return WB_ERR_NODEVICE; }
+    if (major != 9 || minor != 0) { wb_set_error("wb_device_check: device %d is sm_%d%d; libwispb200 is built for sm_90a only", device, major, minor); return WB_ERR_NODEVICE; }
     return WB_OK;
 }
 

@@ -1,4 +1,4 @@
-// wb_raymarch.cu -- OctreeAS._raymarch_ray (wisp/accelstructs/octree_as.py:247-309) on sm_100a.
+// wb_raymarch.cu -- OctreeAS._raymarch_ray (wisp/accelstructs/octree_as.py:247-309) on sm_90a.
 //
 // The reference materialises all R*n candidates ([R,n,3] fp32), queries the octree for each, runs
 // torch.nonzero (host sync + compaction) and four fancy-index gathers.  Here one warp owns one ray:

@@ -1,26 +1,26 @@
-// wb_shade_tc.cu -- fused "shade" stage with tensor-core decoders (precision 1): tcgen05.mma + TMEM + TMA-staged weights.
+// wb_shade_tc.cu -- fused "shade" stage with tensor-core decoders (precision 1): wgmma + TMA-staged weights (sm_90a).
 //
 // Numerics = the reference under torch.cuda.amp.autocast (nerf_hash.yaml:76 enable_amp: True): decoder operands in
 // fp16, fp32 accumulation; unlike the reference the hash table is read as fp32 master (no per-call .half() copy,
 // ops/grid.py:88-89), features are blended in fp32 and table gradients accumulate in fp32.
 //
-// Unit of work = a 128-sample sub-tile handled by a GROUP of 256 threads: row r of the tile == TMEM lane r is shared by two
-// threads (column halves).  Per layer ("round", tc_round):  every thread writes its part of the fp16 operand tile (slab layout,
-// wb_tc.cuh) -> fence -> group barrier -> two elected issuer threads launch the round's UMMA chains from a shared-memory issue
-// table (A = sample tile, B = TMA-staged weight pack, D in TMEM; the bias is an init UMMA Ones x Bias^T) and commit to the
-// group's mbarrier -> the group waits, tcgen05.ld's its accumulator columns, applies the activation, writes the next tile.
-// Groups are independent (own named barrier, own mbarrier, own TMEM columns): the forward runs 3 one-group CTAs per SM, the
-// backward one two-group CTA per SM.
+// Unit of work = a 64-sample sub-tile handled by a GROUP of 128 threads = one warpgroup: row r of the tile is shared by two
+// threads (column halves) for the per-sample work, and the warpgroup issues the layer's wgmma chain (A = sample tile, B = the
+// TMA-staged weight pack, D[64 x N] in registers, initialised with the fp16 bias).  Per layer: every thread writes its part of
+// the fp16 operand tile (slab layout, wb_tc.cuh) -> proxy fence -> group barrier -> wgmma chain -> wait -> group barrier ->
+// epilogue straight from the accumulator fragments (relu -> next tile, relu' mask -> next dY, dL/dfeat -> planes) or, where a
+// row needs its whole output (density / colour heads), through a small fp32 scratch tile.  Groups are independent (own named
+// barrier, own tiles): the forward runs TC_FWD_GROUPS groups per CTA and several CTAs per SM, the backward one CTA per SM.
 //
 // Forward  (wb_shade_fwd_tc_kernel): gather 15 LODs x 8 corners (fp32 blend) -> decoders -> (r,g,b,sigma).  It also saves
 //   the gathered feature rows (fp16, chunk-major [Kp0/8][S] x 16 B: coalesced both ways) for the backward.
 // Backward (wb_mlp_bwd_tc_kernel): reloads those rows -- it touches neither the hash table nor the octree -- recomputes the
-//   decoders (tiles stay in shared memory) and per layer issues
-//     weight grad   acc_l[in, out] += X_l^T . dY_l   (both operands MN-major straight from the sample tiles; accumulators
-//                                                     stay in TMEM for the whole kernel; a constant-one slab behind every
-//                                                     X_l tile makes row `Kp_l` the bias gradient)
-//     data grad     dX_l = dY_l . W_l                (weight pack read MN-major: no transposed copy)
-//   and writes dL/dfeat as fp16 level-major planes [L][S][F].
+//   decoders (all activation tiles stay in shared memory) and per layer issues
+//     weight grad   acc_l^T[out, in | 1] += dY_l^T . [X_l | 1]  (both operands MN-major straight from the sample tiles; a
+//                                                               constant-one slab behind every X_l tile gives the bias gradient;
+//                                                               fp32 accumulators in shared memory, one private copy per group)
+//     data grad     dX_l = dY_l . W_l                           (weight pack read MN-major: no transposed copy)
+//   and writes dL/dfeat as fp16 level-major planes [L][S][F], or scatters it into the hash table in its last epilogue.
 // Scatter  (wb_table_scatter_kernel, SIMT): lanes = consecutive samples; a thread builds its sample position once and walks all
 //   LODs; per LOD, runs of lanes that fall into the same cell are summed with a segmented warp scan and only the last lane of a
 //   run issues the reductions (x-neighbour entries that differ only in bit 0 as one 16-byte red.global.add.v4.f32).
@@ -34,91 +34,61 @@
 #include <math.h>
 
 #define TC_ML 16
-constexpr int TC_ROWS = 128;          // samples per sub-tile (UMMA M)
-constexpr int TC_GROUP = 256;         // threads per sub-tile group: 128 rows x 2 column halves
-constexpr int TC_BWD_GROUPS = 2;      // sub-tile groups per CTA in the decoder backward
-constexpr int TC_ISSUERS = 2;         // issuer warps per group (backward: weight grad | data grad)
+constexpr int TC_ROWS = 64;                 // samples per sub-tile (wgmma M)
+constexpr int TC_GROUP = 128;               // threads per sub-tile group: one warpgroup, 64 rows x 2 column halves
+constexpr int TC_SLAB = TC_ROWS * 16;       // bytes of one slab (8 features of every sample of the tile)
+constexpr int TC_FWD_GROUPS = 2;            // sub-tile groups per forward CTA (they share the staged weights)
+constexpr int TC_SCR_LD = 33;               // fp32 scratch tile [64][33]: the <= 32 columns an epilogue needs row by row
+constexpr int TC_SCR_BYTES = (TC_ROWS * TC_SCR_LD * 4 + 15) / 16 * 16;
+constexpr int TC_SMEM_MAX = 227 * 1024 - 1024;      // dynamic shared memory per CTA (H100: 227 KB, minus the static barriers)
 
 struct WbTc {
     int nl_d, nl_c;
     int I[TC_ML], O[TC_ML], Kp[TC_ML], Np[TC_ML];
     int w_off[TC_ML], b_off[TC_ML];            // byte offsets in the parameter blob: weight pack, bias pack [Np x 16] (bias at k = 0)
     int has_bias;
-    int ones_off;                              // byte offset (from smem base) of the constant [128 x 16] tile (feature 0 = 1) of the bias UMMA
     int src_w[TC_ML], src_b[TC_ML];
     int blob_bytes;
-    int tile_off[TC_ML];                       // byte offset of layer l's INPUT tile inside a sub-tile region
-    int dy_off[2];                             // byte offset (from smem base) of the dY tile of sub-tile 0/1
-    int sub_off[2];                            // byte offset of the sub-tile regions
-    int w_smem_off;                            // byte offset of the staged parameter blob
+    int maxw;
+    int tile_off[TC_ML];                       // byte offset of layer l's INPUT tile inside a group region
+    int dy_off, scr_off, acc_off;              // byte offsets inside a group region: dY tile, fp32 scratch, weight-grad accumulators
+    int acc_l[TC_ML];                          // float offset of layer l's accumulator [O][I + 1] (column I = bias), -1: not in this pass
+    int group_bytes;                           // stride of the group regions
+    int groups;                                // sub-tile groups per CTA
+    int w_smem_off;                            // byte offset of the staged parameter blob (behind the group regions)
     int smem_bytes;
-    int acc_col[TC_ML];                        // TMEM column of the weight-grad accumulator of layer l
-    int work_col[2];                           // TMEM working accumulator of sub-tile 0/1
-    int tmem_cols;
     int feat_dim, pos_dim, view_dim, pos_mode, pos_freq, view_mode, view_freq;
-    int fits2;                                 // backward: the two-group kernel (all tiles retained) fits in shared memory
 };
 
 static int tc_round_up(int v, int m) { return (v + m - 1) / m * m; }
-
-// ---- three-group decoder backward (wb_shade_tc_bwd3.cuh): shared-memory plan ----
-constexpr int TC_B3_GROUPS = 3;
-struct TcB3Plan {
-    int P, Q, R, E, GB, blob_off, ones_off, smem_bytes;          // byte offsets (P..E from the group base, GB = group stride)
-    int groups;                                                   // 3: every width <= 64;  1: widths up to 128 (hidden_dim = 128)
-    int kind[8], acc_col[8], bias_col[8];                         // weight-grad accumulator of layer l: orientation (see below) and TMEM columns
-    int acc_begin, acc_end;                                       // TMEM column range of all accumulators (zeroed at kernel start)
-};
-
-// host: shared-memory + tensor-memory plan; returns false when the configuration is outside the kernel's scope.
-// Accumulator kinds (one group, 128-wide layers: 416 accumulator columns in the [in, out] orientation + 128 working columns would not
-// fit the 512 TMEM columns, and a 128-row X^T leaves no row for the bias gradient):
-//   0  acc[in, out] += X^T . dY, the tile's constant-one slab makes row Kp the bias gradient             (Np columns;  Kp < 128)
-//   1  the same, bias gradient in a 16-column accumulator of its own: bias[out, 0] += dY^T . Ones         (Np + 16;     Kp == 128)
-//   2  acc^T[out, in | 1] += dY^T . [X | 1]                                                              (Kp + 16;     used when Kp + 16 < Np)
-// hidden_dim 128 on the app/nerf field: 48 + 32 + 64 + 144 + 32 = 320 accumulator columns + 128 working columns.
-static bool tc_b3_plan(const WbTc& m, TcB3Plan* p)
-{
-    if (m.nl_d != 2 || m.nl_c != 3) return false;
-    int maxw = 0, sumN = 0;
-    for (int l = 0; l < 5; ++l) { maxw = max(maxw, max(m.Kp[l], m.Np[l])); sumN += m.Np[l]; }
-    if (maxw > 128) return false;
-    if (maxw > 64 && maxw != 128) return false;      // the one-group layout has been validated on B200 for 128-wide decoders only (hidden_dim 128);
-                                                     // widths in between keep training on the fp32 kernels, as before
-    // the hidden activation tiles X1, X3, X4 share the buffers P and Q, whose constant-one slab sits behind a maxw-wide tile: the
-    // hidden width must BE the widest tile (true for app/nerf: 64-wide hidden layers over 32 / 42 inputs; a 32-wide decoder over a
-    // 42-wide colour input would read its bias-gradient row from a stale slab)
-    if (m.Kp[1] != maxw || m.Kp[3] != maxw || m.Kp[4] != maxw || m.Np[0] != maxw || m.Np[2] != maxw || m.Np[3] != maxw) return false;
-    memset(p, 0, sizeof(*p));
-    p->groups = (maxw <= 64 && sumN <= 512 - 3 * 64) ? 3 : 1;    // TMEM: 64 working columns per group (3 groups) / 128 (1 group) + the accumulators
-    const int wc = p->groups == 3 ? 64 : 128;
-    int col = p->groups * wc;
-    p->acc_begin = col;
-    for (int l = 0; l < 5; ++l) {
-        p->kind[l] = p->groups == 3 ? 0 : (m.Kp[l] + 16 < m.Np[l] ? 2 : (m.Kp[l] >= 128 ? 1 : 0));
-        p->acc_col[l] = col; col += p->kind[l] == 2 ? m.Kp[l] + 16 : m.Np[l];
-        p->bias_col[l] = col; if (p->kind[l] == 1) col += 16;
-    }
-    p->acc_end = col;
-    if (col > 512) return false;
-    const int big = (maxw / 8 + 1) * 2048;                       // a maxw-wide tile + its constant-one slab
-    const int small = (max(m.Np[1], m.Np[4]) / 8) * 2048;        // dY1 / dY4
-    p->P = 0; p->Q = big; p->R = 2 * big; p->E = 3 * big; p->GB = 3 * big + small;
-    p->blob_off = p->groups * p->GB;
-    p->ones_off = p->blob_off + m.blob_bytes;
-    int end = p->ones_off + 2 * 2048;
-    // 16-slab read windows of the MN-major A operands (M = 128 feature rows): X tiles in R, and (kinds 1, 2) dY tiles in E
-    const int window = (p->groups - 1) * p->GB + (p->groups == 3 ? p->R : p->E) + 16 * 2048;
-    if (end < window) end = window;
-    p->smem_bytes = end + 64;
-    return p->smem_bytes + 6144 <= 227 * 1024;
-}
-
-
 static int tc_embed_dim(int mode, int freq) { return mode == 0 ? 0 : mode == 1 ? 3 : mode == 2 ? 6 * freq : 3 + 6 * freq; }
 
+// backward shared-memory plan for `groups` groups that accumulate the weight gradients of the layers in `wmask`;
+// returns false when it does not fit
+static bool tc_bwd_layout(WbTc* m, unsigned wmask, int groups)
+{
+    const int nl = m->nl_d + m->nl_c;
+    int off = 0;
+    for (int l = 0; l < nl; ++l) { m->tile_off[l] = off; off += (m->Kp[l] / 8 + 1) * TC_SLAB; }     // + constant-one slab
+    // the weight-grad A operand (dY^T, M = 64 output features) reads 8 slabs even when the layer is narrower
+    m->dy_off = off; off += (max(m->maxw, 64) / 8) * TC_SLAB;
+    m->scr_off = off; off += TC_SCR_BYTES;
+    m->acc_off = off;
+    int acc = 0;
+    for (int l = 0; l < nl; ++l) {
+        m->acc_l[l] = -1;
+        if ((wmask >> l) & 1u) { m->acc_l[l] = acc; acc += m->O[l] * (m->I[l] + 1); }
+    }
+    off += tc_round_up(acc * 4, 16);
+    m->group_bytes = off;
+    m->groups = groups;
+    m->w_smem_off = groups * off;
+    m->smem_bytes = m->w_smem_off + m->blob_bytes;
+    return m->smem_bytes <= TC_SMEM_MAX;
+}
+
 // returns WB_OK, or WB_ERR_INVALID with a message when the configuration does not fit the tensor-core path
-int wb_tc_make(const wb_nef_desc* d, bool backward, WbTc* m, bool tmem_a = false)
+int wb_tc_make(const wb_nef_desc* d, bool backward, WbTc* m)
 {
     WB_CHECK_ARG(d->dens_layers >= 1 && d->col_layers >= 1 && d->dens_layers + d->col_layers <= TC_ML, "unsupported decoder depth");
     WB_CHECK_ARG(d->dens_params && d->col_params, "null decoder parameters");
@@ -149,45 +119,26 @@ int wb_tc_make(const wb_nef_desc* d, bool backward, WbTc* m, bool tmem_a = false
     }
     m->blob_bytes = tc_round_up(off, 16);
     m->has_bias = d->has_bias ? 1 : 0;
-    // shared memory map: [sub0 tiles][sub1 tiles][dY0][dY1][params][pad]
-    int sub_bytes = 0;
-    if (backward) {
-        for (int l = 0; l < nl; ++l) { m->tile_off[l] = sub_bytes; sub_bytes += (m->Kp[l] / 8 + 1) * 2048; }   // + constant-one slab
-    } else {
-        // forward: every layer's input tile is overwritten in place by its output (the layer's UMMAs have completed before the
-        // epilogue writes, and each thread only touches its own row) -> 16 KB per sub-tile, 4 CTAs per SM for the gather
+    m->maxw = maxw;
+    if (!backward) {
+        // every layer's input tile is overwritten in place by its output (the layer's MMAs have completed before the epilogue writes)
         for (int l = 0; l < nl; ++l) m->tile_off[l] = 0;
-        sub_bytes = (maxw / 8) * 2048;
+        m->scr_off = (maxw / 8) * TC_SLAB;
+        m->group_bytes = m->scr_off + TC_SCR_BYTES;
+        m->groups = TC_FWD_GROUPS;
+        m->w_smem_off = m->groups * m->group_bytes;
+        m->smem_bytes = m->w_smem_off + m->blob_bytes;
+        WB_CHECK_ARG(m->smem_bytes <= TC_SMEM_MAX, "tensor-core path: decoder does not fit in shared memory (use precision 0)");
+        return WB_OK;
     }
-    const int groups = backward ? TC_BWD_GROUPS : 1;             // sub-tile groups per CTA
-    m->sub_off[0] = 0; m->sub_off[1] = sub_bytes;
-    int p = groups * sub_bytes;
-    if (backward) { m->dy_off[0] = p; p += (maxw / 8) * 2048; m->dy_off[1] = p; p += (maxw / 8) * 2048; }
-    m->w_smem_off = p; p += m->blob_bytes;
-    m->ones_off = p; p += 2 * 2048;
-    if (backward) {   // weight-grad MMAs read 16 slabs (M = 128 feature rows) from every X tile: keep that window inside the allocation
-        const int need = m->sub_off[groups - 1] + m->tile_off[nl - 1] + 16 * 2048;
-        if (p < need) p = need;
-    }
-    m->smem_bytes = p + 64;
-    // static shared memory of the kernels (issue table, barriers): 3 KB forward, 5 KB backward
-    const bool smem2 = m->smem_bytes + (backward ? 5632 : 3584) <= 227 * 1024;
-    int col = 0;
-    for (int gi = 0; gi < groups; ++gi) { m->work_col[gi] = col; col += maxw; }
-    // forward TMEM-A variant (one group): work_col[1] is otherwise unused and holds the first column of the fp16 activation tile
-    if (tmem_a && !backward) { m->work_col[1] = col; col += maxw / 2; }  // two halfs per 32-bit column
-    if (backward) for (int l = 0; l < nl; ++l) { m->acc_col[l] = col; col += m->Np[l]; }
-    m->fits2 = (smem2 && col <= 512) ? 1 : 0;
-    if (!m->fits2) {       // the two-group backward retains every activation tile and keeps all accumulators [in, out]; the kernel of
-        TcB3Plan plan3;    // wb_shade_tc_bwd3.cuh (uniform buffers, three groups or one wide group, mixed accumulator orientation) may still fit
-        WB_CHECK_ARG(backward && tc_b3_plan(*m, &plan3),
-                     !smem2 ? (backward ? "tensor-core path: decoder backward does not fit in shared memory (use precision 0)"
-                                        : "tensor-core path: decoder does not fit in shared memory (use precision 0)")
-                            : "tensor-core path: accumulators do not fit in TMEM (use precision 0)");
-        col = 512;
-    }
-    int alloc = 32; while (alloc < col) alloc <<= 1;
-    m->tmem_cols = alloc;
+    // backward: decoders whose whole backward fits two groups per CTA in one pass, and decoders of the app/nerf depth (one hidden
+    // density layer, two hidden colour layers) up to width 128, whose weight gradients may take several passes (every layer's
+    // accumulator must fit beside the tiles of one group); deeper, wider decoders train on the fp32 kernels
+    const bool one_pass = tc_bwd_layout(m, (1u << nl) - 1u, 2);
+    bool passes = m->nl_d <= 2 && m->nl_c <= 3;
+    for (int l = 0; l < nl && passes; ++l) passes = tc_bwd_layout(m, 1u << l, 1);
+    WB_CHECK_ARG(one_pass || passes, "tensor-core path: decoder backward does not fit in shared memory (use precision 0)");
+    tc_bwd_layout(m, (1u << nl) - 1u, 1);       // the plan of the first pass is left in *m
     return WB_OK;
 }
 
@@ -234,9 +185,8 @@ __global__ void wb_tc_pack_kernel(WbTc m, const float* __restrict__ dens, const 
             const int kc = e / (Np * 8), n = (e / 8) % Np, k = kc * 8 + (e & 7);      // element (n,k) at (k/8)*(Np*8) + n*8 + k%8 halves
             w[e] = __float2half_rn((n < O && k < I) ? src[m.src_w[l] + n * I + k] : 0.0f);
         }
-        // bias pack B[Np x 16] (K-major, same layout as the weights): column k = 0 holds the bias.  An init UMMA
-        // D = Ones[128 x 16] . B^T puts the bias into the accumulator; the layer UMMAs accumulate on top (fp16 bias: what
-        // F.linear under autocast does)
+        // bias pack B[Np x 16] (K-major, same layout as the weights): column k = 0 holds the bias.  The accumulator
+        // fragments start from it and the layer's MMAs accumulate on top (fp16 bias: what F.linear under autocast does)
         __half* b = reinterpret_cast<__half*>(blob + m.b_off[l]);
         for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < Np * 16; e += gridDim.x * blockDim.x) {
             const int kc = e / (Np * 8), n = (e / 8) % Np, k = kc * 8 + (e & 7);
@@ -290,8 +240,11 @@ struct TcIn {
     const uint4* ray_embed;      // [R][Kc/8] rows prepared by wb_ray_embed_kernel
     uint4* x0_save;              // forward: optional [Kp0/8][S] copy of the density-decoder input rows
     const uint4* x0_saved;       // backward: the same buffer
-    int64_t s_begin, s_end;      // backward kernels that take a sample range (a multiple of 128 .. s_end; s_end == 0: the whole [0, S)); S stays the plane stride
+    int64_t s_begin, s_end;      // backward kernels that take a sample range (a multiple of 64 .. s_end; s_end == 0: the whole [0, S)); S stays the plane stride
 };
+
+// byte offset of (sample s, feature f) in a slab tile
+__device__ __forceinline__ uint32_t tc_slab_off(int s, int f) { return (uint32_t)((f >> 3) * TC_SLAB + s * 16 + (f & 7) * 2); }
 
 __device__ __forceinline__ void tile_store1(uint8_t* tile, int r, int f, float v)
 {
@@ -300,7 +253,7 @@ __device__ __forceinline__ void tile_store1(uint8_t* tile, int r, int f, float v
 __device__ __forceinline__ void tile_store8(uint8_t* tile, int r, int slab, const float v[8])
 {
     uint4 q; q.x = tc_pack2(v[0], v[1]); q.y = tc_pack2(v[2], v[3]); q.z = tc_pack2(v[4], v[5]); q.w = tc_pack2(v[6], v[7]);
-    *reinterpret_cast<uint4*>(tile + slab * 2048 + r * 16) = q;
+    *reinterpret_cast<uint4*>(tile + slab * TC_SLAB + r * 16) = q;
 }
 // embedding (positional_embedder.py:51-66) written into tile features [f0, f0+dim)
 __device__ __forceinline__ void tile_embed(uint8_t* tile, int r, int f0, int mode, int freq, float x, float y, float z)
@@ -381,186 +334,116 @@ __device__ __forceinline__ void tile_gather(const WbGrid& g, uint8_t* tile, int 
 // zero features [f0, f1) of this thread's row
 __device__ __forceinline__ void tile_zero(uint8_t* tile, int r, int f0, int f1) { for (int f = f0; f < f1; ++f) tile_store1(tile, r, f, 0.0f); }
 
-// ---- optional phase timestamps (debug builds only: WB_EXTRA_NVCC_FLAGS=-DWB_TC_TIMING, read by tools/tc_timing.py) ----
-#ifdef WB_TC_TIMING
-#define TC_TS_N 1024
-__device__ long long g_tc_ts[2][2][TC_TS_N];      // [kernel: 0 fwd, 1 bwd][thread 0 / (fwd: last thread, bwd: first thread of group 1)][event]
-#define TC_TS(c) do { if (blockIdx.x == 0 && (threadIdx.x == 0 || threadIdx.x == ((c).tsk ? TC_GROUP : TC_GROUP - 1)) && (c).tsn < TC_TS_N) \
-        g_tc_ts[(c).tsk][threadIdx.x ? 1 : 0][(c).tsn++] = clock64(); } while (0)
-__device__ long long g_tc_ts2[2][TC_TS_N];        // thread 0 only: inside the issue branch (after elect+fence, after the UMMAs, after commit)
-#define TC_TS2(c, n2) do { if (blockIdx.x == 0 && threadIdx.x == 0 && (n2) < TC_TS_N) g_tc_ts2[(c).tsk][(n2)++] = clock64(); } while (0)
-extern "C" int wb_tc_timing_dump2(long long* out)
-{ return (int)cudaMemcpyFromSymbol(out, g_tc_ts2, sizeof(long long) * 2 * TC_TS_N); }
-__device__ long long g_tc_ts3[2][TC_TS_N];        // thread 0 only: hidden-layer epilogue (before tcgen05.ld, after its wait, after the stores)
-#define TC_TS3(c) do { if (blockIdx.x == 0 && threadIdx.x == 0 && (c).tsn3 < TC_TS_N) g_tc_ts3[(c).tsk][(c).tsn3++] = clock64(); } while (0)
-extern "C" int wb_tc_timing_dump3(long long* out)
-{ return (int)cudaMemcpyFromSymbol(out, g_tc_ts3, sizeof(long long) * 2 * TC_TS_N); }
-__device__ long long g_tc_ts4[2][64][16];        // thread 0: stamp before the chain and after every UMMA of the first 64 rounds
-__device__ int g_tc_ts4_round[2];
-extern "C" int wb_tc_timing_dump4(long long* out)
-{ return (int)cudaMemcpyFromSymbol(out, g_tc_ts4, sizeof(long long) * 2 * 64 * 16); }
-extern "C" int wb_tc_timing_dump(long long* out)
-{ return (int)cudaMemcpyFromSymbol(out, g_tc_ts, sizeof(long long) * 2 * 2 * TC_TS_N); }
-#else
-#define TC_TS(c) do { } while (0)
-#define TC_TS2(c, n2) do { } while (0)
-#define TC_TS3(c) do { } while (0)
-#endif
-
-// Issue table (shared memory, built once per CTA): everything the issuer needs for one UMMA chain, so that the critical path
-// after the group barrier is two LDS.128 (issued BEFORE the barrier) + the UTCHMMAs.  Deriving the descriptors from the
-// kernel parameters instead costs ~400 cycles of dependent constant loads / uniform ALU per round (measured).
-struct __align__(16) TcRec {
-    uint32_t a_lo, a_hi, b_lo, b_hi;          // shared-memory descriptors of the first UMMA
-    uint32_t idesc, tmem_d, nk_acc, adv;      // nk | (accumulate-from-start << 8); a advance | b advance << 16 (16-byte units)
-};
-enum { TC_K_FWD = 0, TC_K_BIAS = 1, TC_K_WGRAD = 2, TC_K_DGRAD = 3, TC_KINDS = 4,
-       TC_K_FWD_TA = TC_K_WGRAD };           // forward kernels have no weight grad: the slot holds the A-from-TMEM chain of the TMEM-A variant
-
+// ---------------------------------------------------------------------------------------------------------------
+// wgmma chains of one group
+// ---------------------------------------------------------------------------------------------------------------
 struct TcCtx {
-    uint8_t* smem; uint64_t* bar; uint32_t tmem; uint32_t phase;
-    const TcRec* tab;           // this group's records: tab[kind * TC_ML + layer]
-    int g;                      // sub-tile group of this thread inside the CTA
-    int r, h;                   // row of the sub-tile (== TMEM lane), column half
-    int laneq;                  // 32*(warp%4): the TMEM lane quarter this warp may access
-    int wig;                    // warp index inside the group (warp-uniform)
-#ifdef WB_TC_TIMING
-    int tsn, tsk, tsn2, tsn3;
-#endif
+    uint8_t* sub;               // this group's region (tiles, scratch, accumulators)
+    const uint8_t* blob;        // staged parameter blob (shared by the CTA's groups)
+    float* scr;                 // fp32 scratch tile [TC_ROWS][TC_SCR_LD]
+    int g;                      // sub-tile group of this thread inside the CTA; named barrier g + 1
+    int r, h;                   // row of the sub-tile, column half
+    int wl;                     // thread index inside the warpgroup (accumulator fragment owner)
 };
-__device__ __forceinline__ void tc_ctx_init(TcCtx& c, uint8_t* smem, uint64_t* bars, const TcRec* tab, uint32_t tmem, int kernel_id)
+__device__ __forceinline__ void tc_ctx_init(TcCtx& c, const WbTc& m, uint8_t* smem)
 {
     const int tig = threadIdx.x & (TC_GROUP - 1);
-    c.smem = smem; c.g = threadIdx.x / TC_GROUP; c.bar = bars + c.g; c.tmem = tmem; c.phase = 0;
-    c.tab = tab + c.g * (TC_KINDS * TC_ML);
-    c.r = tig & (TC_ROWS - 1); c.h = tig / TC_ROWS; c.laneq = ((tig >> 5) & 3) * 32;
-    c.wig = __shfl_sync(0xffffffffu, tig >> 5, 0);
-#ifdef WB_TC_TIMING
-    c.tsn = 0; c.tsk = kernel_id; c.tsn2 = 0; c.tsn3 = 0;
-#endif
+    c.g = threadIdx.x / TC_GROUP;
+    c.sub = smem + c.g * m.group_bytes; c.blob = smem + m.w_smem_off;
+    c.scr = reinterpret_cast<float*>(c.sub + m.scr_off);
+    c.r = tig & (TC_ROWS - 1); c.h = tig / TC_ROWS; c.wl = tig;
+}
+__device__ __forceinline__ void tc_sync(const TcCtx& c) { tc_group_sync(c.g + 1, TC_GROUP); }
+// operand tiles written by the group's threads -> visible to the tensor cores of the whole group
+__device__ __forceinline__ void tc_publish(const TcCtx& c) { tc_fence_smem_async(); tc_sync(c); }
+
+// One MMA chain of the group: D[64 x N] = bias (fp16, bias pack: entry n at half index 8n) or 0, then += A . B over nk K-steps of
+// 16; wait; group barrier (every MMA of the group has read its operands: the epilogue may overwrite them); epi(d) on the fragments.
+template <int N, int TA, int TB, class Epi>
+__device__ __forceinline__ void tc_chain(const TcCtx& c, uint64_t da, uint64_t db, int nk, uint32_t aadv, uint32_t badv,
+                                         const __half* bias, Epi&& epi)
+{
+    float d[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) d[i] = bias ? __half2float(bias[tc_frag_col(c.wl, i) * 8]) : 0.0f;
+    tc_wg_fence();
+    for (int kb = 0; kb < nk; ++kb) { WgMma<N, TA, TB>::run(d, da, db, 1u); da += aadv; db += badv; }
+    tc_wg_commit();
+    tc_wg_wait0();
+    tc_wg_hold(d);
+    tc_sync(c);
+    epi(d);
+}
+// the same with N chosen at run time (a multiple of 16, at most NMAX <= 128: the widest padded layer the kernel was built for; a
+// 128-wide accumulator alone needs 64 registers per thread)
+template <int TA, int TB, int NMAX = 128, class Epi>
+__device__ __forceinline__ void tc_chain_n(const TcCtx& c, int N, uint64_t da, uint64_t db, int nk, uint32_t aadv, uint32_t badv,
+                                           const __half* bias, Epi&& epi)
+{
+    switch (N) {
+        case 16: tc_chain<16, TA, TB>(c, da, db, nk, aadv, badv, bias, epi); break;
+        case 32: tc_chain<32, TA, TB>(c, da, db, nk, aadv, badv, bias, epi); break;
+        case 48: tc_chain<48, TA, TB>(c, da, db, nk, aadv, badv, bias, epi); break;
+        case 64: tc_chain<64, TA, TB>(c, da, db, nk, aadv, badv, bias, epi); break;
+        case 80: tc_chain<(80 <= NMAX ? 80 : NMAX), TA, TB>(c, da, db, nk, aadv, badv, bias, epi); break;
+        case 96: tc_chain<(96 <= NMAX ? 96 : NMAX), TA, TB>(c, da, db, nk, aadv, badv, bias, epi); break;
+        case 112: tc_chain<(112 <= NMAX ? 112 : NMAX), TA, TB>(c, da, db, nk, aadv, badv, bias, epi); break;
+        default: tc_chain<NMAX, TA, TB>(c, da, db, nk, aadv, badv, bias, epi); break;
+    }
+}
+// fragments -> fp32 scratch tile, columns [0, ncols); the caller synchronises the group before reading rows
+#define TC_FRAG_TO_SCRATCH(c, d, ncols)                                                                          \
+    do {                                                                                                         \
+        constexpr int NR_ = sizeof(d) / sizeof(float);                                                          \
+        _Pragma("unroll") for (int i = 0; i < NR_; ++i) {                                                        \
+            const int col = tc_frag_col((c).wl, i);                                                              \
+            if (col < (ncols)) (c).scr[tc_frag_row((c).wl, i) * TC_SCR_LD + col] = d[i];                          \
+        }                                                                                                        \
+    } while (0)
+
+// forward layer l: D = bias + X_l . W_l^T   (A: input tile K-major, B: weight pack K-major)
+template <int NMAX, class Epi>
+__device__ __forceinline__ void tc_fwd_layer(const WbTc& m, const TcCtx& c, int l, int N, Epi&& epi)
+{
+    const uint32_t sb = tc_smem_u32(c.sub + m.tile_off[l]), wb = tc_smem_u32(c.blob);
+    const int Np = m.Np[l];
+    tc_chain_n<0, 0, NMAX>(c, N, tc_desc(sb, TC_SLAB, 128), tc_desc(wb + m.w_off[l], Np * 16, 128), m.Kp[l] / 16, (2 * TC_SLAB) >> 4,
+                     (2 * Np * 16) >> 4, m.has_bias ? reinterpret_cast<const __half*>(c.blob + m.b_off[l]) : nullptr, epi);
 }
 
-// one record per (group, kind, layer) + the constant tile of the bias UMMA; called by all threads before the first round
-__device__ __forceinline__ void tc_build_table(const WbTc& m, TcRec* tab, uint8_t* smem, uint32_t tmem, int groups, bool backward, bool ta = false)
+// Decoders of one 64-sample sub-tile, starting from an X0 tile that the group has already written.
+// Returns (per row, both column halves) the density-decoder output df[16] and the colour pre-activations c3[3].
+template <int NMAX>
+__device__ __forceinline__ void tc_decoders(const WbTc& m, const TcCtx& c, const TcIn& in, int64_t ray, float df[16], float c3[3])
 {
     const int nl = m.nl_d + m.nl_c;
-    const int e = threadIdx.x;
-    if (e < TC_ROWS) {                                           // Ones[128 x 16]: feature 0 = 1, features 1..15 = 0
-        uint4 one; one.x = 0x00003C00u; one.y = 0; one.z = 0; one.w = 0;
-        *reinterpret_cast<uint4*>(smem + m.ones_off + e * 16) = one;
-        *reinterpret_cast<uint4*>(smem + m.ones_off + 2048 + e * 16) = make_uint4(0, 0, 0, 0);
-    }
-    if (e >= groups * TC_KINDS * nl) return;
-    const int l = e % nl, kind = (e / nl) % TC_KINDS, g = e / (nl * TC_KINDS);
-    const uint32_t base = tc_smem_u32(smem);
-    const int Np = m.Np[l], Kp = m.Kp[l];
-    uint64_t da = 0, db = 0; uint32_t id = 0, d = 0, nk = 0, acc = 0, aadv = 0, badv = 0;
-    if (kind == TC_K_FWD) {            // D_work[g] (+)= X_l . W_l^T
-        da = tc_desc(base + m.sub_off[g] + m.tile_off[l], 2048, 128); db = tc_desc(base + m.w_smem_off + m.w_off[l], Np * 16, 128);
-        id = tc_idesc(128, Np, 0, 0); d = tmem + m.work_col[g]; nk = Kp / 16; acc = m.has_bias; aadv = 4096 >> 4; badv = (2 * Np * 16) >> 4;
-    } else if (kind == TC_K_BIAS) {    // D_work[g] = Ones . Bias_l^T
-        da = tc_desc(base + m.ones_off, 2048, 128); db = tc_desc(base + m.w_smem_off + m.b_off[l], Np * 16, 128);
-        id = tc_idesc(128, Np, 0, 0); d = tmem + m.work_col[g]; nk = m.has_bias ? 1 : 0;
-    } else if (!backward && kind == TC_K_FWD_TA && ta) {   // D_work (+)= X_l[TMEM] . W_l^T ; a_lo = TMEM address, 8 columns per K step
-        da = (uint64_t)(tmem + (uint32_t)m.work_col[1]); db = tc_desc(base + m.w_smem_off + m.w_off[l], Np * 16, 128);
-        id = tc_idesc(128, Np, 0, 0); d = tmem + m.work_col[g]; nk = (uint32_t)(Kp / 16); acc = m.has_bias; aadv = 8; badv = (2 * Np * 16) >> 4;
-    } else if (!backward) {
-        nk = 0;
-    } else if (kind == TC_K_WGRAD) {   // acc_l[in, out] += X_l^T . dY_l   (K = 128 samples)
-        da = tc_desc(base + m.sub_off[g] + m.tile_off[l], 128, 2048); db = tc_desc(base + m.dy_off[g], 128, 2048);
-        id = tc_idesc(128, Np, 1, 1); d = tmem + m.acc_col[l]; nk = 8; acc = 1; aadv = 256 >> 4; badv = 256 >> 4;
-    } else {                           // D_work[g] = dY_l . W_l         (K = out features)
-        da = tc_desc(base + m.dy_off[g], 2048, 128); db = tc_desc(base + m.w_smem_off + m.w_off[l], 128, Np * 16);
-        id = tc_idesc(128, Kp, 0, 1); d = tmem + m.work_col[g]; nk = Np / 16; aadv = 4096 >> 4; badv = 256 >> 4;
-    }
-    TcRec r = { (uint32_t)da, (uint32_t)(da >> 32), (uint32_t)db, (uint32_t)(db >> 32), id, d, nk | (acc << 8), aadv | (badv << 16) };
-    tab[(g * TC_KINDS + kind) * TC_ML + l] = r;
-}
-template <bool A_IN_TMEM = false>
-__device__ __forceinline__ void tc_issue_rec(const uint4 q0, const uint4 q1, long long* ts = nullptr, int* tn = nullptr)
-{
-    uint64_t da = ((uint64_t)q0.y << 32) | q0.x, db = ((uint64_t)q0.w << 32) | q0.z;
-    const int nk = (int)(q1.z & 0xffu);
-    const uint32_t acc = q1.z >> 8, aadv = q1.w & 0xffffu, badv = q1.w >> 16;
-    for (int kb = 0; kb < nk; ++kb) {
-        if (A_IN_TMEM) tc_mma_ts(q1.y, (uint32_t)da, db, q1.x, acc | (uint32_t)(kb > 0));
-        else tc_mma(q1.y, da, db, q1.x, acc | (uint32_t)(kb > 0));
-        da += aadv; db += badv;
-#ifdef WB_TC_TIMING
-        if (ts && *tn < 16) ts[(*tn)++] = clock64();
-#endif
-    }
-}
-
-// One round of a sub-tile group: operand tiles written -> group barrier -> the group's two issuer warps launch their UMMA
-// chains (warp 0: kind k0a then k0b; warp 1: k1; a negative kind = nothing) and commit to the group's mbarrier -> the group
-// waits for all of them.
-// Measured on B200 (tools/tc_timing.py), first version of this file: a round cost ~600-1200 cycles from barrier to completion and
-// the epilogue of a 64-wide layer another ~1200; the tensor pipe was ~10 % busy.  What this version does about it:
-//  (a) issue table + elect.sync in a warp-uniform branch (descriptors in uniform registers, UTCHMMAs back to back; the first
-//      version's per-thread branch ran a one-lane waterfall loop of ~200 cycles per UMMA),
-//  (b) weight-grad and data-grad chains issued by two different warps,
-//  (c) bias added by an init UMMA (Ones x Bias^T) and relu fused into the fp32->fp16x2 conversion: the hidden-layer epilogue is
-//      tcgen05.ld + 16 F2FP.RELU + 4 STS.128 instead of ~130 instructions,
-//  (d) a row is shared by two threads (column halves),
-//  (e) the groups of a CTA (backward) / the CTAs of an SM (forward) have independent barriers and overlap each other.
-template <bool TA = false>          // TA: warp 0's second chain (k0b) reads its A operand from tensor memory
-__device__ __forceinline__ void tc_round(TcCtx& c, int l, int k0a, int k0b, int k1)
-{
-    TC_TS(c);
-    uint4 qa0 = make_uint4(0, 0, 0, 0), qa1 = qa0, qb0 = qa0, qb1 = qa0;
-    if (c.wig < TC_ISSUERS) {                     // table reads do not depend on the barrier
-        const int ka = c.wig == 0 ? k0a : k1, kb = c.wig == 0 ? k0b : -1;
-        if (ka >= 0) { const uint4* p = reinterpret_cast<const uint4*>(c.tab + ka * TC_ML + l); qa0 = p[0]; qa1 = p[1]; }
-        if (kb >= 0) { const uint4* p = reinterpret_cast<const uint4*>(c.tab + kb * TC_ML + l); qb0 = p[0]; qb1 = p[1]; }
-    }
-    tc_fence_smem_async();
-    tc_fence_before();
-    tc_group_sync(c.g + 1, TC_GROUP);
-    TC_TS(c);
-    if (c.wig < TC_ISSUERS) {
-        if (tc_elect_one()) {
-            tc_fence_after();
-            TC_TS2(c, c.tsn2);
-#ifdef WB_TC_TIMING
-            long long* ts4 = nullptr; int tn4 = 0;
-            if (blockIdx.x == 0 && threadIdx.x == 0 && c.tsn2 / 3 < 64) { ts4 = g_tc_ts4[c.tsk][c.tsn2 / 3]; ts4[tn4++] = clock64(); }
-            if (((qa1.z | qb1.z) & 0xffu) != 0) { tc_issue_rec(qa0, qa1, ts4, &tn4); tc_issue_rec<TA>(qb0, qb1, ts4, &tn4); TC_TS2(c, c.tsn2); tc_commit(c.bar); }
-#else
-            if (((qa1.z | qb1.z) & 0xffu) != 0) { tc_issue_rec(qa0, qa1); tc_issue_rec<TA>(qb0, qb1); TC_TS2(c, c.tsn2); tc_commit(c.bar); }
-#endif
-            else tc_mbar_arrive(c.bar);
-            TC_TS2(c, c.tsn2);
-        }
-        __syncwarp();
-    }
-    TC_TS(c);
-    tc_mbar_wait(c.bar, c.phase);
-    c.phase ^= 1u;
-    tc_fence_after();
-    TC_TS(c);
-}
-
-// Decoders of one 128-sample sub-tile, starting from an X0 tile that the group has already written.
-// Returns (in registers, both column halves) the density-decoder output df[16] and the colour pre-activations c3[3].
-// TA (default forward variant for the F == 2 cat grid): the activation tile lives in tensor memory (m.work_col[1]; lane = row, two halfs per column) and
-// feeds the UMMAs as the A operand directly; nothing but the weights is in shared memory.
-template <bool TA = false>
-__device__ __forceinline__ void tc_decoders(const WbTc& m, TcCtx& c, const TcIn& in, int64_t ray, float df[16], float c3[3])
-{
-    uint8_t* sub = c.smem + m.sub_off[c.g];
-    const int nl = m.nl_d + m.nl_c;
-    const uint32_t arow = c.tmem + ((uint32_t)c.laneq << 16) + (uint32_t)(TA ? m.work_col[1] : 0);
     for (int l = 0; l < nl; ++l) {
-        tc_round<TA>(c, l, TC_K_BIAS, TA ? TC_K_FWD_TA : TC_K_FWD, -1);   // accumulator = bias + X_l . W_l^T
-        const uint32_t trow = c.tmem + ((uint32_t)c.laneq << 16) + m.work_col[c.g];
         const bool last_d = (l == m.nl_d - 1), last_c = (l == nl - 1);
+        tc_publish(c);
+        if (!last_d && !last_c) {
+            // hidden layer: relu(acc) -> next input tile (F2FP.RELU), straight from the fragments; Np[l] == Kp[l+1], padded outputs
+            // are relu(0 + 0) = 0
+            uint8_t* tn = c.sub + m.tile_off[l + 1];
+            tc_fwd_layer<NMAX>(m, c, l, m.Np[l], [&](auto& d) {
+                constexpr int NR = sizeof(d) / sizeof(float);
+#pragma unroll
+                for (int i = 0; i < NR; i += 2) {
+                    const int row = tc_frag_row(c.wl, i), col = tc_frag_col(c.wl, i);
+                    *reinterpret_cast<uint32_t*>(tn + (col >> 3) * TC_SLAB + row * 16 + (col & 7) * 2) = tc_pack2_relu(d[i], d[i + 1]);
+                }
+            });
+            continue;
+        }
+        tc_fwd_layer<NMAX>(m, c, l, 16, [&](auto& d) { TC_FRAG_TO_SCRATCH(c, d, 16); });      // both heads are <= 16 wide
+        tc_sync(c);
+        const float* srow = c.scr + c.r * TC_SCR_LD;
         if (last_d) {
-            tc_ld16(trow, df);
+#pragma unroll
+            for (int j = 0; j < 16; ++j) df[j] = srow[j];
             // colour input = [df[1:], embed(ray_d)], zero padded (nerf.py:248-259): the per-ray row already holds the
             // embedding and the zero padding, only the first dout-1 (<= 15) features are per-sample.  16-byte chunk ch of the
             // row is written by column half ch & 1.
-            uint8_t* tcol = sub + m.tile_off[l + 1];
+            uint8_t* tcol = c.sub + m.tile_off[l + 1];
             const int nd = m.O[l] - 1, nch = m.Kp[l + 1] / 8;
             const uint4* re = in.ray_embed + ray * nch;
             uint4 q = __ldg(re + c.h);
@@ -571,149 +454,37 @@ __device__ __forceinline__ void tc_decoders(const WbTc& m, TcCtx& c, const TcIn&
                 const float dv = c.h == 0 ? df[(j + 1) & 15] : df[(j + 9) & 15];
                 if (8 * c.h + j < nd) hq[j] = __float2half_rn(dv);
             }
-            if (TA) {                                            // chunk ch = 8 features = 4 TMEM columns
-                tc_st4(arow + c.h * 4, q);
-                for (int ch = 2 + c.h; ch < nch; ch += 2) tc_st4(arow + ch * 4, __ldg(re + ch));
-                tc_st_wait();
-            } else {
-                *reinterpret_cast<uint4*>(tcol + c.h * 2048 + c.r * 16) = q;
-                for (int ch = 2 + c.h; ch < nch; ch += 2) *reinterpret_cast<uint4*>(tcol + ch * 2048 + c.r * 16) = __ldg(re + ch);
-            }
-        } else if (last_c) {
-            float v[16]; tc_ld16(trow, v);
-            c3[0] = v[0]; c3[1] = v[1]; c3[2] = v[2];
+            *reinterpret_cast<uint4*>(tcol + c.h * TC_SLAB + c.r * 16) = q;
+            for (int ch = 2 + c.h; ch < nch; ch += 2) *reinterpret_cast<uint4*>(tcol + ch * TC_SLAB + c.r * 16) = __ldg(re + ch);
         } else {
-            // hidden layer: relu(acc) -> next input tile (F2FP.RELU); column half h owns columns [64k + 32h, 64k + 32h + 32)
-            uint8_t* tn = sub + m.tile_off[l + 1];
-            const int Np = m.Np[l];
-            for (int cc = c.h * 32; cc < Np; cc += 64) {
-                float v[32];
-                const int nq = (Np - cc >= 32) ? 4 : 2;
-                TC_TS3(c);
-                if (nq == 4) tc_ld32(trow + cc, v); else tc_ld16(trow + cc, v);
-                TC_TS3(c);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    if (q >= nq) break;
-                    uint4 o;
-                    o.x = tc_pack2_relu(v[q * 8], v[q * 8 + 1]); o.y = tc_pack2_relu(v[q * 8 + 2], v[q * 8 + 3]);
-                    o.z = tc_pack2_relu(v[q * 8 + 4], v[q * 8 + 5]); o.w = tc_pack2_relu(v[q * 8 + 6], v[q * 8 + 7]);
-                    if (TA) tc_st4(arow + (cc >> 1) + q * 4, o);         // features cc + 8q .. +7 -> columns (cc + 8q) / 2 ..
-                    else *reinterpret_cast<uint4*>(tn + ((cc >> 3) + q) * 2048 + c.r * 16) = o;
-                }
-                if (TA) tc_st_wait();
-                TC_TS3(c);
-            }
-            // Np[l] == Kp[l+1] (both round_up(hidden,16)); padded outputs are relu(0 + 0) = 0
+            c3[0] = srow[0]; c3[1] = srow[1]; c3[2] = srow[2];
         }
     }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// forward kernel: CTA = one group = one 128-sample sub-tile at a time; several CTAs per SM overlap gather / UMMA / epilogue
+// forward kernel: CTA = TC_FWD_GROUPS groups, each walking its own 64-sample sub-tiles; several CTAs per SM overlap gather,
+// MMA chains and epilogues
 // ---------------------------------------------------------------------------------------------------------------
-// F == 2 'cat' gather straight into the TMEM activation tile (TMEM-A variant): 4 LODs = 8 features = one 16-byte chunk =
-// 4 TMEM columns of this thread's lane; the chunk is also what the backward wants saved.
-__device__ __forceinline__ void tile_gather_ta(const WbGrid& g, uint32_t arow, int half, float px, float py, float pz,
-                                               uint4* __restrict__ save, int64_t S, int64_t s, bool valid)
-{
-    for (int l0 = 4 * half; l0 < g.L; l0 += 8) {
-        float v[8];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const int l = l0 + q;
-            if (l >= g.L || l >= g.lod_idx) { v[2 * q] = 0.0f; v[2 * q + 1] = 0.0f; continue; }       // hash_grid.py:226-229
-            uint32_t idx[8]; float cf[8];
-            wb_corner_setup(g, l, px, py, pz, idx, cf);
-            const float2* tb = reinterpret_cast<const float2*>(g.table + g.begin[l] * 2);
-            float2 c[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) c[j] = __ldg(tb + idx[j]);
-            float a0 = c[0].x * cf[0], a1 = c[0].y * cf[0];
-#pragma unroll
-            for (int j = 1; j < 8; ++j) { a0 = fmaf(c[j].x, cf[j], a0); a1 = fmaf(c[j].y, cf[j], a1); }
-            v[2 * q] = a0; v[2 * q + 1] = a1;
-        }
-        uint4 qv; qv.x = tc_pack2(v[0], v[1]); qv.y = tc_pack2(v[2], v[3]); qv.z = tc_pack2(v[4], v[5]); qv.w = tc_pack2(v[6], v[7]);
-        tc_st4(arow + (uint32_t)(l0 >> 2) * 4u, qv);
-        if (save != nullptr && valid) save[(int64_t)(l0 >> 2) * S + s] = qv;
-    }
-    tc_st_wait();
-}
-
-// Software-pipelined form of tile_gather_ta (WB_TC_FWD_PIPE=1): the eight corner loads of LOD k are issued, THEN the cell / index /
-// coefficient arithmetic of LOD k+1 runs (~200 instructions), and only then are LOD k's corners blended -- the gather's L1/L2 latency
-// (long_scoreboard: 5.2 stalls per issue, profiles/r02e) overlaps ALU work of the same warp.  Needs more registers than the plain form.
-__device__ __forceinline__ void tile_gather_ta_pipe(const WbGrid& g, uint32_t arow, int half, float px, float py, float pz,
-                                                    uint4* __restrict__ save, int64_t S, int64_t s, bool valid)
-{
-    const int nlev = min(g.L, g.lod_idx);                        // LODs >= lod_idx are zeroed (hash_grid.py:226-229)
-    uint32_t idx[8]; float cf[8]; float2 c[8];
-    int lnext = 4 * half;
-    bool have = false;
-    if (lnext < nlev) {
-        wb_corner_setup(g, lnext, px, py, pz, idx, cf);
-        const float2* tb = reinterpret_cast<const float2*>(g.table + g.begin[lnext] * 2);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) c[j] = __ldg(tb + idx[j]);
-        have = true;
-    }
-    for (int l0 = 4 * half; l0 < g.L; l0 += 8) {
-        float v[8];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-            const int l = l0 + q;
-            if (l >= nlev || !have) { v[2 * q] = 0.0f; v[2 * q + 1] = 0.0f; continue; }
-            float cfl[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) cfl[j] = cf[j];
-            const int ln = ((l & 3) == 3) ? l + 5 : l + 1;         // this thread's next LOD: 4h, 4h+1, 4h+2, 4h+3, 4h+8, ...
-            const bool more = ln < nlev;
-            if (more) wb_corner_setup(g, ln, px, py, pz, idx, cf);
-            float a0 = c[0].x * cfl[0], a1 = c[0].y * cfl[0];
-#pragma unroll
-            for (int j = 1; j < 8; ++j) { a0 = fmaf(c[j].x, cfl[j], a0); a1 = fmaf(c[j].y, cfl[j], a1); }
-            v[2 * q] = a0; v[2 * q + 1] = a1;
-            if (more) {
-                const float2* tb = reinterpret_cast<const float2*>(g.table + g.begin[ln] * 2);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) c[j] = __ldg(tb + idx[j]);
-            }
-            have = more;
-        }
-        uint4 qv; qv.x = tc_pack2(v[0], v[1]); qv.y = tc_pack2(v[2], v[3]); qv.z = tc_pack2(v[4], v[5]); qv.w = tc_pack2(v[6], v[7]);
-        tc_st4(arow + (uint32_t)(l0 >> 2) * 4u, qv);
-        if (save != nullptr && valid) save[(int64_t)(l0 >> 2) * S + s] = qv;
-    }
-    tc_st_wait();
-}
-
-template <int MINB, bool TA, bool GX = false, bool PIPE = false>   // MINB: resident CTAs per SM the register allocation is bounded for; TA: activations in tensor
-                                                // memory; GX: triplanar / octree feature grid (wb_featx.cuh) instead of the hash grid
-__global__ void __launch_bounds__(TC_GROUP, MINB)
+template <int MINB, bool GX, int NMAX>   // MINB: resident CTAs per SM the register allocation is bounded for; GX: triplanar / octree
+                                         // feature grid (wb_featx.cuh) instead of the hash grid; NMAX: widest padded layer (64 or 128)
+__global__ void __launch_bounds__(TC_FWD_GROUPS * TC_GROUP, MINB)
 wb_shade_fwd_tc_kernel(WbGrid g, WbGridX gx, WbTc m, const uint8_t* __restrict__ blob, TcIn in, float4* __restrict__ shaded)
 {
     extern __shared__ __align__(1024) uint8_t smem[];
-    __shared__ __align__(8) uint64_t bars[2];
-    __shared__ uint32_t tmem_s;
-    __shared__ TcRec itab[TC_KINDS * TC_ML];
+    __shared__ __align__(8) uint64_t bar;
     if (threadIdx.x == 0) {
-        tc_mbar_init(&bars[0], TC_ISSUERS); tc_mbar_init(&bars[1], 1); tc_mbar_init_fence();
-        tc_mbar_expect_tx(&bars[1], (uint32_t)m.blob_bytes);
-        tc_bulk_g2s(smem + m.w_smem_off, blob, (uint32_t)m.blob_bytes, &bars[1]);      // TMA: parameters -> shared memory
+        tc_mbar_init(&bar, 1); tc_mbar_init_fence();
+        tc_mbar_expect_tx(&bar, (uint32_t)m.blob_bytes);
+        tc_bulk_g2s(smem + m.w_smem_off, blob, (uint32_t)m.blob_bytes, &bar);      // TMA: parameters -> shared memory
     }
-    if (threadIdx.x < 32) tc_tmem_alloc(&tmem_s, (uint32_t)m.tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    tc_build_table(m, itab, smem, tmem_s, 1, false, TA);
-    __syncthreads();
-    tc_mbar_wait(&bars[1], 0);
-    TcCtx c; tc_ctx_init(c, smem, bars, itab, tmem_s, 0);
-    uint8_t* t0 = smem + m.sub_off[0] + m.tile_off[0];
+    tc_mbar_wait(&bar, 0);
+    TcCtx c; tc_ctx_init(c, m, smem);
+    uint8_t* t0 = c.sub + m.tile_off[0];
     const int nch0 = m.Kp[0] / 8;
     const int64_t ntiles = (in.S + TC_ROWS - 1) / TC_ROWS;
-    for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    for (int64_t tile = (int64_t)blockIdx.x * TC_FWD_GROUPS + c.g; tile < ntiles; tile += (int64_t)gridDim.x * TC_FWD_GROUPS) {
         int64_t s = tile * TC_ROWS + c.r;
         const bool valid = s < in.S;
         if (!valid) s = in.S - 1;
@@ -723,37 +494,28 @@ wb_shade_fwd_tc_kernel(WbGrid g, WbGridX gx, WbTc m, const uint8_t* __restrict__
         const float py = wb_addcmul(__ldg(in.origins + 3 * ray + 1), __ldg(in.dirs + 3 * ray + 1), t);
         const float pz = wb_addcmul(__ldg(in.origins + 3 * ray + 2), __ldg(in.dirs + 3 * ray + 2), t);
         // density-decoder input row: grid features (+ position embedding), zero padded to Kp; the two threads of a row split the LODs
-        if (TA) {
-            if (PIPE) tile_gather_ta_pipe(g, c.tmem + ((uint32_t)c.laneq << 16) + (uint32_t)m.work_col[1], c.h, px, py, pz, in.x0_save, in.S, s, valid);
-            else tile_gather_ta(g, c.tmem + ((uint32_t)c.laneq << 16) + (uint32_t)m.work_col[1], c.h, px, py, pz, in.x0_save, in.S, s, valid);
-        } else {
-            if (!GX) tile_gather(g, t0, c.r, c.h, px, py, pz);
-            else if (c.h == 0) {
-                // one thread of the row pair gathers all LODs.  Splitting the LODs over the pair (partial sums through shared memory for 'sum'
-                // grids) was measured SLOWER on config 4 (231 -> 280 ms per 800^2 frame): the gather is latency-bound, the extra group
-                // barrier and scratch traffic cost more than the halved chain saves
-                wb_featx_gather(gx, px, py, pz, [&](int f, float v) { tile_store1(t0, c.r, f, v); });
-            }
-            if (c.h == 0) {
-                tile_embed(t0, c.r, m.feat_dim, m.pos_mode, m.pos_freq, px, py, pz);
-                tile_zero(t0, c.r, m.I[0], m.Kp[0]);
-            }
-            if (in.x0_save) {
-                tc_group_sync(1, TC_GROUP);
-                if (valid)
-                    for (int ch = c.h; ch < nch0; ch += 2) in.x0_save[(int64_t)ch * in.S + s] = *reinterpret_cast<const uint4*>(t0 + ch * 2048 + c.r * 16);
-            }
+        if (!GX) tile_gather(g, t0, c.r, c.h, px, py, pz);
+        else if (c.h == 0) {
+            // one thread of the row pair gathers all LODs: the gather is latency-bound, splitting it over the pair costs a group
+            // barrier and scratch traffic for partial sums of 'sum' grids
+            wb_featx_gather(gx, px, py, pz, [&](int f, float v) { tile_store1(t0, c.r, f, v); });
+        }
+        if (c.h == 0) {
+            tile_embed(t0, c.r, m.feat_dim, m.pos_mode, m.pos_freq, px, py, pz);
+            tile_zero(t0, c.r, m.I[0], m.Kp[0]);
+        }
+        if (in.x0_save) {
+            tc_sync(c);
+            if (valid)
+                for (int ch = c.h; ch < nch0; ch += 2) in.x0_save[(int64_t)ch * in.S + s] = *reinterpret_cast<const uint4*>(t0 + ch * TC_SLAB + c.r * 16);
         }
         float df[16], c3[3];
-        tc_decoders<TA>(m, c, in, ray, df, c3);
+        tc_decoders<NMAX>(m, c, in, ray, df, c3);
         if (valid && c.h == 0) {
             const float r = 1.0f / (1.0f + expf(-c3[0])), gg = 1.0f / (1.0f + expf(-c3[1])), b = 1.0f / (1.0f + expf(-c3[2]));
             shaded[s] = make_float4(r, gg, b, fmaxf(df[0], 0.0f));
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (threadIdx.x < 32) tc_tmem_dealloc(c.tmem, (uint32_t)m.tmem_cols);
 }
 
 // set by wb_rf_workspace_holds_ray_rows(): the next backward of this thread finds the per-ray colour-input rows in its workspace already
@@ -770,13 +532,10 @@ static int tc_launch_ray_embed(const WbTc& m, const wb_rays* rays, void* workspa
     return WB_OK;
 }
 
-// Tuning knobs (defaults = the measured optimum on B200 for the app/nerf configuration, profiles/README.md); the environment
-// overrides exist for the sweeps and are read once per process.
+// Tuning knobs; the environment overrides exist for sweeps and variant tests and are read once per process.
 static int tc_env_int(const char* name, int dflt) { const char* v = getenv(name); return v && *v ? atoi(v) : dflt; }
-static int tc_knob_fuse_scatter() { static const int v = tc_env_int("WB_TC_FUSE_SCATTER", 1); return v; }     // 0 separate kernel, 1 last epilogue (default), 2 pipelined
-static int tc_knob_bwd_groups() { static const int v = tc_env_int("WB_TC_BWD_GROUPS", 3); return v; }
-static int tc_knob_fwd_tmema() { static const int v = tc_env_int("WB_TC_FWD_TMEMA", 1); return v; }
-static int tc_knob_fwd_pipe() { static const int v = tc_env_int("WB_TC_FWD_PIPE", 0); return v; }
+static int tc_knob_fuse_scatter() { static const int v = tc_env_int("WB_TC_FUSE_SCATTER", 1); return v; }     // 0 separate kernel, 1 last epilogue
+static int tc_knob_bwd_groups() { static const int v = tc_env_int("WB_TC_BWD_GROUPS", 2); return v; }          // upper bound: 1 or 2
 static int tc_knob_fwd_ctas() { static const int v = tc_env_int("WB_TC_FWD_CTAS", 3); return v; }
 static int tc_knob_fuse_scatter_wide() { static const int v = tc_env_int("WB_TC_FUSE_SCATTER_WIDE", 0); return v; }
 static int64_t tc_knob_wide_min_s() { static const int v = tc_env_int("WB_TC_WIDE_MIN_S", 1 << 20); return v; }      // below this many samples the chunked schedule is not worth its launches
@@ -792,121 +551,201 @@ int wb_tc_shade_fwd(const wb_nef_desc* nef, const float* blob, const wb_rays* ra
 {
     WbGrid g; int rc = wb_make_grid(nef, &g); if (rc) return rc;
     WbGridX gx; rc = wb_make_gridx(nef, false, &gx); if (rc) return rc;
-    // Default since round 2 (WB_TC_FWD_TMEMA=0 selects the shared-memory tile): activations in tensor memory, A operand read from TMEM
-    // (wb_tc.cuh tc_mma_ts); measured 3.10 -> 2.86 ms on the 1024^2 frame, same results.
-    // Applies to the specialised F == 2 'cat' gather without position embedding, whose rows are whole 16-byte chunks.
-    const bool ta = tc_knob_fwd_tmema() && nef->grid_kind == 0 && nef->feature_dim == 2 && nef->multiscale == 0 && nef->pos_mode == 0 &&
-                    (nef->num_lods * nef->feature_dim) % 16 == 0;
-    WbTc m; rc = wb_tc_make(nef, false, &m, ta); if (rc) return rc;
-    if (ta) {   // no activation tile in shared memory: the parameter blob and the bias tile move to the front
-        const int tile = m.w_smem_off;
-        m.w_smem_off -= tile; m.ones_off -= tile; m.smem_bytes -= tile;
-    }
+    WbTc m; rc = wb_tc_make(nef, false, &m); if (rc) return rc;
     WB_CHECK_ARG(workspace != nullptr, "precision 1 needs the workspace (wb_rf_workspace_bytes)");
     rc = tc_launch_ray_embed(m, rays, workspace, st); if (rc) return rc;
     TcIn in = { rays->origins, rays->dirs, rec_t, rec_ray, S, reinterpret_cast<const uint4*>(workspace), reinterpret_cast<uint4*>(feat_save), nullptr };
-    // CTAs per SM: each is one sub-tile group; more groups in flight hide the gather and round latencies (measured sweep in
-    // profiles/README.md).  The register bound of the instantiation must match, or the hardware silently runs fewer.
-    int per_sm = (227 * 1024) / (m.smem_bytes + 4096); per_sm = max(1, min(per_sm, 512 / m.tmem_cols));
-    per_sm = max(2, min(min(per_sm, 4), tc_knob_fwd_ctas()));
-    // the generic grids keep more state per thread.  Triplanar (12 planes x 4 texel loads in flight): 3 CTAs per SM at 80 registers beat 2 at 128
-    // despite 144 B of spills (config 4 forward 105 -> 88 ms measured); the octree gather (up to 32 accumulators) stays at 2
-    if (gx.kind != 0) per_sm = max(2, min(min(per_sm, 4), tc_env_int("WB_TC_GX_CTAS", gx.kind == 1 ? 3 : 2)));
-    const bool pipe = ta && tc_knob_fwd_pipe() != 0 && per_sm <= 3;
-    auto kern = gx.kind != 0 ? (per_sm == 4 ? wb_shade_fwd_tc_kernel<4, false, true> : per_sm == 3 ? wb_shade_fwd_tc_kernel<3, false, true> : wb_shade_fwd_tc_kernel<2, false, true>)
-              : pipe ? (per_sm == 2 ? wb_shade_fwd_tc_kernel<2, true, false, true> : wb_shade_fwd_tc_kernel<3, true, false, true>)
-              : ta ? (per_sm == 2 ? wb_shade_fwd_tc_kernel<2, true> : per_sm == 3 ? wb_shade_fwd_tc_kernel<3, true> : wb_shade_fwd_tc_kernel<4, true>)
-                   : (per_sm == 2 ? wb_shade_fwd_tc_kernel<2, false> : per_sm == 3 ? wb_shade_fwd_tc_kernel<3, false> : wb_shade_fwd_tc_kernel<4, false>);
+    // CTAs per SM: more groups in flight hide the gather and chain latencies.  The register bound of the instantiation must match,
+    // or the hardware silently runs fewer.
+    // Decoders up to 64 wide: 2 or 3 CTAs (85 registers per thread); wider ones: 1 or 2 (a 128-wide accumulator is 64 registers).
+    const bool wide = m.maxw > 64;
+    int per_sm = max(1, min(3, TC_SMEM_MAX / (m.smem_bytes + 1024)));
+    per_sm = min(per_sm, max(1, tc_knob_fwd_ctas()));
+    // the generic grids keep more state per thread (octree gather: up to 32 accumulators)
+    if (gx.kind != 0) per_sm = min(per_sm, tc_env_int("WB_TC_GX_CTAS", gx.kind == 1 ? 3 : 2));
+    per_sm = wide ? min(per_sm, 2) : max(per_sm, 2);
+    auto kern = wide ? (gx.kind != 0 ? (per_sm == 2 ? wb_shade_fwd_tc_kernel<2, true, 128> : wb_shade_fwd_tc_kernel<1, true, 128>)
+                                     : (per_sm == 2 ? wb_shade_fwd_tc_kernel<2, false, 128> : wb_shade_fwd_tc_kernel<1, false, 128>))
+                     : (gx.kind != 0 ? (per_sm == 3 ? wb_shade_fwd_tc_kernel<3, true, 64> : wb_shade_fwd_tc_kernel<2, true, 64>)
+                                     : (per_sm == 3 ? wb_shade_fwd_tc_kernel<3, false, 64> : wb_shade_fwd_tc_kernel<2, false, 64>));
     {   // function attributes are driver calls that can wait behind other driver work (e.g. an NVML poll): set them once, not per launch
-        static int64_t done_for[24] = { -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1, -1 };
-        if (done_for[gx.kind != 0 ? 16 + per_sm : pipe ? 10 + per_sm : per_sm + (ta ? 5 : 0)] != WB_ATTR_KEY(m.smem_bytes)) {
+        static int64_t done_for[2][2][4] = { { { -1, -1, -1, -1 }, { -1, -1, -1, -1 } }, { { -1, -1, -1, -1 }, { -1, -1, -1, -1 } } };
+        int64_t& done = done_for[wide ? 1 : 0][gx.kind != 0 ? 1 : 0][per_sm];
+        if (done != WB_ATTR_KEY(m.smem_bytes)) {
             WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, m.smem_bytes));
-            WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                         min(100, (per_sm * (m.smem_bytes + 4096) * 100) / (228 * 1024) + 1)));
-            done_for[gx.kind != 0 ? 16 + per_sm : pipe ? 10 + per_sm : per_sm + (ta ? 5 : 0)] = WB_ATTR_KEY(m.smem_bytes);
+            done = WB_ATTR_KEY(m.smem_bytes);
         }
     }
-    const int64_t ntiles = (S + TC_ROWS - 1) / TC_ROWS;
-    int64_t grid = (int64_t)wb_num_sms() * per_sm; if (grid > ntiles) grid = ntiles;
-    const int xscratch = 0;
-    kern<<<(unsigned)grid, TC_GROUP, m.smem_bytes + xscratch, st>>>(g, gx, m, reinterpret_cast<const uint8_t*>(blob), in, reinterpret_cast<float4*>(shaded));
+    const int64_t ntiles = (S + TC_ROWS - 1) / TC_ROWS, nctas = (ntiles + TC_FWD_GROUPS - 1) / TC_FWD_GROUPS;
+    int64_t grid = (int64_t)wb_num_sms() * per_sm; if (grid > nctas) grid = nctas;
+    if (grid == 0) return WB_OK;
+    kern<<<(unsigned)grid, TC_FWD_GROUPS * TC_GROUP, m.smem_bytes, st>>>(g, gx, m, reinterpret_cast<const uint8_t*>(blob), in, reinterpret_cast<float4*>(shaded));
     WB_LAUNCH_CHECK();
     return WB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// decoder backward kernel: CTA = TC_BWD_GROUPS groups (one per SM: TMEM holds the weight-grad accumulators), each group walks
-// its own sequence of 128-sample sub-tiles with its own barriers, so the groups drift out of phase and overlap
+// decoder backward kernel: CTA = m.groups groups (one CTA per SM: the retained tiles and the weight-grad accumulators fill shared
+// memory), each group walks its own sequence of 64-sample sub-tiles with its own barrier, so the groups drift out of phase and overlap
 // ---------------------------------------------------------------------------------------------------------------
 struct TcGrads { float* gdens; float* gcol; const float* scale; __half* dfeat; int planes, width; };
 
-__global__ void __launch_bounds__(TC_BWD_GROUPS * TC_GROUP, 1)
-wb_mlp_bwd_tc_kernel(WbTc m, const uint8_t* __restrict__ blob, TcIn in, const float4* __restrict__ g_shaded, TcGrads G)
+// One LOD of the hash-table scatter for the 32 consecutive samples of a warp (F == 2): the arithmetic of wb_table_scatter_kernel
+// <2, true, true> (hashgrid_interpolate_cuda.cu:151-160 + run merging + paired 16-byte reductions), callable from the decoder
+// backward's last epilogue so that dL/dfeat never leaves the SM.  s0, s1: this sample's (still loss-scaled) gradient of the LOD's two
+// features.  Warp-collective: every lane of the warp calls it with the same `l`.
+__device__ __forceinline__ void tc_scatter_level_f2(const WbGrid& g, int l, float px, float py, float pz, bool valid, float s0, float s1,
+                                                    float inv_scale, int lane, float* __restrict__ gtable)
+{
+    float* tb = gtable + g.begin[l] * 2;
+    const bool pair_ok = (reinterpret_cast<uintptr_t>(tb) & 15u) == 0;
+    uint32_t idx[8]; float cf[8]; uint64_t key = ~0ull - (uint64_t)lane;    // invalid lanes never merge
+    if (valid) {
+        int ix, iy, iz; float wx, wy, wz, jx, jy, jz;
+        wb_cell(px, g.hres[l], g.hi[l], ix, wx, jx); wb_cell(py, g.hres[l], g.hi[l], iy, wy, jy); wb_cell(pz, g.hres[l], g.hi[l], iz, wz, jz);
+        key = (uint64_t)ix | ((uint64_t)iy << 20) | ((uint64_t)iz << 40);
+        const float xy00 = jx * jy, xy01 = jx * wy, xy10 = wx * jy, xy11 = wx * wy;
+        cf[0] = xy00 * jz; cf[1] = xy00 * wz; cf[2] = xy01 * jz; cf[3] = xy01 * wz;
+        cf[4] = xy10 * jz; cf[5] = xy10 * wz; cf[6] = xy11 * jz; cf[7] = xy11 * wz;
+        wb_corner_indices(g, l, ix, iy, iz, idx);
+    } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { idx[j] = 0; cf[j] = 0.0f; }
+    }
+    const uint64_t kprev = __shfl_up_sync(0xffffffffu, key, 1);
+    const bool head = (lane == 0) || (kprev != key);
+    const uint32_t heads = __ballot_sync(0xffffffffu, head);
+    const int run_head = 31 - __clz(heads & (0xffffffffu >> (31 - lane)));
+    const int dist = lane - run_head;
+    const bool tail = (lane == 31) || ((heads >> (lane + 1)) & 1u);
+    const int maxd = __reduce_max_sync(0xffffffffu, dist);
+    float v0[8], v1[8];
+    if (maxd > 0) {     // run sums as loss-scaled fp16 pairs (one shuffle per corner and scan step), unscaled after the scan
+        __half2 h[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) h[j] = __floats2half2_rn(s0 * cf[j], s1 * cf[j]);
+        for (int o = 1; o <= maxd; o <<= 1) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const __half2 a = __shfl_up_sync(0xffffffffu, h[j], o);
+                if (dist >= o) h[j] = __hadd2(h[j], a);
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { const float2 f = __half22float2(h[j]); v0[j] = f.x * inv_scale; v1[j] = f.y * inv_scale; }
+    } else {
+        const float g0 = s0 * inv_scale, g1 = s1 * inv_scale;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { v0[j] = g0 * cf[j]; v1[j] = g1 * cf[j]; }
+    }
+    if (tail && valid) {
+        float2* t2 = reinterpret_cast<float2*>(tb);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const uint32_t i0 = idx[j], i1 = idx[j + 4];
+            const bool nz0 = (v0[j] != 0.0f || v1[j] != 0.0f), nz1 = (v0[j + 4] != 0.0f || v1[j + 4] != 0.0f);
+            if (pair_ok && ((i0 ^ i1) == 1u)) {
+                if (nz0 || nz1) {
+                    const float4 val = (i0 & 1u) ? make_float4(v0[j + 4], v1[j + 4], v0[j], v1[j]) : make_float4(v0[j], v1[j], v0[j + 4], v1[j + 4]);
+                    atomicAdd(reinterpret_cast<float4*>(t2 + (i0 & ~1u)), val);
+                }
+            } else {
+                if (nz0) atomicAdd(t2 + i0, make_float2(v0[j], v1[j]));
+                if (nz1) atomicAdd(t2 + i1, make_float2(v0[j + 4], v1[j + 4]));
+            }
+        }
+    }
+}
+
+// wmask: layers whose weight gradients this launch accumulates; emit: this launch produces dL/dfeat (planes, or FUSE: the hash-table
+// scatter of an F == 2 'cat' grid in the last epilogue).  Wide decoders whose accumulators do not all fit run several launches.
+template <int NG, bool FUSE>
+__global__ void __launch_bounds__(NG * TC_GROUP, 1)
+wb_mlp_bwd_tc_kernel(WbTc m, const uint8_t* __restrict__ blob, TcIn in, const float4* __restrict__ g_shaded, TcGrads G,
+                     unsigned wmask, int emit, WbGrid g, float* __restrict__ gtable)
 {
     extern __shared__ __align__(1024) uint8_t smem[];
-    __shared__ __align__(8) uint64_t bars[TC_BWD_GROUPS + 1];
-    __shared__ uint32_t tmem_s;
-    __shared__ TcRec itab[TC_BWD_GROUPS * TC_KINDS * TC_ML];
+    __shared__ __align__(8) uint64_t bar;
     const int nl = m.nl_d + m.nl_c;
     if (threadIdx.x == 0) {
-        for (int i = 0; i < TC_BWD_GROUPS; ++i) tc_mbar_init(&bars[i], TC_ISSUERS);
-        tc_mbar_init(&bars[TC_BWD_GROUPS], 1); tc_mbar_init_fence();
-        tc_mbar_expect_tx(&bars[TC_BWD_GROUPS], (uint32_t)m.blob_bytes);
-        tc_bulk_g2s(smem + m.w_smem_off, blob, (uint32_t)m.blob_bytes, &bars[TC_BWD_GROUPS]);
+        tc_mbar_init(&bar, 1); tc_mbar_init_fence();
+        tc_mbar_expect_tx(&bar, (uint32_t)m.blob_bytes);
+        tc_bulk_g2s(smem + m.w_smem_off, blob, (uint32_t)m.blob_bytes, &bar);
     }
-    if (threadIdx.x < 32) tc_tmem_alloc(&tmem_s, (uint32_t)m.tmem_cols);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    tc_build_table(m, itab, smem, tmem_s, TC_BWD_GROUPS, true);
-    TcCtx c; tc_ctx_init(c, smem, bars, itab, tmem_s, 1);
-    uint8_t* sub = smem + m.sub_off[c.g];
-    // constant-one slab behind every input tile: feature 0 = 1, features 1..7 = 0  (bias gradient row of the weight grad)
+    TcCtx c; tc_ctx_init(c, m, smem);
+    float* acc = reinterpret_cast<float*>(c.sub + m.acc_off);
+    const int nacc = (m.group_bytes - m.acc_off) / 4;
+    for (int i = c.wl; i < nacc; i += TC_GROUP) acc[i] = 0.0f;
+    // constant-one slab behind every input tile: feature 0 = 1, features 1..7 = 0  (bias gradient column of the weight grad)
     for (int l = c.h; l < nl; l += 2) {
         uint4 one; one.x = 0x00003C00u; one.y = 0; one.z = 0; one.w = 0;           // fp16 1.0 in the low half
-        *reinterpret_cast<uint4*>(sub + m.tile_off[l] + (m.Kp[l] / 8) * 2048 + c.r * 16) = one;
+        *reinterpret_cast<uint4*>(c.sub + m.tile_off[l] + (m.Kp[l] / 8) * TC_SLAB + c.r * 16) = one;
     }
-    if (threadIdx.x < 128) {                                       // zero the resident weight-grad accumulators (all 128 lanes)
-        const uint32_t tr = c.tmem + ((uint32_t)c.laneq << 16);
-        for (int l = 0; l < nl; ++l)
-            for (int cc = 0; cc < m.Np[l]; cc += 16) tc_st16_zero(tr + m.acc_col[l] + cc);
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    tc_mbar_wait(&bars[TC_BWD_GROUPS], 0);
+    tc_mbar_wait(&bar, 0);
     const float scale = __ldg(G.scale), inv_scale = 1.0f / scale;
-    uint8_t* dyt = smem + m.dy_off[c.g];
-    uint8_t* t0 = sub + m.tile_off[0];
+    uint8_t* dyt = c.sub + m.dy_off;
+    uint8_t* t0 = c.sub + m.tile_off[0];
+    const uint32_t dyb = tc_smem_u32(dyt), wb = tc_smem_u32(c.blob);
     const int nch0 = m.Kp[0] / 8;
-    const int64_t ntiles = (in.S + TC_ROWS - 1) / TC_ROWS;
+    const int64_t s_end = in.s_end ? in.s_end : in.S;             // this launch's sample range (in.S stays the stride of the saved rows / planes)
+    const int64_t tile0 = in.s_begin / TC_ROWS, ntiles = (s_end + TC_ROWS - 1) / TC_ROWS;
     const float z8[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
-    for (int64_t tile = (int64_t)blockIdx.x * TC_BWD_GROUPS + c.g; tile < ntiles; tile += (int64_t)gridDim.x * TC_BWD_GROUPS) {
+    const int lane = threadIdx.x & 31;
+    for (int64_t tile = tile0 + (int64_t)blockIdx.x * NG + c.g; tile < ntiles; tile += (int64_t)gridDim.x * NG) {
         int64_t s = tile * TC_ROWS + c.r;
-        const bool valid = s < in.S;
-        if (!valid) s = in.S - 1;
+        const bool valid = s < s_end;
+        if (!valid) s = s_end - 1;
         const int64_t ray = __ldg(in.rec_ray + s);
         for (int ch = c.h; ch < nch0; ch += 2)                     // saved density-decoder input row (coalesced 16 B per lane)
-            *reinterpret_cast<uint4*>(t0 + ch * 2048 + c.r * 16) = __ldg(in.x0_saved + (int64_t)ch * in.S + s);
+            *reinterpret_cast<uint4*>(t0 + ch * TC_SLAB + c.r * 16) = __ldg(in.x0_saved + (int64_t)ch * in.S + s);
         float df[16], c3[3];
-        tc_decoders(m, c, in, ray, df, c3);
-        float4 go = valid ? __ldg(g_shaded + s) : make_float4(0, 0, 0, 0);
+        tc_decoders<128>(m, c, in, ray, df, c3);
+        const float4 go = valid ? __ldg(g_shaded + s) : make_float4(0, 0, 0, 0);
         // ---- colour decoder, last layer: dY = dL/d(pre-sigmoid), zero padded ----
-        {
-            if (c.h == 0) {
-                const float r = 1.0f / (1.0f + expf(-c3[0])), gg = 1.0f / (1.0f + expf(-c3[1])), b = 1.0f / (1.0f + expf(-c3[2]));
-                float v[8] = { go.x * r * (1.0f - r) * scale, go.y * gg * (1.0f - gg) * scale, go.z * b * (1.0f - b) * scale, 0, 0, 0, 0, 0 };
-                tile_store8(dyt, c.r, 0, v);
-            }
-            for (int sl = 1 + c.h; sl < m.Np[nl - 1] / 8; sl += 2) tile_store8(dyt, c.r, sl, z8);
+        if (c.h == 0) {
+            const float r = 1.0f / (1.0f + expf(-c3[0])), gg = 1.0f / (1.0f + expf(-c3[1])), b = 1.0f / (1.0f + expf(-c3[2]));
+            float v[8] = { go.x * r * (1.0f - r) * scale, go.y * gg * (1.0f - gg) * scale, go.z * b * (1.0f - b) * scale, 0, 0, 0, 0, 0 };
+            tile_store8(dyt, c.r, 0, v);
         }
-        const uint32_t trow = c.tmem + ((uint32_t)c.laneq << 16) + m.work_col[c.g];
+        for (int sl = 1 + c.h; sl < m.Np[nl - 1] / 8; sl += 2) tile_store8(dyt, c.r, sl, z8);
         for (int l = nl - 1; l >= 0; --l) {
-            tc_round(c, l, TC_K_WGRAD, -1, TC_K_DGRAD);
-            // D_work row = dL/d(input of layer l), Kp[l] wide
+            tc_publish(c);
+            const int I = m.I[l], O = m.O[l], Kp = m.Kp[l], Np = m.Np[l];
+            const uint32_t xb = tc_smem_u32(c.sub + m.tile_off[l]);
+            if (m.acc_l[l] >= 0) {
+                // acc_l^T[out, in] += dY_l^T . X_l and, from the constant-one slab, acc_l^T[out, I] += dY_l^T . 1  (K = the 64 samples)
+                float* al = acc + m.acc_l[l];
+                for (int mb = 0; mb < Np; mb += 64) {
+                    const uint64_t da = tc_desc(dyb + (uint32_t)(mb / 8) * TC_SLAB, 128, TC_SLAB);
+                    tc_chain_n<1, 1>(c, Kp, da, tc_desc(xb, 128, TC_SLAB), TC_ROWS / 16, 256 >> 4, 256 >> 4, nullptr, [&](auto& d) {
+                        constexpr int NR = sizeof(d) / sizeof(float);
+#pragma unroll
+                        for (int i = 0; i < NR; ++i) {
+                            const int o = mb + tc_frag_row(c.wl, i), k = tc_frag_col(c.wl, i);
+                            if (o < O && k < I) al[o * (I + 1) + k] += d[i];
+                        }
+                    });
+                    if (m.src_b[l] >= 0)
+                        tc_chain<8, 1, 1>(c, da, tc_desc(xb + (uint32_t)(Kp / 8) * TC_SLAB, 128, TC_SLAB), TC_ROWS / 16, 256 >> 4, 256 >> 4, nullptr, [&](auto& d) {
+#pragma unroll
+                            for (int i = 0; i < 4; ++i) {
+                                const int o = mb + tc_frag_row(c.wl, i);
+                                if (o < O && tc_frag_col(c.wl, i) == 0) al[o * (I + 1) + I] += d[i];
+                            }
+                        });
+                }
+            }
+            if (l == 0 && !emit) break;
+            // dX_l = dY_l . W_l  (A: dY tile K-major over the Np outputs, B: weight pack read MN-major); the first colour layer only needs
+            // the gradient of its dout - 1 <= 15 density features
+            const int N = (l == m.nl_d) ? 16 : Kp;
+            const uint64_t da = tc_desc(dyb, TC_SLAB, 128), db = tc_desc(wb + m.w_off[l], 128, Np * 16);
             if (l == m.nl_d) {
                 // first colour layer: inputs [df[1:dout], embed(ray_d)]; only the first dout-1 carry gradient (nerf.py:259)
-                float v[16]; tc_ld16(trow, v);
+                tc_chain_n<0, 1>(c, N, da, db, Np / 16, (2 * TC_SLAB) >> 4, 256 >> 4, nullptr, [&](auto& d) { TC_FRAG_TO_SCRATCH(c, d, 16); });
+                tc_sync(c);
+                const float* v = c.scr + c.r * TC_SCR_LD;
                 const int dout = m.O[m.nl_d - 1];
                 float gdf[16];
                 gdf[0] = (df[0] > 0.0f) ? go.w * scale : 0.0f;   // relu' of density (nerf.py:263)
@@ -914,80 +753,72 @@ wb_mlp_bwd_tc_kernel(WbTc m, const uint8_t* __restrict__ blob, TcIn in, const fl
                 for (int j = 1; j < 16; ++j) gdf[j] = (j < dout) ? v[j - 1] : 0.0f;
                 if (c.h == 0) tile_store8(dyt, c.r, 0, gdf); else tile_store8(dyt, c.r, 1, gdf + 8);
                 for (int sl = 2 + c.h; sl < m.Np[l - 1] / 8; sl += 2) tile_store8(dyt, c.r, sl, z8);
+            } else if (l == 0 && FUSE) {
+                // dL/d(grid features) -> hash table: column half h holds features [16h, 16h+16) = LODs 8h .. 8h+7; a warp = 32
+                // consecutive samples of one half
+                tc_chain_n<0, 1>(c, N, da, db, Np / 16, (2 * TC_SLAB) >> 4, 256 >> 4, nullptr, [&](auto& d) { TC_FRAG_TO_SCRATCH(c, d, 32); });
+                tc_sync(c);
+                const float* v = c.scr + c.r * TC_SCR_LD + c.h * 16;
+                const float t = __ldg(in.rec_t + s);
+                const float px = wb_addcmul(__ldg(in.origins + 3 * ray), __ldg(in.dirs + 3 * ray), t);
+                const float py = wb_addcmul(__ldg(in.origins + 3 * ray + 1), __ldg(in.dirs + 3 * ray + 1), t);
+                const float pz = wb_addcmul(__ldg(in.origins + 3 * ray + 2), __ldg(in.dirs + 3 * ray + 2), t);
+#pragma unroll
+                for (int q = 0; q < 8; ++q) {
+                    const int lv = c.h * 8 + q;
+                    if (lv < G.planes) tc_scatter_level_f2(g, lv, px, py, pz, valid, v[2 * q], v[2 * q + 1], inv_scale, lane, gtable);
+                }
             } else if (l == 0) {
-                // dL/d(grid features) -> fp16 planes [plane][S][width] (still loss-scaled); tcgen05.ld is warp-collective
+                // dL/d(grid features) -> fp16 planes [plane][S][width] (still loss-scaled), straight from the fragments
                 const int W = G.width, nfe = G.planes * W;
-                for (int f0 = c.h * 16; f0 < nfe; f0 += 32) {
-                    float v[16]; tc_ld16(trow + f0, v);
-                    if (!valid) continue;
-                    if (W == 2) {
+                const int64_t srow0 = tile * TC_ROWS;
+                tc_chain_n<0, 1>(c, N, da, db, Np / 16, (2 * TC_SLAB) >> 4, 256 >> 4, nullptr, [&](auto& d) {
+                    constexpr int NR = sizeof(d) / sizeof(float);
 #pragma unroll
-                        for (int qq = 0; qq < 8; ++qq) {
-                            const int pl = (f0 >> 1) + qq;
-                            if (pl < G.planes) reinterpret_cast<__half2*>(G.dfeat)[(int64_t)pl * in.S + s] = __floats2half2_rn(v[2 * qq], v[2 * qq + 1]);
-                        }
-                    } else {
-#pragma unroll
-                        for (int jj = 0; jj < 16; ++jj) {
-                            const int fe = f0 + jj;
-                            if (fe < nfe) G.dfeat[((int64_t)(fe / W) * in.S + s) * W + (fe % W)] = __float2half_rn(v[jj]);
+                    for (int i = 0; i < NR; i += 2) {
+                        const int64_t sr = srow0 + tc_frag_row(c.wl, i);
+                        const int fe = tc_frag_col(c.wl, i);
+                        if (sr >= s_end || fe >= nfe) continue;
+                        if (W == 2) reinterpret_cast<__half2*>(G.dfeat)[(int64_t)(fe >> 1) * in.S + sr] = __floats2half2_rn(d[i], d[i + 1]);
+                        else {
+                            G.dfeat[((int64_t)(fe / W) * in.S + sr) * W + (fe % W)] = __float2half_rn(d[i]);
+                            if (fe + 1 < nfe) G.dfeat[((int64_t)((fe + 1) / W) * in.S + sr) * W + ((fe + 1) % W)] = __float2half_rn(d[i + 1]);
                         }
                     }
-                }
+                });
             } else {
                 // hidden layer input: apply relu' from the retained activation tile, write the next dY (Np[l-1] == Kp[l])
-                const uint8_t* xt = sub + m.tile_off[l];
-                const int Kp = m.Kp[l];
-                for (int cc = c.h * 32; cc < Kp; cc += 64) {
-                    float v[32];
-                    const int nq = (Kp - cc >= 32) ? 4 : 2;
-                    if (nq == 4) tc_ld32(trow + cc, v); else tc_ld16(trow + cc, v);
+                const uint8_t* xt = c.sub + m.tile_off[l];
+                tc_chain_n<0, 1>(c, N, da, db, Np / 16, (2 * TC_SLAB) >> 4, 256 >> 4, nullptr, [&](auto& d) {
+                    constexpr int NR = sizeof(d) / sizeof(float);
+                    const __half2 z2 = __float2half2_rn(0.0f);
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) {
-                        if (q >= nq) break;
+                    for (int i = 0; i < NR; i += 2) {
+                        const int row = tc_frag_row(c.wl, i), col = tc_frag_col(c.wl, i);
+                        const int off = (col >> 3) * TC_SLAB + row * 16 + (col & 7) * 2;
                         // relu'(x) as a 16-bit lane mask of the retained fp16 activation (>= 0 by construction)
-                        const uint4 a = *reinterpret_cast<const uint4*>(xt + ((cc >> 3) + q) * 2048 + c.r * 16);
-                        const __half2 z2 = __float2half2_rn(0.0f);
-                        uint4 o;
-                        o.x = tc_pack2(v[q * 8], v[q * 8 + 1]) & __hgt2_mask(*reinterpret_cast<const __half2*>(&a.x), z2);
-                        o.y = tc_pack2(v[q * 8 + 2], v[q * 8 + 3]) & __hgt2_mask(*reinterpret_cast<const __half2*>(&a.y), z2);
-                        o.z = tc_pack2(v[q * 8 + 4], v[q * 8 + 5]) & __hgt2_mask(*reinterpret_cast<const __half2*>(&a.z), z2);
-                        o.w = tc_pack2(v[q * 8 + 6], v[q * 8 + 7]) & __hgt2_mask(*reinterpret_cast<const __half2*>(&a.w), z2);
-                        *reinterpret_cast<uint4*>(dyt + ((cc >> 3) + q) * 2048 + c.r * 16) = o;
+                        const uint32_t a = *reinterpret_cast<const uint32_t*>(xt + off);
+                        *reinterpret_cast<uint32_t*>(dyt + off) = tc_pack2(d[i], d[i + 1]) & __hgt2_mask(*reinterpret_cast<const __half2*>(&a), z2);
                     }
-                }
+                });
             }
         }
     }
-    // ---- flush weight / bias gradient accumulators (TMEM rows = input feature, row Kp = bias) ----
-    tc_fence_before();
+    // ---- flush the weight / bias gradient accumulators of every group ----
     __syncthreads();
-    tc_fence_after();
-    if (threadIdx.x < 128) {
-        const int row = threadIdx.x;
-        const uint32_t tr = c.tmem + ((uint32_t)c.laneq << 16);
-        for (int l = 0; l < nl; ++l) {
-            float* gbase = l < m.nl_d ? G.gdens : G.gcol;
-            const int I = m.I[l], O = m.O[l];
-            // all 32 lanes of a warp must execute tcgen05.ld: decide per warp, predicate the stores per lane
-            const int wrow0 = row & ~31;
-            if (wrow0 > m.Kp[l]) continue;
-            for (int cc = 0; cc < m.Np[l]; cc += 16) {
-                float v[16]; tc_ld16(tr + m.acc_col[l] + cc, v);
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int o = cc + j;
-                    if (o >= O) continue;
-                    const float val = v[j] * inv_scale;
-                    if (row < I) { if (val != 0.0f) atomicAdd(gbase + m.src_w[l] + o * I + row, val); }
-                    else if (row == m.Kp[l] && m.src_b[l] >= 0) atomicAdd(gbase + m.src_b[l] + o, val);
-                }
-            }
+    for (int l = 0; l < nl; ++l) {
+        if (m.acc_l[l] < 0) continue;
+        float* gbase = l < m.nl_d ? G.gdens : G.gcol;
+        const int I = m.I[l], O = m.O[l];
+        for (int e = threadIdx.x; e < O * (I + 1); e += blockDim.x) {
+            float v = 0.0f;
+            for (int gi = 0; gi < NG; ++gi) v += reinterpret_cast<const float*>(smem + gi * m.group_bytes + m.acc_off)[m.acc_l[l] + e];
+            const int o = e / (I + 1), i = e % (I + 1);
+            const float val = v * inv_scale;
+            if (i < I) { if (val != 0.0f) atomicAdd(gbase + m.src_w[l] + o * I + i, val); }
+            else if (m.src_b[l] >= 0) atomicAdd(gbase + m.src_b[l] + o, val);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (threadIdx.x < 32) tc_tmem_dealloc(c.tmem, (uint32_t)m.tmem_cols);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1212,11 +1043,9 @@ wb_featx_scatter_kernel(WbGridX gx, TcIn in, const __half* __restrict__ dfeat, i
     }
 }
 
-#include "wb_shade_tc_bwd3.cuh"          // three-group variant: the default for the app/nerf decoder shape (WB_TC_BWD_GROUPS=2 selects the kernel above)
-
 // decoder backward only: dL/d(shaded) -> weight gradients + dL/dfeat planes in the workspace
-// grad_table != NULL asks for the table scatter to be fused into the decoder backward; *fused_out reports whether it was (it is for the
-// app/nerf shape: F == 2 'cat' hash grid, three-group kernel) -- otherwise the caller runs wb_tc_table_scatter afterwards
+// grad_table != NULL asks for the table scatter to be fused into the decoder backward; *fused_out reports whether it was (it is for
+// F == 2 'cat' hash grids) -- otherwise the caller runs wb_tc_table_scatter afterwards
 int wb_tc_decoder_bwd_ex(const wb_nef_desc* nef, const float* blob, const wb_rays* rays, const float* rec_t, const int32_t* rec_ray,
                          int64_t S, const float* g_shaded, const float* scale, const void* feat_saved, void* workspace,
                          float* grad_dens, float* grad_col, float* grad_table, int* fused_out, cudaStream_t st);
@@ -1226,6 +1055,20 @@ int wb_tc_decoder_bwd(const wb_nef_desc* nef, const float* blob, const wb_rays* 
 {
     return wb_tc_decoder_bwd_ex(nef, blob, rays, rec_t, rec_ray, S, g_shaded, scale, feat_saved, workspace, grad_dens, grad_col, nullptr, nullptr, st);
 }
+
+// the launches of one decoder backward: layer masks of the weight-grad accumulators that fit beside the tiles, and the group count
+static int tc_bwd_passes(WbTc* m, unsigned masks[TC_ML])
+{
+    const int nl = m->nl_d + m->nl_c;
+    int n = 0; unsigned cur = 0;
+    for (int l = 0; l < nl; ++l) {
+        if (cur && !tc_bwd_layout(m, cur | (1u << l), 1)) { masks[n++] = cur; cur = 0; }
+        cur |= 1u << l;
+    }
+    masks[n++] = cur;
+    return n;
+}
+
 int wb_tc_decoder_bwd_ex(const wb_nef_desc* nef, const float* blob, const wb_rays* rays, const float* rec_t, const int32_t* rec_ray,
                          int64_t S, const float* g_shaded, const float* scale, const void* feat_saved, void* workspace,
                          float* grad_dens, float* grad_col, float* grad_table, int* fused_out, cudaStream_t st)
@@ -1242,45 +1085,38 @@ int wb_tc_decoder_bwd_ex(const wb_nef_desc* nef, const float* blob, const wb_ray
     TcIn in = { rays->origins, rays->dirs, rec_t, rec_ray, S, reinterpret_cast<const uint4*>(workspace), nullptr, reinterpret_cast<const uint4*>(feat_saved),
                 g_tc_s_begin, g_tc_s_end };
     const int64_t S_launch = (g_tc_s_end ? g_tc_s_end : S) - g_tc_s_begin;
+    if (S_launch <= 0) return WB_OK;
     TcGrads G = { grad_dens, grad_col, scale, dfeat, planes, width };
-    TcB3Plan plan;
-    if ((tc_knob_bwd_groups() == 3 || !m.fits2) && tc_b3_plan(m, &plan)) {     // wb_shade_tc_bwd3.cuh: three sub-tile groups per SM (4.53 -> 3.69 ms measured),
-        WbGrid g; memset(&g, 0, sizeof(g));                                     // or one 128-wide group (hidden_dim = 128)
-        const int wide = plan.groups == 1 ? 1 : 0;
-        // one wide group per SM: the fused scatter has only 8 warps to issue from and measured slower than the stand-alone scatter kernel
-        // (16.0 vs 13.7 ms at hidden_dim 128 on the 1024^2 frame), so it is opt-in there (WB_TC_FUSE_SCATTER_WIDE=1)
-        const bool fuse = grad_table != nullptr && tc_knob_fuse_scatter() && nef->grid_kind == 0 && nef->feature_dim == 2 && nef->multiscale == 0 &&
-                          planes <= 16 && (!wide || tc_knob_fuse_scatter_wide());
+    unsigned masks[TC_ML];
+    const int npass = tc_bwd_passes(&m, masks);
+    for (int p = 0; p < npass; ++p) {
+        tc_bwd_layout(&m, masks[p], 1);
+        // two groups per CTA where they fit (the groups overlap each other's barrier and MMA latencies)
+        if (tc_knob_bwd_groups() >= 2) { WbTc m2 = m; if (tc_bwd_layout(&m2, masks[p], 2)) m = m2; }
+        const bool emit = p == npass - 1;
+        // fused table scatter: F == 2 'cat' hash grids with <= 16 live LODs (32 features: the scratch tile); with one group per SM
+        // only on request (WB_TC_FUSE_SCATTER_WIDE=1): the stand-alone scatter kernel runs beside the decoder CTAs instead
+        const bool fuse = emit && grad_table != nullptr && tc_knob_fuse_scatter() && nef->grid_kind == 0 && nef->feature_dim == 2 &&
+                          nef->multiscale == 0 && planes <= 16 && (m.groups > 1 || tc_knob_fuse_scatter_wide());
+        WbGrid g; memset(&g, 0, sizeof(g));
         if (fuse) { rc = wb_make_grid(nef, &g); if (rc) return rc; }
-        const int fmode = !fuse ? 0 : (tc_knob_fuse_scatter() == 2 ? 2 : (tc_knob_fuse_scatter() == 3 && !wide) ? 3 : 1);
-        auto kern3 = wide ? (fmode == 2 ? wb_mlp_bwd3_tc_kernel<2, 1> : fmode ? wb_mlp_bwd3_tc_kernel<1, 1> : wb_mlp_bwd3_tc_kernel<0, 1>)
-                          : fmode == 3 ? wb_mlp_bwd3_tc_kernel<3, 3> : fmode == 2 ? wb_mlp_bwd3_tc_kernel<2, 3> : fmode == 1 ? wb_mlp_bwd3_tc_kernel<1, 3> : wb_mlp_bwd3_tc_kernel<0, 3>;
-        static int64_t done3[2][4] = { { -1, -1, -1, -1 }, { -1, -1, -1, -1 } };
-        if (done3[wide][fmode] != WB_ATTR_KEY(plan.smem_bytes)) {
-            WB_CUDA(cudaFuncSetAttribute(kern3, cudaFuncAttributeMaxDynamicSharedMemorySize, plan.smem_bytes));
-            done3[wide][fmode] = WB_ATTR_KEY(plan.smem_bytes);
+        auto kern = m.groups == 2 ? (fuse ? wb_mlp_bwd_tc_kernel<2, true> : wb_mlp_bwd_tc_kernel<2, false>)
+                                  : (fuse ? wb_mlp_bwd_tc_kernel<1, true> : wb_mlp_bwd_tc_kernel<1, false>);
+        {
+            static int64_t done_for[2][2] = { { -1, -1 }, { -1, -1 } };
+            int64_t& done = done_for[m.groups - 1][fuse ? 1 : 0];
+            if (done != WB_ATTR_KEY(TC_SMEM_MAX)) {        // the passes of one call differ in size: allow the largest once
+                WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
+                done = WB_ATTR_KEY(TC_SMEM_MAX);
+            }
         }
-        const int64_t nctas3 = ((S_launch + TC_ROWS - 1) / TC_ROWS + plan.groups - 1) / plan.groups;
-        int64_t grid3 = (int64_t)wb_num_sms(); if (grid3 > nctas3) grid3 = nctas3;
-        kern3<<<(unsigned)grid3, plan.groups * TC_GROUP, plan.smem_bytes, st>>>(m, plan, reinterpret_cast<const uint8_t*>(blob), in,
-                                                                          reinterpret_cast<const float4*>(g_shaded), G, g, grad_table);
+        const int64_t nctas = ((S_launch + g_tc_s_begin % TC_ROWS + TC_ROWS - 1) / TC_ROWS + m.groups - 1) / m.groups;
+        int64_t grid = (int64_t)wb_num_sms(); if (grid > nctas) grid = nctas;         // 1 CTA / SM: shared memory holds the tiles and accumulators
+        kern<<<(unsigned)grid, m.groups * TC_GROUP, m.smem_bytes, st>>>(m, reinterpret_cast<const uint8_t*>(blob), in,
+                                                                        reinterpret_cast<const float4*>(g_shaded), G, masks[p], emit ? 1 : 0, g, grad_table);
         WB_LAUNCH_CHECK();
         if (fuse && fused_out) *fused_out = 1;
-        return WB_OK;
     }
-    WB_CHECK_ARG(m.fits2, "tensor-core path: decoder backward does not fit in shared memory (use precision 0)");
-    {
-        static int64_t done_for = -1;
-        if (done_for != WB_ATTR_KEY(m.smem_bytes)) {
-            WB_CUDA(cudaFuncSetAttribute(wb_mlp_bwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, m.smem_bytes));
-            done_for = WB_ATTR_KEY(m.smem_bytes);
-        }
-    }
-    const int64_t nctas = ((S + TC_ROWS - 1) / TC_ROWS + TC_BWD_GROUPS - 1) / TC_BWD_GROUPS;
-    int64_t grid = (int64_t)wb_num_sms(); if (grid > nctas) grid = nctas;         // 1 CTA / SM: TMEM holds the weight-grad accumulators
-    wb_mlp_bwd_tc_kernel<<<(unsigned)grid, TC_BWD_GROUPS * TC_GROUP, m.smem_bytes, st>>>(m, reinterpret_cast<const uint8_t*>(blob), in,
-                                                                           reinterpret_cast<const float4*>(g_shaded), G);
-    WB_LAUNCH_CHECK();
     return WB_OK;
 }
 // table scatter only: dL/dfeat planes (written by wb_tc_decoder_bwd into the same workspace) -> grad_table
@@ -1340,11 +1176,16 @@ int wb_tc_shade_bwd(const wb_nef_desc* nef, const float* blob, const wb_rays* ra
                     float* grad_table, float* grad_dens, float* grad_col, cudaStream_t st)
 {
     {
-        WbTc m; TcB3Plan plan;
+        WbTc m; unsigned masks[TC_ML];
         int chunks = tc_knob_wide_chunks(); if (chunks > 16) chunks = 16;
         TcSide* side = nullptr;
-        if (chunks > 1 && S >= tc_knob_wide_min_s() && nef->grid_kind == 0 && grad_table && wb_tc_make(nef, true, &m) == WB_OK && !m.fits2 &&
-            tc_b3_plan(m, &plan) && plan.groups == 1 && !tc_knob_fuse_scatter_wide() && (side = tc_side_stream()) != nullptr) {
+        bool wide = false;         // one group per SM (wide decoders): the decoder backward leaves most warp slots idle
+        if (chunks > 1 && S >= tc_knob_wide_min_s() && nef->grid_kind == 0 && grad_table && wb_tc_make(nef, true, &m) == WB_OK) {
+            tc_bwd_passes(&m, masks);
+            tc_bwd_layout(&m, masks[0], 1);
+            wide = !(tc_knob_bwd_groups() >= 2 && tc_bwd_layout(&m, masks[0], 2));
+        }
+        if (wide && !tc_knob_fuse_scatter_wide() && (side = tc_side_stream()) != nullptr) {
             const int64_t per = ((S + chunks - 1) / chunks + TC_ROWS - 1) / TC_ROWS * TC_ROWS;
             int rc = WB_OK, c = 0;
             for (int64_t s0 = 0; s0 < S && rc == WB_OK; s0 += per, ++c) {

@@ -1,12 +1,13 @@
 #!/usr/bin/env python
-"""Build oracle/_ref/libwisp_ref_kernels.so from the REFERENCE's own CUDA sources (TEST INFRASTRUCTURE; build container only).
+"""Build oracle/_ref/libwisp_ref_kernels.so from the REFERENCE's own CUDA sources (TEST INFRASTRUCTURE; needs a kaolin-wisp checkout).
 
-    python oracle/ref_kernels/build_ref.py        (also called by __graft_entry__.build() when /root/reference exists)
+    python oracle/ref_kernels/build_ref.py        (also called by __graft_entry__.build() when the checkout exists)
 
-Compiles, where they lie under /root/reference/wisp/csrc, with nvcc for sm_100a against this image's torch headers:
+Compiles, where they lie under the checkout's wisp/csrc, with nvcc for sm_90a against the installed torch headers:
     ops/hashgrid_interpolate.cpp, ops/hashgrid_interpolate_cuda.cu, ops/uniform_sample.cpp, ops/uniform_sample_cuda.cu,
     render/find_depth_bound.cpp, render/find_depth_bound_cuda.cu
-plus oracle/ref_kernels/ref_shim.cpp (C entry points), and links them into oracle/_ref/ (git-ignored, shipped to the GPU box by gpurun).
+plus oracle/ref_kernels/ref_shim.cpp (C entry points), and links them into oracle/_ref/ (git-ignored).  oracle/make_ref_golden.py runs them once
+to store what tests/test_gpu_ref_kernels.py compares against under tests/golden/.
 No reference source enters the repository.  One deviation, as SURVEY.md 8(c) found: hashgrid_interpolate_cuda.cu does not compile
 against torch >= 2.x because `AT_DISPATCH_*(tensor.type(), ...)` no longer converts (lines 358, 375, 413, 433); the recipe compiles a
 TEMPORARY copy (under /tmp, deleted afterwards) in which `.type()` inside those dispatch macros reads `.scalar_type()` -- a one-token
@@ -28,7 +29,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 def build(force: bool = False) -> str:
     if not os.path.isdir(REF):
-        raise RuntimeError("the reference checkout is not present (GPU box): the prebuilt oracle/_ref library is used as is")
+        raise RuntimeError("the reference checkout is not present")
     srcs = ["ops/hashgrid_interpolate.cpp", "ops/hashgrid_interpolate_cuda.cu", "ops/uniform_sample.cpp", "ops/uniform_sample_cuda.cu",
             "render/find_depth_bound.cpp", "render/find_depth_bound_cuda.cu"]
     deps = [os.path.join(REF, s) for s in srcs] + [os.path.join(HERE, "ref_shim.cpp"), os.path.abspath(__file__)]
@@ -37,7 +38,7 @@ def build(force: bool = False) -> str:
     import torch
     ti = os.path.join(os.path.dirname(torch.__file__), "include")
     tl = os.path.join(os.path.dirname(torch.__file__), "lib")
-    flags = ["-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "-O2", "-Xcompiler", "-fPIC", "-DWITH_CUDA",
+    flags = ["-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O2", "-Xcompiler", "-fPIC", "-DWITH_CUDA",
              f"-D_GLIBCXX_USE_CXX11_ABI={int(torch._C._GLIBCXX_USE_CXX11_ABI)}", "-I", ti, "-I", os.path.join(ti, "torch", "csrc", "api", "include"),
              "-I", os.path.join(REF, "ops"), "-I", os.path.join(REF, "render"), "-w"]
     os.makedirs(OUT_DIR, exist_ok=True)

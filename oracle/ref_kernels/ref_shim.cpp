@@ -1,6 +1,6 @@
 // ref_shim.cpp -- TEST INFRASTRUCTURE.  C entry points around the REFERENCE's own CUDA operators (compiled from the sources under
-// /root/reference/wisp/csrc by oracle/ref_kernels/build_ref.py into oracle/_ref/libwisp_ref_kernels.so), so that the GPU tests can put
-// this repository's kernels side by side with the kernels they replace, on the B200:
+// a kaolin-wisp checkout's wisp/csrc by oracle/ref_kernels/build_ref.py into oracle/_ref/libwisp_ref_kernels.so), so that
+// oracle/make_ref_golden.py can store what the kernels this repository replaces compute, for the GPU tests:
 //   wisp::hashgrid_interpolate_cuda / _backward_cuda   (wisp/csrc/ops/hashgrid_interpolate.cpp:46-105, hashgrid_interpolate_cuda.cu)
 //   wisp::uniform_sample_cuda                          (wisp/csrc/ops/uniform_sample.cpp:28-42, uniform_sample_cuda.cu)
 //   wisp::find_depth_bound_cuda                        (wisp/csrc/render/find_depth_bound.cpp:23-36, find_depth_bound_cuda.cu)

@@ -77,14 +77,15 @@ def _run_variant(hidden: str, knobs: dict):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("knob", ["WB_TC_FWD_TMEMA=0,WB_TC_BWD_GROUPS=2", "WB_TC_WIDE_MIN_S=1000:128", "WB_TC_FUSE_SCATTER_WIDE=1:128"])
+@pytest.mark.parametrize("knob", ["WB_TC_FUSE_SCATTER=0,WB_TC_BWD_GROUPS=1", "WB_TC_WIDE_MIN_S=1000:128", "WB_TC_FUSE_SCATTER_WIDE=1:128"])
 def test_kernel_variant_matches_default(knob):
-    """Default kernels (TMEM-A forward, three-group decoder backward: validated and faster on B200 in round 2) against the
-    round-1 kernels they replaced, which stay selectable through the knobs (forward and backward variant in ONE run: they are
-    different kernels).  The knobs are read once per process, hence the subprocesses: same samples, rgb within fp16 round-off of
-    each other, gradients within the precision-1 tolerance.
-    ':128' runs the case with hidden_dim = 128 (the one-group backward): its chunked schedule (decoder backward of chunk c+1 beside
-    the table scatter of chunk c, normally only above 2^20 samples) against the single launch pair, and its fused-scatter variant."""
+    """Default kernels (two-group decoder backward with the hash-table scatter fused into its last epilogue) against the variants
+    the knobs select (one group per CTA, separate scatter kernel: different kernels in ONE run).  The knobs are read once per
+    process, hence the subprocesses: same samples, rgb within fp16 round-off of each other, gradients within the precision-1
+    tolerance.
+    ':128' runs the case with hidden_dim = 128 (one group per CTA, weight gradients over two passes): its chunked schedule (decoder
+    backward of chunk c+1 beside the table scatter of chunk c, normally only above 2^20 samples) against the single launch pair,
+    and its fused-scatter variant."""
     knob, _, hidden = knob.partition(":")
     if hidden not in _VARIANT_DEFAULTS:
         _VARIANT_DEFAULTS[hidden] = _run_variant(hidden, {})

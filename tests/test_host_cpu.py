@@ -1,6 +1,6 @@
 """CPU tests of the product's host side: the C-ABI library loads and exports every symbol include/wispb200.h declares,
 the ctypes struct layouts match the header, the host-side SPC builder matches the oracle, and compute entry points
-refuse to run without a B200 (no CPU fallback)."""
+refuse to run without an H100 (no CPU fallback)."""
 import ctypes as C
 import os
 import re
