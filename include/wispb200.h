@@ -340,7 +340,13 @@ int wb_rf_loss_scale(const float* absmax, float* scale, wb_stream s);
 
 /* The two stages of the precision-1 backward, callable separately (wb_rf_shade_bwd runs them back to back):
  * wb_rf_decoder_bwd writes the weight gradients and leaves dL/dfeat (fp16 planes) in the workspace; wb_rf_table_scatter
- * turns those planes into hash-table updates with warp-level merging of samples that share a cell. */
+ * turns those planes into hash-table updates with warp-level merging of samples that share a cell.
+ * Workspace layout (bytes), R rays, S samples, Kc = width of the colour-decoder input rounded up to 16:
+ *   [0, R * Kc * 2)                     per-ray colour-input rows, fp16 [R][Kc] (view embedding at features dout-1 .., zeros)
+ *   [align256(R * Kc * 2), + P * S * F * 2)  dL/dfeat, fp16 [P][S][F], still multiplied by the loss scale; F = feature_dim,
+ *                                       P = one plane per live LOD ('cat': min(lod_idx, num_lods)) or 1 ('sum').
+ * feat_saved (wb_rf_shade_fwd's feat_save): the density-decoder input rows, fp16, chunk-major [Kp0 / 8][S] x 8 features
+ *   (Kp0 = its width rounded up to 16): grid features, then the position embedding, then zeros. */
 int wb_rf_decoder_bwd(const wb_nef_desc* nef, const float* blob, const wb_rays* rays, const float* rec_t, const int32_t* rec_ray,
                       int64_t S, const float* g_shaded, const float* loss_scale, const void* feat_saved, void* workspace,
                       float* grad_dens, float* grad_col, wb_stream s);
@@ -411,9 +417,11 @@ int wb_prune_samples(const int16_t* points, int64_t N, int32_t level, const floa
 int wb_prune_update(const float* shaded, int64_t N, float decay, float min_density, float* occupancy, uint8_t* keep, wb_stream s);
 
 /* ------------------------------------------------------------------------------------------------
- * Diagnostics: one-tile tcgen05 GEMM that pins the shared-memory operand layouts of the tensor-core decoder
- * kernels (csrc/wb_tc.cuh).  a_img / b_img are byte images of the operand tiles; D is [128, N] fp32.
- * mode 0: D = A[128xK] . W[NxK]^T   mode 1: D = A[128xK] . W[KxN]   mode 2: D = A[128x128]^T . B[128xN]
+ * Diagnostics: one-tile wgmma GEMM that pins the shared-memory operand layouts of the tensor-core decoder
+ * kernels (csrc/wb_tc.cuh).  a_img / b_img are byte images of the operand tiles (R = 128 sample rows, or 64 -- the
+ * decoder kernels' tile -- when mode has bit 4 set); D is fp32, [R, N] for modes 0 / 1 and [128, N] for mode 2.
+ * mode 0: D = A[RxK] . W[NxK]^T   mode 1: D = A[RxK] . W[KxN]   mode 2: D = A[Rx128]^T . B[RxN]
+ * N = 8 or a multiple of 16 up to 128.
  * ---------------------------------------------------------------------------------------------- */
 int wb_tc_selftest(const void* a_img, int a_bytes, const void* b_img, int b_bytes, float* D, int N, int K, int mode, wb_stream s);
 

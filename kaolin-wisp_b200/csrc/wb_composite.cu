@@ -258,9 +258,13 @@ extern "C" int wb_composite_bwd_loss(const float* shaded, const float* depth, co
 __global__ void wb_loss_scale_kernel(const float* __restrict__ absmax, float* __restrict__ scale)
 {
     const float amax = fmaxf(*absmax, 1e-30f);
-    float k = floorf(log2f(64.0f / amax));
-    k = fminf(fmaxf(k, -20.0f), 60.0f);
-    *scale = __int_as_float(((int)k + 127) << 23);
+    // floor(log2(64 / amax)) = 6 - ceil(log2(amax)), from the exponent: amax = f * 2^e with f in [0.5, 1).  (log2f(64.0f / amax)
+    // rounds to the next integer for amax just above a power of two and gives a scale twice too large.)
+    int e;
+    const float f = frexpf(amax, &e);
+    int k = isinf(amax) ? -20 : 6 - (f == 0.5f ? e - 1 : e);
+    k = min(max(k, -20), 60);
+    *scale = __int_as_float((k + 127) << 23);
 }
 extern "C" int wb_rf_loss_scale(const float* absmax, float* scale, wb_stream s)
 {

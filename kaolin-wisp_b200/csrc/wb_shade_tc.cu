@@ -271,13 +271,17 @@ __device__ __forceinline__ void tile_embed(uint8_t* tile, int r, int f0, int mod
     }
 }
 // hash-grid gather of one sample -> features [0, feat_dim) of the X0 tile (fp32 blend, fp16 store)
-// `half` (0/1): the two threads of a row split the work -- slab (4 LODs) k goes to half k & 1 on the F == 2 'cat' path, the
-// generic paths are done by half 0 alone
+// `half` (0/1): the two threads of a row split the work -- slab (4 LODs) k goes to half k & 1 on the F == 2 'cat' path, except a
+// partial last slab (L % 4 != 0), which goes to half 0: its zero-filled tail holds the first features of the position embedding,
+// which half 0 writes after the gather, so the two halves store disjoint bytes.  The generic paths are done by half 0 alone.
 __device__ __forceinline__ void tile_gather(const WbGrid& g, uint8_t* tile, int r, int half, float px, float py, float pz)
 {
     const int L = g.L, F = g.F;
     if (g.multiscale == 0 && F == 2) {
-        for (int l0 = 4 * half; l0 < L; l0 += 8) {              // 4 levels = 8 features = one slab row (16 B store)
+        const int nslab = (L + 3) >> 2, partial = (L & 3) ? nslab - 1 : -1;
+        for (int sl = 0; sl < nslab; ++sl) {                    // 4 levels = 8 features = one slab row (16 B store)
+            if ((sl == partial ? 0 : (sl & 1)) != half) continue;
+            const int l0 = 4 * sl;
             float v[8];
 #pragma unroll
             for (int q = 0; q < 4; ++q) {

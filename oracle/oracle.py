@@ -253,16 +253,19 @@ class Nef:
 
 def make_nef(num_lods=16, feature_dim=2, codebook_bitwidth=19, min_res=16, max_res=512, hidden_dim=64,
              num_layers=1, bias=True, multiscale="cat", view_freq=4, seed=0, feature_std=1e-4,
-             table_scale: Optional[float] = None) -> Nef:
+             table_scale: Optional[float] = None, pos_mode=0, pos_freq=0, view_mode=3) -> Nef:
     """Random-init NeuralRadianceField in the shape of app/nerf/configs/nerf_hash.yaml.
-    nn.Linear default init (kaiming-uniform, bound 1/sqrt(fan_in)); density lout.bias[0]=1 (nerf.py:162-163)."""
+    nn.Linear default init (kaiming-uniform, bound 1/sqrt(fan_in)); density lout.bias[0]=1 (nerf.py:162-163).
+    Embedders (nerf.py:103-106): pos_mode 0 none, 1 identity, 2 positional, 3 positional + input (pos_freq bands);
+    view_mode 0 none, 1 identity, 3 positional + input (view_freq bands)."""
     rng = np.random.default_rng(seed)
     res = geometric_resolutions(num_lods, min_res, max_res)
     begin = table_layout(res, codebook_bitwidth)
     std = feature_std if table_scale is None else table_scale
     table = (rng.standard_normal((int(begin[-1]), feature_dim)) * std).astype(np.float32)
-    feat = num_lods * feature_dim if multiscale == "cat" else feature_dim
-    view_dim = 3 + 6 * view_freq
+    embed_dim = lambda mode, freq: 0 if mode == 0 else 3 if mode == 1 else 6 * freq if mode == 2 else 3 + 6 * freq
+    feat = (num_lods * feature_dim if multiscale == "cat" else feature_dim) + embed_dim(pos_mode, pos_freq)
+    view_dim = embed_dim(view_mode, view_freq)
 
     def linear(i, o):
         bound = 1.0 / np.sqrt(i)
@@ -282,7 +285,7 @@ def make_nef(num_lods=16, feature_dim=2, codebook_bitwidth=19, min_res=16, max_r
     db[-1][0] = 1.0
     cW, cb = mlp(15 + view_dim, 3, num_layers + 1)
     return Nef(res, feature_dim, codebook_bitwidth, table, dW, db if bias else None, cW, cb if bias else None,
-               multiscale=multiscale, view_mode=3, view_freq=view_freq)
+               multiscale=multiscale, pos_mode=pos_mode, pos_freq=pos_freq, view_mode=view_mode, view_freq=view_freq)
 
 
 # ----------------------------------------------------------------------------------------------

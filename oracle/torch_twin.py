@@ -135,13 +135,17 @@ def pack_index(boundary: torch.Tensor) -> torch.Tensor:
 
 
 def cumsum_pack(x: torch.Tensor, boundary: torch.Tensor, exclusive: bool) -> torch.Tensor:
-    """[KAOLIN-EXT] spc_render.cumsum: segmented prefix sum."""
+    """[KAOLIN-EXT] spc_render.cumsum: segmented prefix sum, restarted at every pack.  Formed as a running sum over all packs minus
+    the sum before the pack, in float64 and rounded once: in float32 every pack would inherit the rounding error of the running
+    sum of all the packs before it (the reference sums each pack on its own), and that error would depend on how the CPU's
+    torch.cumsum orders its additions."""
     pid = pack_index(boundary)
-    cs = torch.cumsum(x, 0)
+    xd = x.double()
+    cs = torch.cumsum(xd, 0)
     starts = torch.nonzero(boundary)[:, 0]
-    base = torch.cat([torch.zeros(1, x.shape[1]), cs])[starts]     # cumsum before each pack
+    base = torch.cat([torch.zeros(1, x.shape[1], dtype=torch.float64), cs])[starts]     # cumsum before each pack
     out = cs - base[pid]
-    return out - x if exclusive else out
+    return (out - xd if exclusive else out).to(x.dtype)
 
 
 def sum_reduce(x: torch.Tensor, boundary: torch.Tensor) -> torch.Tensor:

@@ -449,11 +449,20 @@ SHAPES = [dict(num_lods=8, feature_dim=4, codebook_bitwidth=14, min_res=8, max_r
           # one-group tensor-core backward (mixed accumulator orientation), with the fused table scatter (F = 2 'cat') and without it
           dict(num_lods=16, feature_dim=2, codebook_bitwidth=14, min_res=16, max_res=256, hidden_dim=128, multiscale="cat", view_freq=4, bias=True),
           dict(num_lods=8, feature_dim=4, codebook_bitwidth=13, min_res=8, max_res=128, hidden_dim=128, multiscale="cat", view_freq=2, bias=True),
-          dict(num_lods=16, feature_dim=2, codebook_bitwidth=14, min_res=16, max_res=256, hidden_dim=128, multiscale="cat", view_freq=4, bias=False)]
+          dict(num_lods=16, feature_dim=2, codebook_bitwidth=14, min_res=16, max_res=256, hidden_dim=128, multiscale="cat", view_freq=4, bias=False),
+          # position embeddings (positional + input, identity) and the identity view embedding; F = 2 'cat' with L = 6 puts the position
+          # embedding in the same 16-byte slab row as the last grid features
+          dict(num_lods=8, feature_dim=2, codebook_bitwidth=13, min_res=8, max_res=128, hidden_dim=64, multiscale="cat", view_freq=4, bias=True,
+               pos_mode=3, pos_freq=3),
+          dict(num_lods=6, feature_dim=4, codebook_bitwidth=12, min_res=8, max_res=96, hidden_dim=32, multiscale="sum", view_freq=0, bias=True,
+               pos_mode=1, view_mode=1),
+          dict(num_lods=6, feature_dim=2, codebook_bitwidth=12, min_res=8, max_res=96, hidden_dim=32, multiscale="cat", view_freq=2, bias=True,
+               pos_mode=3, pos_freq=2)]
 
 
 @pytest.mark.parametrize("precision", [0, 1])
-@pytest.mark.parametrize("shape", SHAPES, ids=lambda c: f"F{c['feature_dim']}{c['multiscale']}L{c['num_lods']}h{c['hidden_dim']}")
+@pytest.mark.parametrize("shape", SHAPES, ids=lambda c: f"F{c['feature_dim']}{c['multiscale']}L{c['num_lods']}h{c['hidden_dim']}"
+                         + (f"pos{c['pos_mode']}" if c.get('pos_mode') else "") + (f"view{c['view_mode']}" if 'view_mode' in c else ""))
 def test_trace_other_shapes_vs_oracle(W, shape, precision):
     """Feature widths 2/4/8, 'cat' and 'sum', decoder widths that are not powers of two, no bias: the generic gather / scatter paths
     of the fused kernels (the app/nerf shape takes the specialised F == 2 'cat' path), forward + backward vs the oracle."""
@@ -506,10 +515,10 @@ def test_no_rays_and_no_hits(W):
 # tensor-core operand layouts (csrc/wb_tc.cuh)
 # ---------------------------------------------------------------------------------------------------------------
 def slab_image(X):
-    """[128, C] -> byte image: element (s, f) at (f/8)*2048 + s*16 + (f%8)*2."""
+    """[R, C] -> byte image: element (s, f) at (f/8)*(R*16) + s*16 + (f%8)*2."""
     S, Cc = X.shape
-    assert S == 128 and Cc % 8 == 0
-    return np.ascontiguousarray(X.astype(np.float16).reshape(128, Cc // 8, 8).transpose(1, 0, 2)).view(np.uint8).reshape(-1)
+    assert S in (64, 128) and Cc % 8 == 0
+    return np.ascontiguousarray(X.astype(np.float16).reshape(S, Cc // 8, 8).transpose(1, 0, 2)).view(np.uint8).reshape(-1)
 
 
 def weight_image(Wm):
@@ -518,26 +527,71 @@ def weight_image(Wm):
     return np.ascontiguousarray(Wm.astype(np.float16).reshape(N, K // 8, 8).transpose(1, 0, 2)).view(np.uint8).reshape(-1)
 
 
-@pytest.mark.parametrize("mode,N,K", [(0, 64, 32), (0, 16, 64), (0, 64, 48), (1, 48, 64), (1, 32, 64), (1, 64, 16), (2, 64, 128), (2, 16, 128)])
-def test_tcgen05_operand_layouts(W, mode, N, K):
+def _selftest(W, mode, rows, N, K, a, b):
     import ctypes as C
-    rng = np.random.default_rng(mode * 100 + N)
-    q = lambda a: a.astype(np.float16).astype(np.float32)
-    if mode == 0:
-        X, Wm = q(rng.standard_normal((128, K))), q(rng.standard_normal((N, K)))
-        a, b, ref = slab_image(X), weight_image(Wm), X @ Wm.T
-    elif mode == 1:
-        dY, Wm = q(rng.standard_normal((128, K))), q(rng.standard_normal((K, N)))      # W: out=K rows, in=N cols
-        a, b, ref = slab_image(dY), weight_image(Wm), dY @ Wm
-    else:
-        X, dY = q(rng.standard_normal((128, 128))), q(rng.standard_normal((128, N)))
-        a, b, ref = slab_image(X), slab_image(dY), X.T @ dY
-    D = torch.zeros((128, N), dtype=torch.float32, device="cuda")
+    D = torch.zeros((128 if mode == 2 else rows, N), dtype=torch.float32, device="cuda")
     ta, tb = dev(a), dev(b)
     A = W._cabi
-    A.check(A.lib().wb_tc_selftest(A.ptr(ta), C.c_int(a.size), A.ptr(tb), C.c_int(b.size), A.ptr(D), C.c_int(N), C.c_int(K), C.c_int(mode), A.stream()))
+    m = mode | (4 if rows == 64 else 0)
+    A.check(A.lib().wb_tc_selftest(A.ptr(ta), C.c_int(a.size), A.ptr(tb), C.c_int(b.size), A.ptr(D), C.c_int(N), C.c_int(K), C.c_int(m), A.stream()))
     torch.cuda.synchronize()
-    np.testing.assert_allclose(D.cpu().numpy(), ref, atol=2e-3, rtol=1e-3)
+    return D.cpu().numpy()
+
+
+def _operand_case(W, mode, N, K, rows, seed):
+    rng = np.random.default_rng(seed)
+    q = lambda a: a.astype(np.float16).astype(np.float32)
+    if mode == 0:
+        X, Wm = q(rng.standard_normal((rows, K))), q(rng.standard_normal((N, K)))
+        a, b, ref = slab_image(X), weight_image(Wm), X.astype(np.float64) @ Wm.T
+    elif mode == 1:
+        dY, Wm = q(rng.standard_normal((rows, K))), q(rng.standard_normal((K, N)))      # W: out=K rows, in=N cols
+        a, b, ref = slab_image(dY), weight_image(Wm), dY.astype(np.float64) @ Wm
+    else:
+        X, dY = q(rng.standard_normal((rows, 128))), q(rng.standard_normal((rows, N)))
+        if N == 8:                                              # the constant-one slab: feature 0 = 1, features 1..7 = 0
+            dY[:] = 0.0; dY[:, 0] = 1.0
+        a, b, ref = slab_image(X), slab_image(dY), X.T.astype(np.float64) @ dY
+    np.testing.assert_allclose(_selftest(W, mode, rows, N, K, a, b), ref, atol=2e-3, rtol=1e-3)
+
+
+@pytest.mark.parametrize("mode,N,K", [(0, 64, 32), (0, 16, 64), (0, 64, 48), (1, 48, 64), (1, 32, 64), (1, 64, 16), (2, 64, 128), (2, 16, 128)])
+def test_tcgen05_operand_layouts(W, mode, N, K):
+    """128-row tiles (slab = 2048 bytes, two warpgroups).  The name predates the Hopper port: the self-test runs wgmma."""
+    _operand_case(W, mode, N, K, 128, mode * 100 + N)
+
+
+# the decoder kernels' 64-row tile (slab = 1024 bytes, one warpgroup for modes 0 / 1); N = 80 / 96 / 112: the tc_chain_n instances of
+# 80..112-wide layers; N = 8 (mode 2): the bias-gradient chain
+@pytest.mark.parametrize("mode,N,K", [(0, 80, 96), (0, 96, 128), (0, 112, 32), (0, 128, 112), (0, 16, 16), (0, 64, 48),
+                                      (1, 80, 112), (1, 96, 64), (1, 112, 128), (1, 16, 96), (1, 64, 16),
+                                      (2, 8, 64), (2, 80, 64), (2, 96, 64), (2, 112, 64), (2, 128, 64), (2, 16, 64), (2, 64, 64)])
+def test_wgmma_operand_layouts(W, mode, N, K):
+    _operand_case(W, mode, N, K, 64, mode * 100 + N + 64)
+
+
+def test_wgmma_accumulation_precision(W):
+    """Measured fp32 accumulation error of wgmma.mma_async .f32.f16.f16 on random fp16 operands with a wide exponent range, K up to
+    128: max |D - exact| / sum |a b| must not exceed the gamma(K) the interval reference of the decoders (oracle/tc_decoders.py) uses."""
+    from oracle import tc_decoders as T
+    rng = np.random.default_rng(42)
+    worst = {}
+    for K in (16, 64, 128):
+        for rep in range(4):
+            X = rng.standard_normal((64, K)) * 2.0 ** rng.integers(-8, 8, (64, K))
+            Wm = rng.standard_normal((128, K)) * 2.0 ** rng.integers(-8, 8, (128, K))
+            if rep % 2:                                         # cancellation: sums much smaller than sum |terms|
+                X[:, K // 2:] = X[:, :K // 2]
+                Wm[:, K // 2:] = -Wm[:, :K // 2] * (1.0 + 2.0 ** -9 * rng.standard_normal((128, K // 2)))
+            X, Wm = X.astype(np.float16).astype(np.float64), Wm.astype(np.float16).astype(np.float64)
+            assert np.isfinite(X).all() and np.isfinite(Wm).all()
+            D = _selftest(W, 0, 64, 128, K, slab_image(X), weight_image(Wm))
+            exact, mag = X @ Wm.T, np.abs(X) @ np.abs(Wm).T
+            ratio = float((np.abs(D - exact) / mag).max())
+            worst[K] = max(worst.get(K, 0.0), ratio)
+    print("wgmma accumulation max|err|/sum|terms|:", {k: f"{v:.3e} (gamma {T.gamma(k):.3e}, {v / 2.0 ** -24:.2f} units of 2^-24)" for k, v in worst.items()})
+    for K, v in worst.items():
+        assert v <= T.gamma(K), (K, v, T.gamma(K))
 
 
 # ---------------------------------------------------------------------------------------------------------------
