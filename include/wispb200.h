@@ -309,8 +309,9 @@ int wb_rf_march_fill(const wb_rays* rays, int32_t num_samples, const float* jitt
  * blob: float [wb_rf_param_blob_floats(nef)]. */
 int64_t wb_rf_param_blob_floats(const wb_nef_desc* nef, int32_t precision);
 /* 1 if the decoder configuration can run at `precision` (forward only, or forward + backward), else 0 with the reason in
- * wb_last_error().  precision 0 always can; precision 1 is limited by shared memory / TMEM (e.g. 64-wide decoders with
- * backward, 128-wide forward only).  Host-side query, no device work. */
+ * wb_last_error().  precision 0 always can; precision 1 needs layers at most 128 wide and, for the backward, a decoder whose
+ * activation tiles and weight-gradient accumulators fit in shared memory (decoders with up to one hidden density and two hidden
+ * colour layers may split the accumulators over several passes).  Host-side query, no device work. */
 int wb_rf_precision_supported(const wb_nef_desc* nef, int32_t precision, int32_t backward);
 int wb_rf_pack_params(const wb_nef_desc* nef, int32_t precision, float* blob, wb_stream s);
 /* precision 1 scratch: workspace = per-ray view-embedding rows (+ dL/dfeat planes when backward != 0);
@@ -331,7 +332,8 @@ int wb_rf_shade_bwd(const wb_nef_desc* nef, const float* blob, int32_t precision
 
 /* Precision 1: wb_rf_shade_fwd writes the per-ray colour-input rows (view embedding) at the start of its workspace; a caller that hands
  * the SAME workspace (sized with backward = 1) and the same rays to the backward can say so right before that call and save the
- * launch that would rebuild them.  Applies to the next wb_rf_shade_bwd / wb_rf_decoder_bwd of the calling thread only. */
+ * launch that would rebuild them.  Applies to the next wb_rf_shade_bwd / wb_rf_decoder_bwd of the calling thread only, whatever
+ * that call returns (also with S == 0, precision 0 or an argument error). */
 int wb_rf_workspace_holds_ray_rows(int32_t yes);
 
 /* scale = 2^clamp(floor(log2(64 / max(absmax, 1e-30))), -20, 60): the loss scale wb_rf_decoder_bwd / wb_rf_table_scatter expect,

@@ -83,6 +83,18 @@ __device__ __forceinline__ void wb_ray_range(const WbMarch& m, int64_t r, float&
 }
 // torch.addcmul(origins, dirs, depth) (octree_as.py:283): a + alpha*b*c == fma(b, c, a)
 __device__ __forceinline__ float wb_addcmul(float o, float d, float t) { return __fmaf_rn(d, t, o); }
+// the point at depth t of ray `ray`, as above
+__device__ __forceinline__ float3 wb_ray_point(const float* origins, const float* dirs, int64_t ray, float t) {
+    return make_float3(wb_addcmul(__ldg(origins + 3 * ray), __ldg(dirs + 3 * ray), t),
+                       wb_addcmul(__ldg(origins + 3 * ray + 1), __ldg(dirs + 3 * ray + 1), t),
+                       wb_addcmul(__ldg(origins + 3 * ray + 2), __ldg(dirs + 3 * ray + 2), t));
+}
+// position of sample record s.  A kernel that holds the ray index already passes it to wb_ray_point: the compiler does not merge a
+// second load of rec_ray[s] across barriers.
+__device__ __forceinline__ float3 wb_sample_pos(const float* origins, const float* dirs, const int32_t* rec_ray, const float* rec_t, int64_t s) {
+    const int64_t ray = __ldg(rec_ray + s);
+    return wb_ray_point(origins, dirs, ray, __ldg(rec_t + s));
+}
 
 // ---------------------------------------------------------------------------------------------
 // Octree occupancy  [KAOLIN-EXT unbatched_query, SURVEY.md Appendix A]

@@ -16,53 +16,46 @@
 // reductions (red.global.add.v2.f32).  No S-sized activation tensor ever exists in HBM.
 #include "wb_common.cuh"
 #include "wb_featx.cuh"
+#include "wb_shade_tc.cuh"
 #include <math.h>
 
 #define WB_ML 16          // max linear layers over both decoders
-
-// tensor-core variant (wb_shade_tc.cu)
-int wb_tc_blob_floats(const wb_nef_desc* nef);
-int wb_tc_pack(const wb_nef_desc* nef, float* blob, cudaStream_t st);
-int wb_tc_shade_fwd(const wb_nef_desc* nef, const float* blob, const wb_rays* rays, const float* rec_t, const int32_t* rec_ray,
-                    int64_t S, float* shaded, void* feat_save, void* workspace, cudaStream_t st);
-int wb_tc_shade_bwd(const wb_nef_desc* nef, const float* blob, const wb_rays* rays, const float* rec_t, const int32_t* rec_ray,
-                    int64_t S, const float* g_shaded, const float* scale, const void* feat_saved, void* workspace,
-                    float* grad_table, float* grad_dens, float* grad_col, cudaStream_t st);
-int wb_tc_decoder_bwd(const wb_nef_desc* nef, const float* blob, const wb_rays* rays, const float* rec_t, const int32_t* rec_ray,
-                      int64_t S, const float* g_shaded, const float* scale, const void* feat_saved, void* workspace,
-                      float* grad_dens, float* grad_col, cudaStream_t st);
-int wb_tc_table_scatter(const wb_nef_desc* nef, const wb_rays* rays, const float* rec_t, const int32_t* rec_ray, int64_t S,
-                        const float* scale, void* workspace, float* grad_table, cudaStream_t st);
-int64_t wb_tc_workspace_bytes(const wb_nef_desc* nef, int64_t R, int64_t S, int backward);
-int64_t wb_tc_feat_bytes(const wb_nef_desc* nef, int64_t S);
 
 extern "C" int64_t wb_rf_workspace_bytes(const wb_nef_desc* nef, int32_t precision, int64_t R, int64_t S, int32_t backward)
 {
     if (precision != 1) return 0;
     return wb_tc_workspace_bytes(nef, R, S, backward);
 }
+
+// Set by wb_rf_workspace_holds_ray_rows() for the next backward call of this thread only: the backward entries take it (read and
+// clear) before anything else, so a call that returns early cannot leave it behind for a later call with another workspace.
+static thread_local bool g_ray_rows_ready = false;
+extern "C" int wb_rf_workspace_holds_ray_rows(int32_t yes) { g_ray_rows_ready = yes != 0; return WB_OK; }
+static bool wb_take_ray_rows_ready() { const bool v = g_ray_rows_ready; g_ray_rows_ready = false; return v; }
+
 // precision-1 backward in its two stages (wb_rf_shade_bwd == decoder_bwd followed by table_scatter)
 extern "C" int wb_rf_decoder_bwd(const wb_nef_desc* nef, const float* blob, const wb_rays* rays, const float* rec_t, const int32_t* rec_ray,
                                  int64_t S, const float* g_shaded, const float* loss_scale, const void* feat_saved, void* workspace,
                                  float* grad_dens, float* grad_col, wb_stream s)
 {
+    const bool ray_rows_ready = wb_take_ray_rows_ready();
     if (S == 0) return WB_OK;
     WB_CHECK_ARG(nef && blob && rays && rays->origins && rays->dirs && rec_t && rec_ray && g_shaded && grad_dens && grad_col, "null pointer");
-    return wb_tc_decoder_bwd(nef, blob, rays, rec_t, rec_ray, S, g_shaded, loss_scale, feat_saved, workspace, grad_dens, grad_col, (cudaStream_t)s);
+    return wb_tc_decoder_bwd_ex(nef, blob, rays, rec_t, rec_ray, S, 0, S, g_shaded, loss_scale, feat_saved, workspace, ray_rows_ready,
+                                grad_dens, grad_col, nullptr, nullptr, (cudaStream_t)s);
 }
 extern "C" int wb_rf_table_scatter(const wb_nef_desc* nef, const wb_rays* rays, const float* rec_t, const int32_t* rec_ray, int64_t S,
                                    const float* loss_scale, void* workspace, float* grad_table, wb_stream s)
 {
     if (S == 0) return WB_OK;
     WB_CHECK_ARG(nef && rays && rays->origins && rays->dirs && rec_t && rec_ray, "null pointer");
-    return wb_tc_table_scatter(nef, rays, rec_t, rec_ray, S, loss_scale, workspace, grad_table, (cudaStream_t)s);
+    return wb_tc_table_scatter(nef, rays, rec_t, rec_ray, S, 0, S, loss_scale, workspace, grad_table, (cudaStream_t)s);
 }
 extern "C" int64_t wb_rf_feat_bytes(const wb_nef_desc* nef, int32_t precision, int64_t S)
 {
     if (precision != 1) return 0;
     return wb_tc_feat_bytes(nef, S);
 }
-int wb_tc_supported(const wb_nef_desc* nef, int backward);
 extern "C" int wb_rf_precision_supported(const wb_nef_desc* nef, int32_t precision, int32_t backward)
 {
     if (precision == 0) return 1;
@@ -519,17 +512,13 @@ wb_shade_bwd_kernel(WbGrid g, WbGridX gx, WbMlp m, const float* __restrict__ blo
         }
         // ---- scatter dL/dfeat into the table (hashgrid_interpolate_cuda.cu:151-160) ----
         if (valid) {
-            const int ray = __ldg(in.rec_ray + s);
-            const float t = __ldg(in.rec_t + s);
-            const float px = wb_addcmul(__ldg(in.origins + 3 * (int64_t)ray), __ldg(in.dirs + 3 * (int64_t)ray), t);
-            const float py = wb_addcmul(__ldg(in.origins + 3 * (int64_t)ray + 1), __ldg(in.dirs + 3 * (int64_t)ray + 1), t);
-            const float pz = wb_addcmul(__ldg(in.origins + 3 * (int64_t)ray + 2), __ldg(in.dirs + 3 * (int64_t)ray + 2), t);
+            const float3 p = wb_sample_pos(in.origins, in.dirs, in.rec_ray, in.rec_t, s);
             const int L = g.L, F = g.F;
             const int lmax = gx.kind != 0 ? 0 : g.multiscale == 0 ? min(L, g.lod_idx) : L;
-            if (gx.kind != 0) wb_featx_scatter(gx, px, py, pz, [&](int f) { return gout[f * NTP]; });     // triplanar / octree grid
+            if (gx.kind != 0) wb_featx_scatter(gx, p.x, p.y, p.z, [&](int f) { return gout[f * NTP]; });     // triplanar / octree grid
             for (int l = 0; l < lmax; ++l) {
                 uint32_t idx[8]; float cf[8];
-                wb_corner_setup(g, l, px, py, pz, idx, cf);
+                wb_corner_setup(g, l, p.x, p.y, p.z, idx, cf);
                 float* tb = G.gtable + g.begin[l] * F;
                 if (F == 2) {
                     const float g0 = g.multiscale == 0 ? gout[(l * 2) * NTP] : gout[0];
@@ -571,11 +560,14 @@ extern "C" int wb_rf_shade_bwd(const wb_nef_desc* nef, const float* blob, int32_
                                const float* loss_scale, const void* feat_saved, void* workspace,
                                float* grad_table, float* grad_dens, float* grad_col, wb_stream s)
 {
+    const bool ray_rows_ready = wb_take_ray_rows_ready();
     WB_CHECK_ARG(precision == 0 || precision == 1, "precision must be 0 (fp32) or 1 (fp16 tensor cores)");
     if (S == 0) return WB_OK;
     WB_CHECK_ARG(blob && rays && rays->origins && rays->dirs && rec_t && rec_ray && g_shaded, "null pointer");
     WB_CHECK_ARG((grad_table || nef->grid_kind != 0) && grad_dens && grad_col, "null gradient buffer");
-    if (precision == 1) return wb_tc_shade_bwd(nef, blob, rays, rec_t, rec_ray, S, g_shaded, loss_scale, feat_saved, workspace, grad_table, grad_dens, grad_col, (cudaStream_t)s);
+    if (precision == 1)
+        return wb_tc_shade_bwd(nef, blob, rays, rec_t, rec_ray, S, g_shaded, loss_scale, feat_saved, workspace, ray_rows_ready, grad_table,
+                               grad_dens, grad_col, (cudaStream_t)s);
     WbGrid g; int rc = wb_make_grid(nef, &g); if (rc) return rc;
     WbGridX gx; rc = wb_make_gridx(nef, true, &gx); if (rc) return rc;
     WbMlp m; rc = wb_make_mlp(nef, true, &m); if (rc) return rc;

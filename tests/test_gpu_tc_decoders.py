@@ -2,7 +2,8 @@
 (oracle/tc_decoders.py): every output must lie inside centre +- radius, which any kernel that rounds at the same points lands
 in whatever order it sums.  Covers what the end-to-end parity tests cannot resolve at their fp32-oracle tolerances: decoder
 widths 16..128 and unequal widths, bias on / off, density-head widths 2..16, decoder depths, the view / position embeddings,
-the saved X0 rows, the fused and the stand-alone table scatter, the loss scale, and sample counts around the 64-sample tile.
+the saved X0 rows, the fused and the stand-alone table scatter, the chunked backward of wide decoders, the loss scale, and sample
+counts around the 64-sample tile.
 
 Case ids name the kernel instances: fwd64 / fwd128 = the forward kernel's widest padded layer (NMAX), gNpM = the decoder backward
 runs N groups per CTA in M passes (bwd_plan mirrors tc_bwd_layout / tc_bwd_passes of wb_shade_tc.cu), +fused = the table
@@ -368,6 +369,54 @@ def test_tc_no_samples_touches_nothing(W):
     torch.cuda.synchronize()
     for t in (shaded, gd, gc, gt):
         assert bool((t == sentinel).all())
+
+
+def test_chunked_backward_matches_two_stages(W):
+    """From 2^20 samples on, wb_rf_shade_bwd of a decoder whose backward runs one group per CTA cuts the samples into four chunks and
+    runs the table scatter of each chunk on a side stream beside the decoder backward of the next.  It must compute what
+    wb_rf_decoder_bwd followed by wb_rf_table_scatter over all samples computes, up to the order of the atomic additions."""
+    case = Case("chunked", [128], [128, 128], view=(3, 4), L=16, S=(1 << 20) + 4097, R=5000)
+    plan = bwd_plan(case)
+    assert plan[0] == 1
+    s = Setup(W, case)
+    s.forward()
+    g = (np.random.default_rng(5).standard_normal((s.S, 4)) * 1e-2).astype(np.float32)
+    scale = s.loss_scale(g)
+    n0 = s.A.launch_count()
+    gd1, gc1, gt1 = s.shade_bwd(g, scale)
+    # the per-ray rows once, then per chunk every pass of the decoder backward and one scatter
+    assert s.A.launch_count() - n0 == 1 + 4 * (len(plan) + 1)
+    gd2, gc2, _ = s.decoder_bwd(g, scale)
+    gt2 = s.table_scatter(scale)
+    report = [case_id(case)]
+    for nm, a, b in (("grad_table", gt1, gt2), ("grad_dens", gd1, gd2), ("grad_col", gc1, gc2)):
+        top = float(np.abs(b).max())
+        ratio = float(np.abs(a - b).max()) / top
+        report.append(f"{nm}: max|chunked - two-stage| / max|two-stage| = {ratio:.2e}")
+        assert top > 0.0 and ratio <= TOL1_GRAD, (nm, ratio)
+    print("TCREPORT " + " | ".join(report))
+
+
+def test_ray_rows_flag_applies_to_the_next_backward_only(W):
+    """wb_rf_workspace_holds_ray_rows(1) covers the next backward call of the thread, also when that call has nothing to do (S == 0):
+    a later backward into a workspace without the per-ray colour-input rows must write them itself."""
+    s = Setup(W, Case("rows", [64], [64, 64], view=(3, 4), L=16))
+    rng = np.random.default_rng(3)
+    X = T.f16(rng.standard_normal((s.S, s.dens_dims[0])) * 0.7)
+    s.set_x0_rows(X.astype(np.float16))
+    g = (rng.standard_normal((s.S, 4)) * 1e-2).astype(np.float32)
+    scale = s.loss_scale(g)
+    want = s.decoder_bwd(g, scale)
+    A, L, p = s.A, s.L, s.A.ptr
+    gd, gc, _ = s.zeros_grads()
+    A.check(L.wb_rf_workspace_holds_ray_rows(C.c_int32(1)))
+    A.check(L.wb_rf_decoder_bwd(C.byref(s.desc), p(s.blob), C.byref(s.rays), p(s.t_rec_t), p(s.t_rec_ray), C.c_int64(0), p(gd), p(scale),
+                                p(s.feat), p(s.ws), p(gd), p(gc), A.stream()))
+    s.ws.fill_(0xFF)                          # a fresh workspace: 0xFFFF is an fp16 NaN
+    got = s.decoder_bwd(g, scale)
+    bw = T.Reference(s.dec, X, s.view).backward(g, float(scale.item()), s.planes, 2, wgrad_n=s.wgrad_n())
+    for a, b, key in zip(got, want, ("dens", "col", "dfeat")):
+        assert np.all(np.abs(a - b) <= 2 * bw[key][1]), key        # both inside the reference interval: atomic order only
 
 
 def _scale_formula(a):

@@ -17,7 +17,7 @@ def functions(path):
         m = re.search(r"Function : (\S+)", line)
         if m:
             cur = m.group(1); funcs[cur] = []; continue
-        if cur and re.search(r"/\*[0-9a-f]{4}\*/", line):
+        if cur and re.search(r"/\*[0-9a-f]{4,}\*/", line):
             funcs[cur].append(re.sub(r"\s+", " ", re.sub(r"/\*.*?\*/", "", line)).strip())
     return funcs
 
