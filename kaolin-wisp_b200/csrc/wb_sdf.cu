@@ -18,158 +18,9 @@
 //   Numerics: fp32 decoder (the tracer runs under torch.no_grad() without autocast); octree features rounded to fp16 on load and
 //   per-LOD results rounded to fp16, as the call site does (octree_grid.py:147-149).  The decoder's summation order differs from
 //   cuBLAS: results agree to fp32 rounding, hit decisions can differ only where |sdf| is within ~1e-6 of a threshold.
-#include "wb_common.cuh"
+#include "wb_sdf.cuh"
 #include <cooperative_groups.h>
 namespace cg = cooperative_groups;
-
-constexpr int WB_SDF_MAX_IN = 132;        // 3 + 6*freq position embedding + features
-constexpr int WB_SDF_MAX_H = 128;
-constexpr int WB_SDF_THREADS = 256;
-
-struct WbSdf {
-    // octree grid
-    const int16_t* points; const int32_t* trinkets;
-    const float* feats[WB_MAX_LODS];
-    int F, base_lod, num_lods, multiscale, half_round;
-    // decoder
-    int pos_mode, pos_freq, pos_dim, feat_dim, in_dim, in_pad, H, nh;      // nh hidden layers (>= 1), all H wide
-    const float* params;                                                     // packed [W0, b0, W1, b1, ..., Wout, bout] (nn.Linear layout)
-    int smem_floats;
-};
-
-static int sdf_embed_dim(int mode, int freq) { return mode == 0 ? 0 : mode == 1 ? 3 : mode == 2 ? 6 * freq : 3 + 6 * freq; }
-
-static int wb_make_sdf(const wb_sdf_desc* d, WbSdf* m)
-{
-    WB_CHECK_ARG(d != nullptr && d->points && d->trinkets && d->feats && d->params, "null pointer in wb_sdf_desc");
-    WB_CHECK_ARG(d->num_lods >= 1 && d->num_lods <= WB_MAX_LODS && d->base_lod >= 0, "bad LOD range");
-    WB_CHECK_ARG(d->feature_dim >= 1 && d->feature_dim <= 64, "feature_dim must be in [1,64]");
-    WB_CHECK_ARG(d->multiscale == 0 || d->multiscale == 1, "multiscale must be 0 ('cat') or 1 ('sum')");
-    WB_CHECK_ARG(d->num_layers >= 1 && d->num_layers <= 4 && d->hidden_dim >= 1 && d->hidden_dim <= WB_SDF_MAX_H, "decoder: 1..4 hidden layers, <= 128 wide");
-    WB_CHECK_ARG(d->pos_mode >= 0 && d->pos_mode <= 3 && d->pos_freq >= 0 && d->pos_freq <= 10, "bad position embedding");
-    m->points = d->points; m->trinkets = d->trinkets;
-    for (int k = 0; k < d->num_lods; ++k) { WB_CHECK_ARG(d->feats[k] != nullptr, "null feature level"); m->feats[k] = d->feats[k]; }
-    m->F = d->feature_dim; m->base_lod = d->base_lod; m->num_lods = d->num_lods; m->multiscale = d->multiscale; m->half_round = d->half_round;
-    m->pos_mode = d->pos_mode; m->pos_freq = d->pos_freq; m->pos_dim = sdf_embed_dim(d->pos_mode, d->pos_freq);
-    m->feat_dim = d->multiscale ? d->feature_dim : d->feature_dim * d->num_lods;
-    m->in_dim = m->pos_dim + m->feat_dim; m->in_pad = (m->in_dim + 3) & ~3;
-    WB_CHECK_ARG(m->in_dim <= WB_SDF_MAX_IN, "decoder input too wide");
-    m->H = d->hidden_dim; m->nh = d->num_layers; m->params = d->params;
-    WB_CHECK_ARG(m->nh == 1 || (m->H % 4) == 0, "hidden_dim must be a multiple of 4 for multi-layer decoders");
-    m->smem_floats = m->H * m->in_pad + m->H + (m->nh - 1) * (m->H * m->H + m->H) + m->H + 4;
-    WB_CHECK_ARG(m->smem_floats * 4 <= 200 * 1024, "decoder does not fit in shared memory");
-    return WB_OK;
-}
-
-// shared-memory image: W0 rows padded to in_pad floats | b0 | (W_k [H x H] | b_k) ... | Wout [H] | bout
-__device__ __forceinline__ void sdf_stage(const WbSdf& m, float* sw)
-{
-    const float* p = m.params;
-    int o = 0, src = 0;
-    for (int e = threadIdx.x; e < m.H * m.in_pad; e += blockDim.x) {
-        const int j = e / m.in_pad, k = e - j * m.in_pad;
-        sw[e] = k < m.in_dim ? __ldg(p + j * m.in_dim + k) : 0.0f;
-    }
-    o += m.H * m.in_pad; src += m.H * m.in_dim;
-    for (int e = threadIdx.x; e < m.H; e += blockDim.x) sw[o + e] = __ldg(p + src + e);
-    o += m.H; src += m.H;
-    for (int l = 1; l < m.nh; ++l) {
-        for (int e = threadIdx.x; e < m.H * m.H + m.H; e += blockDim.x) sw[o + e] = __ldg(p + src + e);
-        o += m.H * m.H + m.H; src += m.H * m.H + m.H;
-    }
-    for (int e = threadIdx.x; e < m.H + 1; e += blockDim.x) sw[o + e] = __ldg(p + src + e);
-    __syncthreads();
-}
-
-__device__ __forceinline__ float sdf_h(float v) { return __half2float(__float2half_rn(v)); }
-
-// positional_embedder.py:51-66 / neural_sdf.py:86-99: [x (include_input), sin(winded), cos(winded)], winded freq-major coord-minor
-__device__ __forceinline__ int sdf_embed(int mode, int freq, float x, float y, float z, float* out)
-{
-    if (mode == 0) return 0;
-    int o = 0;
-    if (mode == 1 || mode == 3) { out[0] = x; out[1] = y; out[2] = z; o = 3; }
-    if (mode == 1) return 3;
-    float band = 1.0f;
-    for (int f = 0; f < freq; ++f) {
-        out[o + f * 3 + 0] = sinf(x * band); out[o + f * 3 + 1] = sinf(y * band); out[o + f * 3 + 2] = sinf(z * band);
-        out[o + 3 * freq + f * 3 + 0] = cosf(x * band); out[o + 3 * freq + f * 3 + 1] = cosf(y * band); out[o + 3 * freq + f * 3 + 2] = cosf(z * band);
-        band *= 2.0f;
-    }
-    return o + 6 * freq;
-}
-
-// OctreeGrid.interpolate for LODs 0..nl-1 of one point -> feat[] (zeros where the point leaves the octree); FT > 0: compile-time
-// feature width of a 'sum' grid (accumulators in registers)
-template <int FT>
-__device__ __forceinline__ void sdf_features(const WbOct& oc, const WbSdf& m, int nl, float cx, float cy, float cz, float* feat)
-{
-    const int F = FT > 0 ? FT : m.F;
-    const bool sum = FT > 0 ? true : (m.multiscale != 0 && nl > 1);         // lod_idx == 0: a single LOD either way (octree_grid.py:190-198)
-    const int width = sum ? F : nl * F;
-#pragma unroll
-    for (int f = 0; f < (FT > 0 ? FT : 1); ++f) feat[f] = 0.0f;
-    if (FT == 0) for (int f = 0; f < width; ++f) feat[f] = 0.0f;
-    const int L = m.base_lod + nl - 1;                                       // level of the finest LOD used
-    const float h = ldexpf(1.0f, L - 1), inv_h = ldexpf(1.0f, -(L - 1)), maxq = (float)((1 << L) - 1);
-    int qx, qy, qz;
-    if (!(wb_quantize(cx, h, inv_h, maxq, qx) && wb_quantize(cy, h, inv_h, maxq, qy) && wb_quantize(cz, h, inv_h, maxq, qz))) return;
-    int node = 0;
-    for (int l = 0; l <= L; ++l) {
-        if (l > 0) {
-            const int d = L - l;
-            const int ci = (((qx >> d) & 1) << 2) | (((qy >> d) & 1) << 1) | ((qz >> d) & 1);
-            const uint32_t b = __ldg(oc.octree + node);
-            if (!(b & (1u << ci))) return;
-            node = __ldg(oc.prefix + node) + __popc(b & ((2u << ci) - 1u));
-        }
-        const int k = l - m.base_lod;
-        if (k < 0) continue;
-        const float hl = ldexpf(1.0f, l - 1);
-        const float ux = __fmaf_rn(cx, hl, hl) - (float)__ldg(m.points + 3 * (int64_t)node);
-        const float uy = __fmaf_rn(cy, hl, hl) - (float)__ldg(m.points + 3 * (int64_t)node + 1);
-        const float uz = __fmaf_rn(cz, hl, hl) - (float)__ldg(m.points + 3 * (int64_t)node + 2);
-        const float ix = 1.0f - ux, iy = 1.0f - uy, iz = 1.0f - uz;
-        float cf[8];
-        cf[0] = (ix * iy) * iz; cf[1] = (ix * iy) * uz; cf[2] = (ix * uy) * iz; cf[3] = (ix * uy) * uz;
-        cf[4] = (ux * iy) * iz; cf[5] = (ux * iy) * uz; cf[6] = (ux * uy) * iz; cf[7] = (ux * uy) * uz;
-        const int4 t0 = __ldg(reinterpret_cast<const int4*>(m.trinkets + 8 * (int64_t)node));
-        const int4 t1 = __ldg(reinterpret_cast<const int4*>(m.trinkets + 8 * (int64_t)node) + 1);
-        const int tk[8] = { t0.x, t0.y, t0.z, t0.w, t1.x, t1.y, t1.z, t1.w };
-        const float* ft = m.feats[k];
-        if (FT > 0 && (FT % 4) == 0) {
-            float acc[FT > 0 ? FT : 1];
-#pragma unroll
-            for (int f = 0; f < FT; ++f) acc[f] = 0.0f;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const float4* row = reinterpret_cast<const float4*>(ft + (int64_t)tk[j] * FT);
-#pragma unroll
-                for (int q = 0; q < FT / 4; ++q) {
-                    float4 v = __ldg(row + q);
-                    if (m.half_round) { v.x = sdf_h(v.x); v.y = sdf_h(v.y); v.z = sdf_h(v.z); v.w = sdf_h(v.w); }
-                    acc[4 * q] = fmaf(v.x, cf[j], acc[4 * q]); acc[4 * q + 1] = fmaf(v.y, cf[j], acc[4 * q + 1]);
-                    acc[4 * q + 2] = fmaf(v.z, cf[j], acc[4 * q + 2]); acc[4 * q + 3] = fmaf(v.w, cf[j], acc[4 * q + 3]);
-                }
-            }
-#pragma unroll
-            for (int f = 0; f < FT; ++f) feat[f] += m.half_round ? sdf_h(acc[f]) : acc[f];
-        } else {
-            for (int f = 0; f < F; ++f) {
-                float acc = 0.0f;
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    float v = __ldg(ft + (int64_t)tk[j] * F + f);
-                    if (m.half_round) v = sdf_h(v);
-                    acc = fmaf(v, cf[j], acc);
-                }
-                if (m.half_round) acc = sdf_h(acc);
-                if (sum) feat[f] += acc; else feat[k * F + f] = acc;
-            }
-        }
-        if (k == nl - 1) return;
-    }
-}
 
 // NeuralSDF.sdf at one point.  FT/PT > 0: the app/nglod shape ('sum' grid of FT features, identity position input) with the
 // input vector in registers; otherwise the generic path through local arrays.
@@ -456,7 +307,6 @@ wb_sdf_phase_kernel(WbSdfTrace T, int phase, int it, int cb)
 // ---------------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------------
-static bool sdf_fast_shape(const WbSdf& m) { return m.multiscale == 1 && m.F == 16 && m.pos_mode == 1 && m.nh == 1; }
 
 extern "C" int wb_sdf_eval(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, const float* coords, int64_t N, float* out, wb_stream s)
 {

@@ -1,0 +1,257 @@
+// wb_sdf_train.cu -- the training step of app/nglod, SDFTrainer.step (wisp/trainers/sdf_trainer.py:65-124), over NeuralSDF.sdf
+// (wisp/models/nefs/neural_sdf.py:120-155) on an OctreeGrid: forward, L2 loss and backward of one loss LOD in ONE launch.
+// The reference runs the grid kernel, a cat, two cuBLAS GEMMs, the loss ops and their autograd backward (cuBLAS + the grid
+// scatter) per LOD.
+//
+// A CTA works on tiles of WB_SDF_TRAIN_TILE samples, grid-stride:
+//   pass 1, thread per sample: the forward of wb_sdf_eval (wb_sdf.cuh: same features, same summation order, so the same y), the
+//     loss, and dL/dx = dy * sum_{j: a_j > 0} wout_j W0[j,:], whose feature part is scattered into the grid gradients at once with
+//     wb_octree_interp_bwd's arithmetic (fp32 gradient, zeros skipped, no gradient to the coordinates; the fp16 rounding of the
+//     forward is passed straight through).  The decoder input x and dy stay in shared memory.
+//   pass 2, thread per hidden unit j: a_j recomputed for every sample of the tile (same order, so the same relu mask) and
+//     dL/dW0[j,:] += da x, dL/db0[j] += da, dL/dwout[j] += dy relu(a), accumulated over all tiles of the CTA and added to
+//     grad_params once at the end (per-sample atomics into the decoder would serialise on a few thousand addresses).
+// fp32 SIMT throughout: ~15 kFLOP per sample against ~3 KB of feature gather and ~6 KB of scatter read-modify-write.
+#include "wb_sdf.cuh"
+#include "wb_featx.cuh"
+
+constexpr int WB_SDF_TRAIN_TILE = 128;
+
+struct WbSdfTrain {
+    const float* coords; const float* gt; int64_t N; float inv_count;
+    float* gparams; float* loss;
+    int xs_off, gw_off, red_off;          // shared-memory offsets (floats): x [TILE][in_pad] + dy [TILE] | dL/dW0 [H][in_pad+1] | reduction
+};
+
+// 'sum' grid of FT features (FT % 4 == 0): every LOD gets the same dL/dfeat g (registers); one float4 reduction per corner and quad
+template <int FT>
+__device__ __forceinline__ void sdf_scatter_sum(const WbGridX& x, float cx, float cy, float cz, const float* g)
+{
+    wb_oct_walk(x, cx, cy, cz, [&](int l, int node) {
+        float cf[8]; int tk[8];
+        wb_oct_cell(x, node, l, cx, cy, cz, cf, tk);
+        float4* gt = reinterpret_cast<float4*>(x.gptr[l - x.base_lod]);
+#pragma unroll
+        for (int q = 0; q < FT / 4; ++q) {
+            if (g[4 * q] == 0.0f && g[4 * q + 1] == 0.0f && g[4 * q + 2] == 0.0f && g[4 * q + 3] == 0.0f) continue;
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+                atomicAdd(gt + (int64_t)tk[j] * (FT / 4) + q, make_float4(g[4 * q] * cf[j], g[4 * q + 1] * cf[j], g[4 * q + 2] * cf[j], g[4 * q + 3] * cf[j]));
+        }
+    });
+}
+
+template <int FT, int PT>
+__global__ void __launch_bounds__(WB_SDF_TRAIN_TILE)
+wb_sdf_train_kernel(WbOct oc, WbSdf m, WbGridX gx, int nl, WbSdfTrain T)
+{
+    constexpr bool FAST = FT > 0 && PT == 1;             // dispatch guarantees nh == 1, 'sum', identity position input
+    constexpr int INF = FAST ? ((3 + FT + 3) & ~3) : 1;  // compile-time in_pad of the fast shape
+    extern __shared__ __align__(16) float sw[];
+    sdf_stage(m, sw);
+    const int H = m.H, INP = FAST ? INF : m.in_pad, IN = m.in_dim;
+    const float* b0 = sw + H * INP; const float* wo = b0 + H;
+    float* xs = sw + T.xs_off; float* dys = xs + WB_SDF_TRAIN_TILE * INP;
+    float* gw = sw + T.gw_off;                             // generic shape: dL/dW0, row j owned by thread j (odd stride: no bank conflicts)
+    const int tid = threadIdx.x, GS = INP + 1;
+    float gwr[INF];                                       // fast shape: dL/dW0[tid, :] in registers
+#pragma unroll
+    for (int k = 0; k < INF; ++k) gwr[k] = 0.0f;
+    if (!FAST) for (int e = tid; e < H * GS; e += blockDim.x) gw[e] = 0.0f;
+    float gb = 0.0f, gwo = 0.0f, lsum = 0.0f, dsum = 0.0f;
+    for (int64_t base = (int64_t)blockIdx.x * WB_SDF_TRAIN_TILE; base < T.N; base += (int64_t)gridDim.x * WB_SDF_TRAIN_TILE) {
+        const int64_t i = base + tid;
+        float* xr = xs + tid * INP;
+        float dy = 0.0f;
+        if (i < T.N) {
+            const float x = __ldg(T.coords + 3 * i), y = __ldg(T.coords + 3 * i + 1), z = __ldg(T.coords + 3 * i + 2);
+            if constexpr (FAST) {
+                float in[INF], g[INF];
+                in[0] = x; in[1] = y; in[2] = z;
+                sdf_features<FT>(oc, m, nl, x, y, z, in + 3);
+#pragma unroll
+                for (int k = 3 + FT; k < INF; ++k) in[k] = 0.0f;
+#pragma unroll
+                for (int k = 0; k < INF; ++k) g[k] = 0.0f;
+                float out = wo[H];
+                int j = 0;
+                for (; j + 4 <= H; j += 4) {                    // wb_sdf_eval's order: four chains, output layer in unit order
+                    float a0 = b0[j], a1 = b0[j + 1], a2 = b0[j + 2], a3 = b0[j + 3];
+                    const float4* w0 = reinterpret_cast<const float4*>(sw + j * INF);
+                    const float4* w1 = reinterpret_cast<const float4*>(sw + (j + 1) * INF);
+                    const float4* w2 = reinterpret_cast<const float4*>(sw + (j + 2) * INF);
+                    const float4* w3 = reinterpret_cast<const float4*>(sw + (j + 3) * INF);
+#pragma unroll
+                    for (int q = 0; q < INF / 4; ++q) {
+                        const float4 u0 = w0[q], u1 = w1[q], u2 = w2[q], u3 = w3[q];
+                        const float x0 = in[4 * q], x1 = in[4 * q + 1], x2 = in[4 * q + 2], x3 = in[4 * q + 3];
+                        a0 = fmaf(u0.x, x0, a0); a1 = fmaf(u1.x, x0, a1); a2 = fmaf(u2.x, x0, a2); a3 = fmaf(u3.x, x0, a3);
+                        a0 = fmaf(u0.y, x1, a0); a1 = fmaf(u1.y, x1, a1); a2 = fmaf(u2.y, x1, a2); a3 = fmaf(u3.y, x1, a3);
+                        a0 = fmaf(u0.z, x2, a0); a1 = fmaf(u1.z, x2, a1); a2 = fmaf(u2.z, x2, a2); a3 = fmaf(u3.z, x2, a3);
+                        a0 = fmaf(u0.w, x3, a0); a1 = fmaf(u1.w, x3, a1); a2 = fmaf(u2.w, x3, a2); a3 = fmaf(u3.w, x3, a3);
+                    }
+                    out = fmaf(wo[j], fmaxf(a0, 0.0f), out); out = fmaf(wo[j + 1], fmaxf(a1, 0.0f), out);
+                    out = fmaf(wo[j + 2], fmaxf(a2, 0.0f), out); out = fmaf(wo[j + 3], fmaxf(a3, 0.0f), out);
+                    const float c0 = a0 > 0.0f ? wo[j] : 0.0f, c1 = a1 > 0.0f ? wo[j + 1] : 0.0f;
+                    const float c2 = a2 > 0.0f ? wo[j + 2] : 0.0f, c3 = a3 > 0.0f ? wo[j + 3] : 0.0f;
+#pragma unroll
+                    for (int q = 0; q < INF / 4; ++q) {
+                        const float4 u0 = w0[q], u1 = w1[q], u2 = w2[q], u3 = w3[q];
+                        g[4 * q] = fmaf(c0, u0.x, fmaf(c1, u1.x, fmaf(c2, u2.x, fmaf(c3, u3.x, g[4 * q]))));
+                        g[4 * q + 1] = fmaf(c0, u0.y, fmaf(c1, u1.y, fmaf(c2, u2.y, fmaf(c3, u3.y, g[4 * q + 1]))));
+                        g[4 * q + 2] = fmaf(c0, u0.z, fmaf(c1, u1.z, fmaf(c2, u2.z, fmaf(c3, u3.z, g[4 * q + 2]))));
+                        g[4 * q + 3] = fmaf(c0, u0.w, fmaf(c1, u1.w, fmaf(c2, u2.w, fmaf(c3, u3.w, g[4 * q + 3]))));
+                    }
+                }
+                for (; j < H; ++j) {
+                    const float4* wr = reinterpret_cast<const float4*>(sw + j * INF);
+                    float a = b0[j];
+#pragma unroll
+                    for (int q = 0; q < INF / 4; ++q) {
+                        const float4 w = wr[q];
+                        a = fmaf(w.x, in[4 * q], a); a = fmaf(w.y, in[4 * q + 1], a); a = fmaf(w.z, in[4 * q + 2], a); a = fmaf(w.w, in[4 * q + 3], a);
+                    }
+                    out = fmaf(wo[j], fmaxf(a, 0.0f), out);
+                    const float c = a > 0.0f ? wo[j] : 0.0f;
+#pragma unroll
+                    for (int q = 0; q < INF / 4; ++q) {
+                        const float4 w = wr[q];
+                        g[4 * q] = fmaf(c, w.x, g[4 * q]); g[4 * q + 1] = fmaf(c, w.y, g[4 * q + 1]);
+                        g[4 * q + 2] = fmaf(c, w.z, g[4 * q + 2]); g[4 * q + 3] = fmaf(c, w.w, g[4 * q + 3]);
+                    }
+                }
+                const float d = out - __ldg(T.gt + i);
+                lsum = fmaf(d, d, lsum);
+                dy = T.inv_count * (2.0f * d);
+                float4* x4 = reinterpret_cast<float4*>(xr);
+#pragma unroll
+                for (int q = 0; q < INF / 4; ++q) x4[q] = make_float4(in[4 * q], in[4 * q + 1], in[4 * q + 2], in[4 * q + 3]);
+                float gf[FAST ? FT : 1];
+#pragma unroll
+                for (int f = 0; f < FT; ++f) gf[f] = dy * g[3 + f];
+                sdf_scatter_sum<FT>(gx, x, y, z, gf);
+            } else {
+                float g[WB_SDF_MAX_IN];
+                const int pd = sdf_embed(m.pos_mode, m.pos_freq, x, y, z, xr);
+                sdf_features<0>(oc, m, nl, x, y, z, xr + pd);
+                for (int k = IN; k < INP; ++k) xr[k] = 0.0f;
+                for (int k = pd; k < IN; ++k) g[k] = 0.0f;
+                float out = wo[H];
+                for (int j = 0; j < H; ++j) {                   // wb_sdf_eval's order
+                    const float* wj = sw + j * INP;
+                    float a = b0[j];
+                    for (int k = 0; k < IN; ++k) a = fmaf(wj[k], xr[k], a);
+                    out = fmaf(wo[j], fmaxf(a, 0.0f), out);
+                    if (a > 0.0f) for (int k = pd; k < IN; ++k) g[k] = fmaf(wo[j], wj[k], g[k]);
+                }
+                const float d = out - __ldg(T.gt + i);
+                lsum = fmaf(d, d, lsum);
+                dy = T.inv_count * (2.0f * d);
+                wb_featx_scatter(gx, x, y, z, [&](int f) { return dy * g[pd + f]; });
+            }
+        }
+        dys[tid] = dy; dsum += dy;
+        __syncthreads();
+        const int cnt = (int)min((int64_t)WB_SDF_TRAIN_TILE, T.N - base);
+        if (tid < H) {
+            const int j = tid;
+            const float bj = b0[j], woj = wo[j];
+            if constexpr (FAST) {
+                float wr[INF];
+                const float4* w4 = reinterpret_cast<const float4*>(sw + j * INF);
+#pragma unroll
+                for (int q = 0; q < INF / 4; ++q) { const float4 w = w4[q]; wr[4 * q] = w.x; wr[4 * q + 1] = w.y; wr[4 * q + 2] = w.z; wr[4 * q + 3] = w.w; }
+                for (int s = 0; s < cnt; ++s) {
+                    const float4* x4 = reinterpret_cast<const float4*>(xs + s * INF);
+                    float xv[INF];
+#pragma unroll
+                    for (int q = 0; q < INF / 4; ++q) { const float4 v = x4[q]; xv[4 * q] = v.x; xv[4 * q + 1] = v.y; xv[4 * q + 2] = v.z; xv[4 * q + 3] = v.w; }
+                    float a = bj;
+#pragma unroll
+                    for (int k = 0; k < INF; ++k) a = fmaf(wr[k], xv[k], a);
+                    const float ds = dys[s];
+                    const float da = a > 0.0f ? ds * woj : 0.0f;
+                    gb += da; gwo = fmaf(ds, fmaxf(a, 0.0f), gwo);
+#pragma unroll
+                    for (int k = 0; k < INF; ++k) gwr[k] = fmaf(da, xv[k], gwr[k]);
+                }
+            } else {
+                const float* wj = sw + j * INP;
+                float* gj = gw + j * GS;
+                for (int s = 0; s < cnt; ++s) {
+                    const float* xv = xs + s * INP;
+                    float a = bj;
+                    for (int k = 0; k < IN; ++k) a = fmaf(wj[k], xv[k], a);
+                    const float ds = dys[s];
+                    const float da = a > 0.0f ? ds * woj : 0.0f;
+                    gb += da; gwo = fmaf(ds, fmaxf(a, 0.0f), gwo);
+                    if (da != 0.0f) for (int k = 0; k < IN; ++k) gj[k] = fmaf(da, xv[k], gj[k]);
+                }
+            }
+        }
+        __syncthreads();
+    }
+    // flush: the decoder gradients of this CTA, then the loss and dL/dbout reduced over the CTA
+    float* gp = T.gparams;
+    if (tid < H) {
+        const int j = tid;
+        if constexpr (FAST) {
+#pragma unroll
+            for (int k = 0; k < INF; ++k) if (k < IN && gwr[k] != 0.0f) atomicAdd(gp + j * IN + k, gwr[k]);
+        } else {
+            for (int k = 0; k < IN; ++k) { const float v = gw[j * GS + k]; if (v != 0.0f) atomicAdd(gp + j * IN + k, v); }
+        }
+        if (gb != 0.0f) atomicAdd(gp + H * IN + j, gb);
+        if (gwo != 0.0f) atomicAdd(gp + H * IN + H + j, gwo);
+    }
+    float* red = sw + T.red_off;
+    lsum = wb_warp_sum(lsum); dsum = wb_warp_sum(dsum);
+    if ((tid & 31) == 0) { red[2 * (tid >> 5)] = lsum; red[2 * (tid >> 5) + 1] = dsum; }
+    __syncthreads();
+    if (tid == 0) {
+        float l = 0.0f, d = 0.0f;
+        for (int w = 0; w < WB_SDF_TRAIN_TILE / 32; ++w) { l += red[2 * w]; d += red[2 * w + 1]; }
+        if (l != 0.0f) atomicAdd(T.loss, l * T.inv_count);
+        if (d != 0.0f) atomicAdd(gp + H * IN + 2 * H, d);
+    }
+}
+
+extern "C" int wb_sdf_train(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, const float* coords, const float* sdf_gt, int64_t N,
+                            float inv_count, float* const* grad_feats, float* grad_params, float* loss_out, wb_stream s)
+{
+    WbSdf m; int rc = wb_make_sdf(nef, &m); if (rc) return rc;
+    WB_CHECK_ARG(m.nh == 1, "the fused training step covers decoders with exactly one hidden layer (num_layers == 1)");
+    WB_CHECK_ARG(lod_idx >= 0 && lod_idx < m.num_lods, "lod_idx out of range");
+    WB_CHECK_ARG(m.multiscale == 1 || lod_idx == m.num_lods - 1, "'cat' grids feed the decoder all LODs: lod_idx must be num_lods-1");
+    WB_CHECK_ARG(coords && sdf_gt && grad_feats && grad_params && loss_out && N >= 0, "null pointer");
+    if (N == 0) return WB_OK;
+    WbOct oc; rc = wb_make_oct(oct, m.base_lod + lod_idx, &oc); if (rc) return rc;
+    const bool fast = sdf_fast_shape(m);
+    WbGridX gx; memset(&gx, 0, sizeof(gx));
+    gx.kind = 2; gx.nl = lod_idx + 1; gx.sum = m.multiscale; gx.C = m.F;
+    gx.octree = oc.octree; gx.prefix = oc.prefix; gx.points = m.points; gx.trinkets = m.trinkets;
+    gx.base_lod = m.base_lod; gx.half_round = m.half_round;
+    for (int k = 0; k <= lod_idx; ++k) {
+        WB_CHECK_ARG(grad_feats[k] != nullptr, "null gradient level");
+        WB_CHECK_ARG(!fast || (reinterpret_cast<uintptr_t>(grad_feats[k]) & 15u) == 0, "gradient levels must be 16-byte aligned");
+        gx.ptr[k] = m.feats[k]; gx.gptr[k] = grad_feats[k];
+    }
+    WbSdfTrain T;
+    T.coords = coords; T.gt = sdf_gt; T.N = N; T.inv_count = inv_count; T.gparams = grad_params; T.loss = loss_out;
+    T.xs_off = (m.smem_floats + 3) & ~3;
+    T.gw_off = T.xs_off + WB_SDF_TRAIN_TILE * m.in_pad + WB_SDF_TRAIN_TILE;
+    T.red_off = T.gw_off + (fast ? 0 : m.H * (m.in_pad + 1));
+    const int smem = (T.red_off + 2 * (WB_SDF_TRAIN_TILE / 32)) * 4;
+    WB_CHECK_ARG(smem <= 227 * 1024, "decoder does not fit in shared memory");
+    const void* kern = fast ? (const void*)wb_sdf_train_kernel<16, 1> : (const void*)wb_sdf_train_kernel<0, 0>;
+    if (smem > 48 * 1024) WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    int per_sm = 0;
+    WB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, WB_SDF_TRAIN_TILE, smem));
+    WB_CHECK_ARG(per_sm >= 1, "training kernel does not fit on an SM");
+    int64_t ctas = (N + WB_SDF_TRAIN_TILE - 1) / WB_SDF_TRAIN_TILE; const int64_t cap = (int64_t)wb_num_sms() * per_sm; if (ctas > cap) ctas = cap;
+    int nl = lod_idx + 1;
+    void* args[] = { &oc, &m, &gx, &nl, &T };
+    WB_CUDA(cudaLaunchKernel(kern, dim3((unsigned)ctas), dim3(WB_SDF_TRAIN_TILE), args, (size_t)smem, (cudaStream_t)s));
+    wb_count_launch();
+    return WB_OK;
+}

@@ -634,6 +634,24 @@ def sdf_eval(nef, coords: torch.Tensor, lod_idx: Optional[int] = None) -> Option
     return out
 
 
+def sdf_train(fd, coords: torch.Tensor, sdf_gt: torch.Tensor, lod_idx: int, inv_count: float, grad_feats: Sequence[torch.Tensor],
+              grad_params: torch.Tensor, loss_out: torch.Tensor) -> None:
+    """Forward, L2 loss and backward of SDFTrainer.step (sdf_trainer.py:65-124) for one loss LOD in one launch (wb_sdf_train).
+    fd: sdf_field(nef) (its params pointer may be re-aimed at a flat decoder buffer); coords f32 [N,3], sdf_gt f32 [N] on the device.
+    Accumulates: loss_out[0] += sum (y - gt)^2 * inv_count, grad_params (packed like the decoder) and grad_feats[k], k <= lod_idx."""
+    d, oct, _ = fd
+    A.require_device(coords)
+    if not (coords.dtype == sdf_gt.dtype == grad_params.dtype == loss_out.dtype == torch.float32 and coords.is_contiguous() and sdf_gt.is_contiguous()):
+        raise A.WispB200Error("sdf_train wants contiguous float32 coords / sdf_gt and float32 gradient and loss buffers")
+    if sdf_gt.numel() != coords.shape[0]:
+        raise A.WispB200Error(f"sdf_gt has {sdf_gt.numel()} values for {coords.shape[0]} points")
+    gptrs = (C.c_void_p * len(grad_feats))(*[g.data_ptr() for g in grad_feats])
+    od = oct.desc()
+    with _stage("sdf_train"):
+        A.check(A.lib().wb_sdf_train(C.byref(od), C.byref(d), C.c_int32(lod_idx), A.ptr(coords), A.ptr(sdf_gt), C.c_int64(coords.shape[0]),
+                                     C.c_float(inv_count), gptrs, A.ptr(grad_params), A.ptr(loss_out), A.stream()))
+
+
 class _SdfState:
     """Per-pack state tensors of the sphere tracer (struct wb_sdf_state), owned by PyTorch."""
 

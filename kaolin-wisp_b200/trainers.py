@@ -246,3 +246,118 @@ class MultiviewStep:
                 dist.all_reduce(g, op=dist.ReduceOp.SUM, group=self.group)
         self.opt.step(grads, grad_scale=1.0 / world, zero_grad=False)
         return loss.detach()
+
+
+class SDFStep:
+    """The optimisation step of wisp.trainers.SDFTrainer (wisp/trainers/sdf_trainer.py:65-124) with the optimiser of
+    BaseTrainer.init_optimizer (wisp/trainers/base_trainer.py:205-239): parameter groups by name ('decoder' -> weight decay,
+    'grid' -> lr * grid_lr_weight, the rest -> lr; parameters with requires_grad=False are skipped, as torch.optim.Adam skips
+    them), loss = sum over loss_lods of sum((pred - gt)^2), divided by the batch size.  loss_lods is the last LOD when
+    `only_last` (nglod_octree.yaml), otherwise every LOD.
+
+    A NeuralSDF over an OctreeGrid with one hidden layer (every app/nglod octree config) trains natively: per loss LOD one
+    wb_sdf_train launch (forward, loss and backward, no autograd), then NativeAdam over every parameter in one launch.  The
+    decoder's parameters are flattened in place into one buffer, which the kernel reads, whose gradient it writes and which is
+    one Adam segment.  The decoder runs in fp32 whatever the autocast state; the reference's enable_amp fp16 nn.Linear is not
+    reproduced.  Every other field (NeuralSDF over a HashGrid or TriplanarGrid, deeper decoders) takes autograd plus the same
+    NativeAdam."""
+
+    def __init__(self, pipeline, lr: float = 1e-3, eps: float = 1e-15, weight_decay: float = 0.0, grid_lr_weight: float = 1.0,
+                 betas=(0.9, 0.999), only_last: bool = True):
+        self.pipeline, self.nef = pipeline, pipeline.nef
+        nef = self.nef
+        n = int(nef.grid.num_lods)
+        self.loss_lods = [n - 1] if only_last else list(range(n))            # sdf_trainer.py:55-58
+        named = [(k, p) for k, p in nef.named_parameters() if p.requires_grad]
+        if not named:
+            raise A.WispB200Error("SDFStep: the field has no trainable parameters")
+        A.require_device(named[0][1])                                         # no CPU fallback
+        self.device = named[0][1].device
+        self.fd = self._fused_field(nef, [p for _, p in named])
+        self.fused = self.fd is not None
+        if self.fused:
+            feats = list(nef.grid.features)
+            tensors = [(f.data, lr * grid_lr_weight, 0.0) for f in feats] + [(self.dec_flat, lr, weight_decay)]
+            self.g_feats = [torch.zeros_like(f.data) for f in feats]
+            self.g_dec = torch.zeros_like(self.dec_flat)
+        else:
+            tensors = [(p.data, lr if "decoder" in k or "grid" not in k else lr * grid_lr_weight, weight_decay if "decoder" in k else 0.0)
+                       for k, p in named]
+            self.params = [p for _, p in named]
+        self.opt = NativeAdam(tensors, betas=betas, eps=eps)
+        self.loss_buf = torch.zeros(1, dtype=torch.float32, device=self.device)
+
+    def _fused_field(self, nef, params):
+        """ops.sdf_field of the field with the decoder flattened in place and the description aimed at that buffer, or None when
+        the field is outside wb_sdf_train (not an OctreeGrid, not one hidden layer, or trainable parameters beyond grid and decoder)."""
+        grid, dec = getattr(nef, "grid", None), getattr(nef, "decoder", None)
+        if grid is None or dec is None or getattr(grid, "dictionary", None) is not None or len(getattr(dec, "layers", [])) != 1:
+            return None
+        feats = list(getattr(grid, "features", []))
+        if not feats or any(not isinstance(f, torch.Tensor) or f.dim() != 2 or f.shape[1] != grid.feature_dim or f.dtype != torch.float32 or not f.is_contiguous() for f in feats):
+            return None
+        dparams = ops.decoder_params(dec)
+        if {id(p) for p in params} != {id(p) for p in feats + dparams} or any(p.dtype != torch.float32 for p in dparams):
+            return None
+        if ops.sdf_field(nef) is None:
+            return None
+        self.dec_flat = _flatten_in_place(dparams)
+        fd = ops.sdf_field(nef)
+        d, oct, keep = fd
+        if any(d.feats[k] != f.data_ptr() for k, f in enumerate(feats)):
+            return None
+        d.params = self.dec_flat.data_ptr()
+        return d, oct, keep + [self.dec_flat]
+
+    def _lod_check(self, N: int) -> None:
+        g = self.nef.grid
+        if self.fused and g.multiscale_type == 'cat' and min(self.loss_lods) < g.num_lods - 1:
+            lin = self.nef.decoder.layers[0]
+            pd = lin.in_features - g.feature_dim * g.num_lods
+            k = min(self.loss_lods)
+            raise RuntimeError(f"mat1 and mat2 shapes cannot be multiplied ({N}x{pd + g.feature_dim * (k + 1)} and "
+                               f"{lin.in_features}x{lin.out_features})")      # what nn.Linear raises on a lower LOD of a 'cat' grid
+
+    def step(self, coords: torch.Tensor, sdf_gt: torch.Tensor, zero_grad: bool = True, update: bool = True) -> torch.Tensor:
+        """One optimisation step on (coords [N,3], sdf_gt [N,1]); returns the loss as a device scalar (no host sync).  Host tensors
+        are copied to the device (`.to(self.device)`, sdf_trainer.py:69-70).  `update=False` stops after the backward: the
+        gradients stay in g_feats / g_dec (autograd route: in the parameters' .grad), parameters and optimiser state untouched."""
+        pts, gts = coords.to(self.device), sdf_gt.to(self.device)
+        N = int(pts.shape[0])
+        if N == 0:
+            raise A.WispB200Error("SDFStep.step: empty batch (the reference divides the loss by the batch size)")
+        self._lod_check(N)
+        if not self.fused:
+            return self._step_autograd(pts, gts, N, update)
+        c, g = A.f32c(pts).reshape(-1, 3), A.f32c(gts).reshape(-1)
+        self.loss_buf.zero_()
+        for lod in self.loss_lods:
+            ops.sdf_train(self.fd, c, g, lod, 1.0 / N, self.g_feats, self.g_dec, self.loss_buf)
+        loss = self.loss_buf.clone()
+        if update:
+            with ops._stage("adam"):
+                self.opt.step(self.g_feats + [self.g_dec], grad_scale=1.0, zero_grad=zero_grad)
+        return loss[0]
+
+    def zero_grads(self) -> None:
+        """Clear every gradient accumulator (after a step(update=False) whose gradients were only inspected)."""
+        if self.fused:
+            for t in self.g_feats + [self.g_dec]:
+                t.zero_()
+        else:
+            for p in self.params:
+                p.grad = None
+
+    def _step_autograd(self, pts, gts, N, update):
+        for p in self.params:
+            p.grad = None                                                     # self.pipeline.zero_grad() (:77)
+        loss = 0.0
+        for lod in self.loss_lods:
+            pred = self.nef(coords=pts, lod_idx=lod, channels="sdf")
+            loss = loss + ((pred - 1.0 * gts) ** 2).sum()
+        loss = loss / N
+        loss.backward()
+        if update:
+            grads = [(p.grad if p.grad is not None else torch.zeros_like(p)).contiguous() for p in self.params]
+            self.opt.step(grads, grad_scale=1.0, zero_grad=False)
+        return loss.detach()
