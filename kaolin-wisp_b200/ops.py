@@ -588,7 +588,7 @@ def sdf_field(nef):
     if nh > 1 and H % 4:
         return None
     em = _sdf_embed_mode(nef)
-    if em is None or g.feature_dim > 64:
+    if em is None or em[1] > 10 or g.feature_dim > 64:          # wb_make_sdf: pos_freq <= 10, feature_dim <= 64
         return None
     dev = g.features[0].device
     blas = g.blas
@@ -610,7 +610,13 @@ def sdf_field(nef):
     d.pos_mode, d.pos_freq = em
     d.num_layers, d.hidden_dim, d.params = nh, H, params.data_ptr()
     pos_dim = 0 if em[0] == 0 else 3 if em[0] == 1 else 6 * em[1] + (3 if em[0] == 3 else 0)
-    if layers[0].in_features != pos_dim + (g.feature_dim if d.multiscale else g.feature_dim * g.num_lods):
+    in_dim = layers[0].in_features
+    if in_dim != pos_dim + (g.feature_dim if d.multiscale else g.feature_dim * g.num_lods):
+        return None
+    # the decoder input must be at most 132 wide and its shared-memory image must fit in 200 KB: the same limits and formula as
+    # wb_make_sdf (csrc/wb_sdf.cuh)
+    smem_floats = H * ((in_dim + 3) & ~3) + H + (nh - 1) * (H * H + H) + H + 4
+    if in_dim > 132 or smem_floats * 4 > 200 * 1024:
         return None
     return d, oct, [ptrs, feats, params, trinkets]
 

@@ -160,12 +160,14 @@ def neural_sdf(case, coords: np.ndarray, lod_idx=None) -> np.ndarray:
     return (h @ Ws[-1].T + bs[-1]).astype(np.float32)
 
 
-def sdf_trace(case, num_steps=64, step_size=1.0, min_dis=1e-4, lod_idx=None, dist_max=6.0, with_normals=True, return_debug=False):
+def sdf_trace(case, num_steps=64, step_size=1.0, min_dis=1e-4, lod_idx=None, dist_max=6.0, with_normals=True, return_debug=False, field=None):
     """PackedSDFTracer.trace (packed_sdf_tracer.py:78-174), statement by statement, on numpy arrays.
     Kept quirks: `t += dist` also advances packs that already terminated (so depth drifts by dist per executed iteration after
-    the hit while xyz does not); the loop ends when no pack is alive anywhere; find_depth_bound's bounds (see above)."""
+    the hit while xyz does not); the loop ends when no pack is alive anywhere; find_depth_bound's bounds (see above).
+    field(coords, lod_idx) -> [N,1] float32 is the SDF (default: the case's own NeuralSDF, neural_sdf)."""
     spc, o, d = case["spc"], case["origins"], case["dirs"]
     lod_idx = len(case["active_lods"]) - 1 if lod_idx is None else lod_idx
+    sdf = field or (lambda x, lod=None: neural_sdf(case, x, lod))
     rt = O.raytrace(spc, o, d, case["active_lods"][lod_idx])
     ridx, depth = rt["ridx"], rt["depth"].copy()
     R = o.shape[0]
@@ -187,7 +189,7 @@ def sdf_trace(case, num_steps=64, step_size=1.0, min_dis=1e-4, lod_idx=None, dis
     x = fma(t)
     dist = np.zeros_like(t)
     step = np.float32(step_size)
-    dist[mask] = neural_sdf(case, x[mask], lod_idx) * np.float32(1.0) * step
+    dist[mask] = sdf(x[mask], lod_idx) * np.float32(1.0) * step
     dist_prev = dist.copy()
     iters = 0
     for i in range(num_steps):
@@ -209,7 +211,7 @@ def sdf_trace(case, num_steps=64, step_size=1.0, min_dis=1e-4, lod_idx=None, dis
         x = np.where(mask[:, None], fma(t), x)
         if not mask.any():
             break
-        dist[mask] = neural_sdf(case, x[mask], lod_idx) * np.float32(1.0) * step
+        dist[mask] = sdf(x[mask], lod_idx) * np.float32(1.0) * step
     hb = np.zeros(R, bool); hb[first_ridx] = hit
     out["hit"] = hb
     out["xyz"][hb] = x[hit]; out["depth"][hb] = t[hit]
@@ -219,7 +221,7 @@ def sdf_trace(case, num_steps=64, step_size=1.0, min_dis=1e-4, lod_idx=None, dis
         g = []
         for a in range(3):
             e = np.zeros(3, np.float32); e[a] = eps
-            g.append(neural_sdf(case, xh + e) - neural_sdf(case, xh - e))     # lod_idx=None -> finest LOD (gradients.py:29-45)
+            g.append(sdf(xh + e) - sdf(xh - e))     # lod_idx=None -> finest LOD (gradients.py:29-45)
         grad = np.concatenate(g, -1) / np.float32(0.005 * 2.0) if xh.shape[0] else np.zeros((0, 3), np.float32)
         nrm = np.sqrt((grad.astype(np.float32) ** 2).sum(-1, keepdims=True))
         out["normal"][hb] = grad / np.maximum(nrm, np.float32(1e-5))
