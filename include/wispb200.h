@@ -251,14 +251,19 @@ typedef struct wb_sdf_desc {
 int wb_sdf_eval(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, const float* coords, int64_t N, float* sdf, wb_stream s);
 /* wb_sdf_train: one training launch of SDFTrainer.step (wisp/trainers/sdf_trainer.py:65-124) for the loss LOD lod_idx, over
  * NeuralSDF.sdf (wisp/models/nefs/neural_sdf.py:120-155): forward as wb_sdf_eval, loss and backward in the same kernel.
- *   coords f32 [N,3], sdf_gt f32 [N]; decoders with exactly one hidden layer (num_layers == 1).
+ *   coords f32 [N,3], sdf_gt f32 [N]; decoders with 1 to 4 hidden layers whose training footprint fits in shared memory
+ *   (wb_sdf_train_smem_bytes(nef) >= 0; otherwise the call fails).
  *   *loss_out     += sum_i (y_i - gt_i)^2 * inv_count               (inv_count = 1 / batch size: `loss /= batch_size`)
- *   grad_params   += dL/d params, packed like nef->params [W0, b0, Wout, bout]
+ *   grad_params   += dL/d params, packed like nef->params [W0, b0, W1, b1, ..., Wout, bout] (nn.Linear layout: W_k [H, in])
  *   grad_feats[k] += dL/d feats[k] for k = 0 .. lod_idx (HOST array of device pointers, shapes of nef->feats), fp32, as
  *                    wb_octree_interp_bwd: no gradient to the coordinates, the fp16 rounding of the forward passed straight through.
  * Everything accumulates: the caller zeroes loss_out and the gradients; a loss over several LODs is one call per LOD. */
 int wb_sdf_train(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, const float* coords, const float* sdf_gt, int64_t N,
                  float inv_count, float* const* grad_feats, float* grad_params, float* loss_out, wb_stream s);
+/* Dynamic shared memory (bytes) of a wb_sdf_train launch for this field, or < 0 when wb_sdf_train cannot train it (a description
+ * wb_sdf_eval refuses, or a decoder with more than one hidden layer whose weights, weight-gradient accumulators and a 32-sample
+ * tile exceed 227 KB).  Host only: no device is touched. */
+int64_t wb_sdf_train_smem_bytes(const wb_sdf_desc* nef);
 /* Per-pack state of the sphere tracer (pack = ray with >= 1 nugget).  All device pointers, allocated by the caller for R rays;
  * nothing needs initialising.  state bit 0 = alive (the reference's `mask`), bit 1 = hit. */
 typedef struct wb_sdf_state {

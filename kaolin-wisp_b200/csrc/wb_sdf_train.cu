@@ -3,6 +3,7 @@
 // The reference runs the grid kernel, a cat, two cuBLAS GEMMs, the loss ops and their autograd backward (cuBLAS + the grid
 // scatter) per LOD.
 //
+// One hidden layer (wb_sdf_train_kernel; decoders with 2 to 4 hidden layers: wb_sdf_train_deep_kernel below).
 // A CTA works on tiles of WB_SDF_TRAIN_TILE samples, grid-stride:
 //   pass 1, thread per sample: the forward of wb_sdf_eval (wb_sdf.cuh: same features, same summation order, so the same y), the
 //     loss, and dL/dx = dy * sum_{j: a_j > 0} wout_j W0[j,:], whose feature part is scattered into the grid gradients at once with
@@ -216,11 +217,252 @@ wb_sdf_train_kernel(WbOct oc, WbSdf m, WbGridX gx, int nl, WbSdfTrain T)
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// decoders with 2 to 4 hidden layers (H % 4 == 0): layer by layer over a tile of T samples, everything in shared memory
+// ---------------------------------------------------------------------------------------------------------------------
+// Shared memory: the decoder image (sdf_stage) | the CTA's decoder-gradient accumulators in the image's layout | the tile: x
+// [T][SX] | h_0 .. h_{nh-1} [T][SH] | dy [T] | reduction.  Row strides SX, SH = 4 (mod 32) floats: the layer loops put one sample
+// per lane and read a float4 of its row, eight lanes per wavefront hit 32 distinct banks.
+//   forward   layer k, thread per (sample, 4 units): wb_sdf_eval's chains (per unit seeded with the bias, over the inputs in order;
+//             the output over the units in order), so the same y; relu(a) kept per layer (a > 0 <=> relu(a) > 0: the mask)
+//   backward  delta_{nh-1} = relu'(a) * fl(dy wout), then for k = nh-1 .. 0: dL/dW_k += delta_k^T h_{k-1} (4x4 register blocks,
+//             a chain over the CTA's samples in order), dL/db_k += delta_k (thread per unit), and delta_{k-1} = relu'(a_{k-1}) *
+//             W_k^T delta_k (a chain over the units in order) written over h_{k-1}; through W0 the feature columns of the input
+//             gradient, scattered as the one-layer kernel does.
+// T (a multiple of 32, at most 128) is the largest tile that fits next to the image and the accumulators (sdf_train_plan).
+constexpr int WB_SDF_DEEP_THREADS = 256;
+
+struct WbSdfTrainDeep {
+    const float* coords; const float* gt; int64_t N; float inv_count;
+    float* gparams; float* loss;
+    int T, SX, SH;                        // tile, row strides of x and of the hidden rows (floats)
+    int acc_off, tile_off, red_off;       // shared-memory offsets (floats)
+};
+
+static inline int sdf_deep_stride(int n) { return ((n + 31) & ~31) + 4; }
+
+// out[s][j] = relu(b[j] + sum_{i < IN} W[j][i] in[s][i]) for s < cnt, four units per thread
+__device__ __forceinline__ void sdf_deep_fwd(const float* W, int ldw, const float* b, int IN, int H, const float* in, int ldi, float* out, int ldo,
+                                             int T, int cnt)
+{
+    const int items = T * (H / 4);
+    for (int e = threadIdx.x; e < items; e += blockDim.x) {
+        const int s = e % T, j = (e / T) * 4;
+        if (s >= cnt) continue;
+        const float* x = in + s * ldi;
+        const float* w0 = W + j * ldw; const float* w1 = w0 + ldw; const float* w2 = w1 + ldw; const float* w3 = w2 + ldw;
+        float a0 = b[j], a1 = b[j + 1], a2 = b[j + 2], a3 = b[j + 3];
+        int i = 0;
+        for (; i + 4 <= IN; i += 4) {
+            const float4 v = *reinterpret_cast<const float4*>(x + i);
+            const float4 u0 = *reinterpret_cast<const float4*>(w0 + i), u1 = *reinterpret_cast<const float4*>(w1 + i);
+            const float4 u2 = *reinterpret_cast<const float4*>(w2 + i), u3 = *reinterpret_cast<const float4*>(w3 + i);
+            a0 = fmaf(u0.x, v.x, a0); a1 = fmaf(u1.x, v.x, a1); a2 = fmaf(u2.x, v.x, a2); a3 = fmaf(u3.x, v.x, a3);
+            a0 = fmaf(u0.y, v.y, a0); a1 = fmaf(u1.y, v.y, a1); a2 = fmaf(u2.y, v.y, a2); a3 = fmaf(u3.y, v.y, a3);
+            a0 = fmaf(u0.z, v.z, a0); a1 = fmaf(u1.z, v.z, a1); a2 = fmaf(u2.z, v.z, a2); a3 = fmaf(u3.z, v.z, a3);
+            a0 = fmaf(u0.w, v.w, a0); a1 = fmaf(u1.w, v.w, a1); a2 = fmaf(u2.w, v.w, a2); a3 = fmaf(u3.w, v.w, a3);
+        }
+        for (; i < IN; ++i) {
+            const float v = x[i];
+            a0 = fmaf(w0[i], v, a0); a1 = fmaf(w1[i], v, a1); a2 = fmaf(w2[i], v, a2); a3 = fmaf(w3[i], v, a3);
+        }
+        *reinterpret_cast<float4*>(out + s * ldo + j) = make_float4(fmaxf(a0, 0.0f), fmaxf(a1, 0.0f), fmaxf(a2, 0.0f), fmaxf(a3, 0.0f));
+    }
+}
+
+// out[s][i] = sum_{j < H} W[j][i] d[s][j] (units in order) for s < cnt and i in [i0, i1) (multiples of 4), four inputs per thread;
+// mask: zero where the old out[s][i] (the forward's relu(a)) is not positive
+__device__ __forceinline__ void sdf_deep_bwd(const float* W, int ldw, int H, const float* d, int ldd, float* out, int ldo, int i0, int i1, bool mask,
+                                             int T, int cnt)
+{
+    const int items = T * ((i1 - i0) / 4);
+    for (int e = threadIdx.x; e < items; e += blockDim.x) {
+        const int s = e % T, i = i0 + (e / T) * 4;
+        if (s >= cnt) continue;
+        const float* dr = d + s * ldd;
+        float g0 = 0.0f, g1 = 0.0f, g2 = 0.0f, g3 = 0.0f;
+        for (int j = 0; j < H; j += 4) {
+            const float4 dv = *reinterpret_cast<const float4*>(dr + j);
+            const float dd[4] = { dv.x, dv.y, dv.z, dv.w };
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const float4 u = *reinterpret_cast<const float4*>(W + (j + r) * ldw + i);
+                g0 = fmaf(u.x, dd[r], g0); g1 = fmaf(u.y, dd[r], g1); g2 = fmaf(u.z, dd[r], g2); g3 = fmaf(u.w, dd[r], g3);
+            }
+        }
+        float4* o = reinterpret_cast<float4*>(out + s * ldo + i);
+        if (mask) {
+            const float4 h = *o;
+            g0 = h.x > 0.0f ? g0 : 0.0f; g1 = h.y > 0.0f ? g1 : 0.0f; g2 = h.z > 0.0f ? g2 : 0.0f; g3 = h.w > 0.0f ? g3 : 0.0f;
+        }
+        *o = make_float4(g0, g1, g2, g3);
+    }
+}
+
+// G[j][i] += sum_{s < cnt} d[s][j] in[s][i] (samples in order) for j < H, i < INP (multiples of 4), 4 x 4 per thread;
+// gb[j] += sum_{s < cnt} d[s][j], thread per unit
+__device__ __forceinline__ void sdf_deep_grad(float* G, int ldg, float* gb, int H, int INP, const float* d, int ldd, const float* in, int ldi, int cnt)
+{
+    const int nib = INP / 4, items = (H / 4) * nib;
+    for (int e = threadIdx.x; e < items; e += blockDim.x) {
+        const int i = (e % nib) * 4, j = (e / nib) * 4;
+        float acc[4][4];
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const float4 v = *reinterpret_cast<const float4*>(G + (j + r) * ldg + i);
+            acc[r][0] = v.x; acc[r][1] = v.y; acc[r][2] = v.z; acc[r][3] = v.w;
+        }
+        for (int s = 0; s < cnt; ++s) {
+            const float4 dv = *reinterpret_cast<const float4*>(d + s * ldd + j);
+            const float4 xv = *reinterpret_cast<const float4*>(in + s * ldi + i);
+            const float dd[4] = { dv.x, dv.y, dv.z, dv.w };
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                acc[r][0] = fmaf(dd[r], xv.x, acc[r][0]); acc[r][1] = fmaf(dd[r], xv.y, acc[r][1]);
+                acc[r][2] = fmaf(dd[r], xv.z, acc[r][2]); acc[r][3] = fmaf(dd[r], xv.w, acc[r][3]);
+            }
+        }
+#pragma unroll
+        for (int r = 0; r < 4; ++r) *reinterpret_cast<float4*>(G + (j + r) * ldg + i) = make_float4(acc[r][0], acc[r][1], acc[r][2], acc[r][3]);
+    }
+    if (threadIdx.x < H) {
+        const int j = threadIdx.x;
+        float a = gb[j];
+        for (int s = 0; s < cnt; ++s) a += d[s * ldd + j];
+        gb[j] = a;
+    }
+}
+
+__global__ void __launch_bounds__(WB_SDF_DEEP_THREADS)
+wb_sdf_train_deep_kernel(WbOct oc, WbSdf m, WbGridX gx, int nl, WbSdfTrainDeep T)
+{
+    extern __shared__ __align__(16) float sw[];
+    const int H = m.H, INP = m.in_pad, IN = m.in_dim, nh = m.nh, tid = threadIdx.x;
+    const int TS = T.T, SX = T.SX, SH = T.SH;
+    float* acc = sw + T.acc_off;
+    for (int e = tid; e < m.smem_floats; e += blockDim.x) acc[e] = 0.0f;
+    sdf_stage(m, sw);
+    float* xs = sw + T.tile_off;
+    float* hs = xs + TS * SX;                              // h_k: hs + k * TS * SH
+    float* dys = hs + nh * TS * SH;
+    const int lw = H * INP + H + (nh - 1) * (H * H + H);   // offset of wout in the image and in acc
+    const float* wo = sw + lw;
+    float lsum = 0.0f, dsum = 0.0f;
+    for (int64_t base = (int64_t)blockIdx.x * TS; base < T.N; base += (int64_t)gridDim.x * TS) {
+        const int cnt = (int)min((int64_t)TS, T.N - base);
+        if (tid < cnt) {                                   // decoder input of sample tid
+            const int64_t i = base + tid;
+            float* xr = xs + tid * SX;
+            const float x = __ldg(T.coords + 3 * i), y = __ldg(T.coords + 3 * i + 1), z = __ldg(T.coords + 3 * i + 2);
+            const int pd = sdf_embed(m.pos_mode, m.pos_freq, x, y, z, xr);
+            sdf_features<0>(oc, m, nl, x, y, z, xr + pd);
+            for (int k = IN; k < INP; ++k) xr[k] = 0.0f;
+        }
+        __syncthreads();
+        for (int l = 0; l < nh; ++l) {
+            const float* Wl = l == 0 ? sw : sw + H * INP + H + (l - 1) * (H * H + H);
+            sdf_deep_fwd(Wl, l == 0 ? INP : H, Wl + (l == 0 ? H * INP : H * H), l == 0 ? IN : H, H,
+                         l == 0 ? xs : hs + (l - 1) * TS * SH, l == 0 ? SX : SH, hs + l * TS * SH, SH, TS, cnt);
+            __syncthreads();
+        }
+        float* top = hs + (nh - 1) * TS * SH;
+        if (tid < cnt) {                                   // output, loss, dy
+            const float* hr = top + tid * SH;
+            float out = wo[H];
+            for (int j = 0; j < H; j += 4) {
+                const float4 v = *reinterpret_cast<const float4*>(hr + j);
+                out = fmaf(wo[j], v.x, out); out = fmaf(wo[j + 1], v.y, out); out = fmaf(wo[j + 2], v.z, out); out = fmaf(wo[j + 3], v.w, out);
+            }
+            const float d = out - __ldg(T.gt + base + tid);
+            lsum = fmaf(d, d, lsum);
+            const float dy = T.inv_count * (2.0f * d);
+            dys[tid] = dy; dsum += dy;
+        }
+        __syncthreads();
+        if (tid < H) {                                     // dL/dwout, and delta of the last hidden layer over its activations
+            const int j = tid;
+            const float woj = wo[j];
+            float g = acc[lw + j];
+            for (int s = 0; s < cnt; ++s) {
+                const float ds = dys[s], h = top[s * SH + j];
+                g = fmaf(ds, h, g);
+                top[s * SH + j] = h > 0.0f ? ds * woj : 0.0f;
+            }
+            acc[lw + j] = g;
+        }
+        __syncthreads();
+        for (int l = nh - 1; l >= 0; --l) {
+            const int wof = l == 0 ? 0 : H * INP + H + (l - 1) * (H * H + H), ldw = l == 0 ? INP : H;
+            const float* dl = hs + l * TS * SH;
+            float* in = l == 0 ? xs : hs + (l - 1) * TS * SH;
+            const int ldi = l == 0 ? SX : SH;
+            sdf_deep_grad(acc + wof, ldw, acc + wof + H * ldw, H, ldw, dl, SH, in, ldi, cnt);
+            __syncthreads();
+            // l > 0: delta_{l-1} over h_{l-1}; l == 0: the input gradient's feature columns over x (x is no longer needed)
+            const int pd4 = l == 0 ? m.pos_dim & ~3 : 0;
+            sdf_deep_bwd(sw + wof, ldw, H, dl, SH, in, ldi, pd4, ldw, l > 0, TS, cnt);
+            __syncthreads();
+        }
+        if (tid < cnt) {
+            const int64_t i = base + tid;
+            const float* gr = xs + tid * SX + m.pos_dim;
+            wb_featx_scatter(gx, __ldg(T.coords + 3 * i), __ldg(T.coords + 3 * i + 1), __ldg(T.coords + 3 * i + 2), [&](int f) { return gr[f]; });
+        }
+        __syncthreads();
+    }
+    // flush: the decoder gradients of this CTA (W0 rows from in_pad to in_dim wide, the rest as packed), then loss and dL/dbout
+    float* gp = T.gparams;
+    const int P0 = H * INP;
+    for (int e = tid; e < P0; e += blockDim.x) {
+        const int j = e / INP, k = e - j * INP;
+        const float v = acc[e];
+        if (k < IN && v != 0.0f) atomicAdd(gp + j * IN + k, v);
+    }
+    for (int e = P0 + tid; e < lw + H; e += blockDim.x) { const float v = acc[e]; if (v != 0.0f) atomicAdd(gp + H * IN + (e - P0), v); }
+    float* red = sw + T.red_off;
+    lsum = wb_warp_sum(lsum); dsum = wb_warp_sum(dsum);
+    if ((tid & 31) == 0) { red[2 * (tid >> 5)] = lsum; red[2 * (tid >> 5) + 1] = dsum; }
+    __syncthreads();
+    if (tid == 0) {
+        float l = 0.0f, d = 0.0f;
+        for (int w = 0; w < WB_SDF_DEEP_THREADS / 32; ++w) { l += red[2 * w]; d += red[2 * w + 1]; }
+        if (l != 0.0f) atomicAdd(T.loss, l * T.inv_count);
+        if (d != 0.0f) atomicAdd(gp + H * IN + (lw + H - P0), d);
+    }
+}
+
+// shared memory of a wb_sdf_train launch (bytes) and its sample tile, or -1 when the field's training footprint does not fit
+static int sdf_train_plan(const WbSdf& m, int* tile)
+{
+    const int limit = 227 * 1024;
+    if (m.nh == 1) {
+        const int xs_off = (m.smem_floats + 3) & ~3;
+        const int red_off = xs_off + WB_SDF_TRAIN_TILE * m.in_pad + WB_SDF_TRAIN_TILE + (sdf_fast_shape(m) ? 0 : m.H * (m.in_pad + 1));
+        const int smem = (red_off + 2 * (WB_SDF_TRAIN_TILE / 32)) * 4;
+        *tile = WB_SDF_TRAIN_TILE;
+        return smem <= limit ? smem : -1;
+    }
+    const int img = (m.smem_floats + 3) & ~3, row = sdf_deep_stride(m.in_pad) + m.nh * sdf_deep_stride(m.H) + 1;
+    for (int t = 128; t >= 32; t -= 32) {
+        const int smem = (2 * img + t * row + 2 * (WB_SDF_DEEP_THREADS / 32)) * 4;
+        if (smem <= limit) { *tile = t; return smem; }
+    }
+    return -1;
+}
+
+extern "C" int64_t wb_sdf_train_smem_bytes(const wb_sdf_desc* nef)
+{
+    WbSdf m; if (wb_make_sdf(nef, &m)) return -1;
+    int tile = 0;
+    return sdf_train_plan(m, &tile);
+}
+
 extern "C" int wb_sdf_train(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, const float* coords, const float* sdf_gt, int64_t N,
                             float inv_count, float* const* grad_feats, float* grad_params, float* loss_out, wb_stream s)
 {
     WbSdf m; int rc = wb_make_sdf(nef, &m); if (rc) return rc;
-    WB_CHECK_ARG(m.nh == 1, "the fused training step covers decoders with exactly one hidden layer (num_layers == 1)");
+    int tile = 0; const int smem = sdf_train_plan(m, &tile);
+    WB_CHECK_ARG(smem > 0, "decoder weights, their gradient accumulators and a 32-sample tile exceed shared memory (wb_sdf_train_smem_bytes < 0)");
     WB_CHECK_ARG(lod_idx >= 0 && lod_idx < m.num_lods, "lod_idx out of range");
     WB_CHECK_ARG(m.multiscale == 1 || lod_idx == m.num_lods - 1, "'cat' grids feed the decoder all LODs: lod_idx must be num_lods-1");
     WB_CHECK_ARG(coords && sdf_gt && grad_feats && grad_params && loss_out && N >= 0, "null pointer");
@@ -236,20 +478,34 @@ extern "C" int wb_sdf_train(const wb_octree* oct, const wb_sdf_desc* nef, int32_
         WB_CHECK_ARG(!fast || (reinterpret_cast<uintptr_t>(grad_feats[k]) & 15u) == 0, "gradient levels must be 16-byte aligned");
         gx.ptr[k] = m.feats[k]; gx.gptr[k] = grad_feats[k];
     }
+    int nl = lod_idx + 1;
+    if (m.nh > 1) {
+        WbSdfTrainDeep D;
+        D.coords = coords; D.gt = sdf_gt; D.N = N; D.inv_count = inv_count; D.gparams = grad_params; D.loss = loss_out;
+        D.T = tile; D.SX = sdf_deep_stride(m.in_pad); D.SH = sdf_deep_stride(m.H);
+        D.acc_off = (m.smem_floats + 3) & ~3; D.tile_off = 2 * D.acc_off; D.red_off = D.tile_off + tile * (D.SX + m.nh * D.SH + 1);
+        const void* kern = (const void*)wb_sdf_train_deep_kernel;
+        WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        int per_sm = 0;
+        WB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, WB_SDF_DEEP_THREADS, smem));
+        WB_CHECK_ARG(per_sm >= 1, "training kernel does not fit on an SM");
+        int64_t ctas = (N + tile - 1) / tile; const int64_t cap = (int64_t)wb_num_sms() * per_sm; if (ctas > cap) ctas = cap;
+        void* args[] = { &oc, &m, &gx, &nl, &D };
+        WB_CUDA(cudaLaunchKernel(kern, dim3((unsigned)ctas), dim3(WB_SDF_DEEP_THREADS), args, (size_t)smem, (cudaStream_t)s));
+        wb_count_launch();
+        return WB_OK;
+    }
     WbSdfTrain T;
     T.coords = coords; T.gt = sdf_gt; T.N = N; T.inv_count = inv_count; T.gparams = grad_params; T.loss = loss_out;
     T.xs_off = (m.smem_floats + 3) & ~3;
     T.gw_off = T.xs_off + WB_SDF_TRAIN_TILE * m.in_pad + WB_SDF_TRAIN_TILE;
     T.red_off = T.gw_off + (fast ? 0 : m.H * (m.in_pad + 1));
-    const int smem = (T.red_off + 2 * (WB_SDF_TRAIN_TILE / 32)) * 4;
-    WB_CHECK_ARG(smem <= 227 * 1024, "decoder does not fit in shared memory");
     const void* kern = fast ? (const void*)wb_sdf_train_kernel<16, 1> : (const void*)wb_sdf_train_kernel<0, 0>;
     if (smem > 48 * 1024) WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     int per_sm = 0;
     WB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, WB_SDF_TRAIN_TILE, smem));
     WB_CHECK_ARG(per_sm >= 1, "training kernel does not fit on an SM");
     int64_t ctas = (N + WB_SDF_TRAIN_TILE - 1) / WB_SDF_TRAIN_TILE; const int64_t cap = (int64_t)wb_num_sms() * per_sm; if (ctas > cap) ctas = cap;
-    int nl = lod_idx + 1;
     void* args[] = { &oc, &m, &gx, &nl, &T };
     WB_CUDA(cudaLaunchKernel(kern, dim3((unsigned)ctas), dim3(WB_SDF_TRAIN_TILE), args, (size_t)smem, (cudaStream_t)s));
     wb_count_launch();

@@ -640,11 +640,18 @@ def sdf_eval(nef, coords: torch.Tensor, lod_idx: Optional[int] = None) -> Option
     return out
 
 
+def sdf_train_smem_bytes(fd) -> int:
+    """Shared memory of a wb_sdf_train launch for the field fd = sdf_field(nef), or < 0 when the fused step cannot train it
+    (its weights, weight-gradient accumulators and smallest sample tile exceed an SM's shared memory)."""
+    return int(A.lib().wb_sdf_train_smem_bytes(C.byref(fd[0])))
+
+
 def sdf_train(fd, coords: torch.Tensor, sdf_gt: torch.Tensor, lod_idx: int, inv_count: float, grad_feats: Sequence[torch.Tensor],
               grad_params: torch.Tensor, loss_out: torch.Tensor) -> None:
-    """Forward, L2 loss and backward of SDFTrainer.step (sdf_trainer.py:65-124) for one loss LOD in one launch (wb_sdf_train).
-    fd: sdf_field(nef) (its params pointer may be re-aimed at a flat decoder buffer); coords f32 [N,3], sdf_gt f32 [N] on the device.
-    Accumulates: loss_out[0] += sum (y - gt)^2 * inv_count, grad_params (packed like the decoder) and grad_feats[k], k <= lod_idx."""
+    """Forward, L2 loss and backward of SDFTrainer.step (sdf_trainer.py:65-124) for one loss LOD in one launch (wb_sdf_train), for
+    decoders of 1 to 4 hidden layers whose sdf_train_smem_bytes(fd) >= 0.  fd: sdf_field(nef) (its params pointer may be re-aimed
+    at a flat decoder buffer); coords f32 [N,3], sdf_gt f32 [N] on the device.  Accumulates: loss_out[0] += sum (y - gt)^2 *
+    inv_count, grad_params (packed like the decoder: [W0, b0, W1, b1, ..., Wout, bout]) and grad_feats[k], k <= lod_idx."""
     d, oct, _ = fd
     A.require_device(coords)
     if not (coords.dtype == sdf_gt.dtype == grad_params.dtype == loss_out.dtype == torch.float32 and coords.is_contiguous() and sdf_gt.is_contiguous()):

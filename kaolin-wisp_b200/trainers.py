@@ -255,12 +255,13 @@ class SDFStep:
     them), loss = sum over loss_lods of sum((pred - gt)^2), divided by the batch size.  loss_lods is the last LOD when
     `only_last` (nglod_octree.yaml), otherwise every LOD.
 
-    A NeuralSDF over an OctreeGrid with one hidden layer (every app/nglod octree config) trains natively: per loss LOD one
-    wb_sdf_train launch (forward, loss and backward, no autograd), then NativeAdam over every parameter in one launch.  The
-    decoder's parameters are flattened in place into one buffer, which the kernel reads, whose gradient it writes and which is
-    one Adam segment.  The decoder runs in fp32 whatever the autocast state; the reference's enable_amp fp16 nn.Linear is not
-    reproduced.  Every other field (NeuralSDF over a HashGrid or TriplanarGrid, deeper decoders) takes autograd plus the same
-    NativeAdam."""
+    A NeuralSDF over an OctreeGrid with 1 to 4 hidden layers (every app/nglod octree config, with any nef.num_layers up to 4)
+    trains natively: per loss LOD one wb_sdf_train launch (forward, loss and backward, no autograd), then NativeAdam over every
+    parameter in one launch.  The decoder's parameters are flattened in place into one buffer [W0, b0, W1, b1, ..., Wout, bout],
+    which the kernel reads, whose gradient it writes and which is one Adam segment.  The decoder runs in fp32 whatever the
+    autocast state; the reference's enable_amp fp16 nn.Linear is not reproduced.  Every other field (NeuralSDF over a HashGrid
+    or TriplanarGrid, a deeper decoder whose weights, weight-gradient accumulators and smallest sample tile exceed an SM's shared
+    memory: wb_sdf_train_smem_bytes < 0) takes autograd plus the same NativeAdam."""
 
     def __init__(self, pipeline, lr: float = 1e-3, eps: float = 1e-15, weight_decay: float = 0.0, grid_lr_weight: float = 1.0,
                  betas=(0.9, 0.999), only_last: bool = True):
@@ -289,9 +290,10 @@ class SDFStep:
 
     def _fused_field(self, nef, params):
         """ops.sdf_field of the field with the decoder flattened in place and the description aimed at that buffer, or None when
-        the field is outside wb_sdf_train (not an OctreeGrid, not one hidden layer, or trainable parameters beyond grid and decoder)."""
+        the field is outside wb_sdf_train (not an OctreeGrid, a decoder whose training footprint exceeds shared memory, or
+        trainable parameters beyond grid and decoder)."""
         grid, dec = getattr(nef, "grid", None), getattr(nef, "decoder", None)
-        if grid is None or dec is None or getattr(grid, "dictionary", None) is not None or len(getattr(dec, "layers", [])) != 1:
+        if grid is None or dec is None or getattr(grid, "dictionary", None) is not None:
             return None
         feats = list(getattr(grid, "features", []))
         if not feats or any(not isinstance(f, torch.Tensor) or f.dim() != 2 or f.shape[1] != grid.feature_dim or f.dtype != torch.float32 or not f.is_contiguous() for f in feats):
@@ -299,7 +301,8 @@ class SDFStep:
         dparams = ops.decoder_params(dec)
         if {id(p) for p in params} != {id(p) for p in feats + dparams} or any(p.dtype != torch.float32 for p in dparams):
             return None
-        if ops.sdf_field(nef) is None:
+        fd = ops.sdf_field(nef)
+        if fd is None or ops.sdf_train_smem_bytes(fd) < 0:
             return None
         self.dec_flat = _flatten_in_place(dparams)
         fd = ops.sdf_field(nef)

@@ -5,7 +5,10 @@ inputs, alternating the two arms.  Prints one JSON line: ms/step, samples/s and 
 size, the device name and power limit, and a parity block (SDFStep's gradients against the autograd route at batch 65 536; a
 parity failure fails the run).
 
-    python tools/bench_sdf_step.py [--steps 200] [--warmup 20] [--batches 512,65536,1048576]
+    python tools/bench_sdf_step.py [--steps 200] [--warmup 20] [--batches 512,65536,1048576] [--num-layers 1] [--hidden-dim 128]
+
+--num-layers / --hidden-dim replace config 3's decoder (19-128-1) by one with that many hidden layers of that width
+(oracle.sdf_reference.random_decoder, seeded); the grid and the samples stay config 3's.
 """
 from __future__ import annotations
 
@@ -65,6 +68,8 @@ def main():
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--batches", default="512,65536,1048576")
+    ap.add_argument("--num-layers", type=int, default=1)
+    ap.add_argument("--hidden-dim", type=int, default=128)
     args = ap.parse_args()
     import wisp_b200 as W
     from oracle import octree_grid as OG
@@ -72,6 +77,9 @@ def main():
     assert torch.cuda.is_available(), "bench_sdf_step.py measures on a CUDA device"
     torch.cuda.set_device(0)
     case = OG.make_sdf_case(level=7, num_lods=6, feature_dim=16, hidden_dim=128, multiscale="sum", res=4, seed=11, feature_std=0.02)
+    if (args.num_layers, args.hidden_dim) != (1, 128):
+        from oracle import sdf_reference as S
+        case["W"], case["b"] = S.random_decoder(np.random.default_rng(4), 19, 1, args.hidden_dim, args.num_layers, scale=0.2)
     lr, eps = 1e-3, 1e-15
 
     # parity: SDFStep's gradients and loss against the autograd route at batch 65 536
@@ -122,7 +130,7 @@ def main():
                         for k, v in res.items()}
         arms[str(B)]["speedup"] = arms[str(B)]["autograd"]["ms_per_step"] / arms[str(B)]["native"]["ms_per_step"]
     name, power = _gpu_info()
-    print(json.dumps(dict(workload="sdf_step_config3", device=name, power_limit=power, steps=args.steps, warmup=args.warmup,
+    print(json.dumps(dict(workload="sdf_step_config3", num_layers=args.num_layers, hidden_dim=args.hidden_dim, fused=step.fused, device=name, power_limit=power, steps=args.steps, warmup=args.warmup,
                           batches=arms, parity=parity)))
     if not parity["ok"]:
         sys.exit(1)

@@ -3,16 +3,17 @@
 (wisp/trainers/sdf_trainer.py:65-124) with the optimiser of its BaseTrainer.init_optimizer (wisp/trainers/base_trainer.py:205-239),
 run on CPU from an UNMODIFIED kaolin-wisp checkout (TEST INFRASTRUCTURE).
 
-    python tools/make_sdf_train_golden.py [path/to/kaolin-wisp]
+    python tools/make_sdf_train_golden.py [--deep] [path/to/kaolin-wisp]
 
-Writes only sdf_train.npz.  Kaolin calls are answered by the oracle (oracle/ref_import.py).  The two trainer modules are loaded
+Writes only sdf_train.npz, or with --deep only sdf_train_deep.npz.  Kaolin calls are answered by the oracle (oracle/ref_import.py).  The two trainer modules are loaded
 from their files; the trainer object is created without its constructor and given what step() and init_optimizer() read.
 init_optimizer's `instantiate(cfg.optimizer, params=groups)` is answered by torch.optim.Adam(groups, lr, betas, eps): the decoder
 group carries its weight decay, the grid and rest groups Adam's default of none (the reference's instantiate would also pass
 cfg.optimizer.weight_decay as that default; the nglod configs train with weight_decay 0, where the two agree).
 
 Cases (the octahedron model of oracle/make_golden.py:gen_sdf at level 5, 3 LODs, F = 8, H = 16): 'sum' and 'cat' with only_last,
-and 'sum' over all LODs.  grid_lr_weight = 5 and weight_decay = 1e-2 so that every group is pinned.  Recorded per case: the initial
+and 'sum' over all LODs, with one hidden layer; --deep: 'sum' only_last with 2 hidden layers, 'cat' only_last with 3, and 'sum'
+over all LODs with 2 (the deeper layers pass the six |x|-units through unchanged, as oracle.sdf_reference.random_decoder).  grid_lr_weight = 5 and weight_decay = 1e-2 so that every group is pinned.  Recorded per case: the initial
 parameters, the loss of each step, the gradients of step 1 (after backward(), before optimizer.step()) and the parameters after
 steps 1 and 3."""
 from __future__ import annotations
@@ -30,7 +31,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 LR, EPS, WD, GRID_LR_WEIGHT, STEPS, N = 1e-3, 1e-15, 1e-2, 5.0, 3, 256
-CASES = {"sum": ("sum", True), "cat": ("cat", True), "sum_all": ("sum", False)}
+CASES = {"sum": ("sum", True, 1), "cat": ("cat", True, 1), "sum_all": ("sum", False, 1)}
+DEEP_CASES = {"sum": ("sum", True, 2), "cat": ("cat", True, 3), "sum_all": ("sum", False, 2)}
 
 
 def _load(name, path):
@@ -47,8 +49,11 @@ def _params(nef):
 def main():
     from oracle import oracle as O
     from oracle import ref_import
-    if len(sys.argv) > 1:
-        ref_import.REF_ROOT = sys.argv[1]
+    args = sys.argv[1:]
+    deep = "--deep" in args
+    args = [a for a in args if a != "--deep"]
+    if args:
+        ref_import.REF_ROOT = args[0]
     warnings.filterwarnings("ignore")
     ref_import.install()
     import wisp.models, wisp.models.pipeline, wisp.framework, wisp.datasets, wisp.trainers     # noqa: F401
@@ -66,15 +71,18 @@ def main():
     coords = rng.uniform(-0.7, 0.7, (N, 3)).astype(np.float32)
     sdf = ((np.abs(coords).sum(-1, keepdims=True) - 0.3) / np.sqrt(3.0) + rng.normal(0.0, 0.01, (N, 1))).astype(np.float32)
     out = dict(octree=oct_np, level=level, coords=coords, sdf=sdf, lr=LR, eps=EPS, weight_decay=WD, grid_lr_weight=GRID_LR_WEIGHT)
-    for name, (ms, only_last) in CASES.items():
+    for name, (ms, only_last, layers) in (DEEP_CASES if deep else CASES).items():
         torch.manual_seed(7)
         blas = OctreeAS(torch.from_numpy(oct_np))
         grid = OctreeGrid(blas, feature_dim=8, num_lods=3, interpolation_type='linear', multiscale_type=ms, feature_std=0.05)
-        nef = NeuralSDF(grid, pos_embedder='none', position_input=True, hidden_dim=16, num_layers=1)
+        nef = NeuralSDF(grid, pos_embedder='none', position_input=True, hidden_dim=16, num_layers=layers)
         with torch.no_grad():       # sdf ~ (|x|+|y|+|z|)/sqrt(3) - 0.3 + small learned perturbation (as gen_sdf)
             W0 = nef.decoder.layers[0].weight; W0.mul_(0.05)
             W0[:6, :3] = torch.tensor([[1, 0, 0], [-1, 0, 0], [0, 1, 0], [0, -1, 0], [0, 0, 1], [0, 0, -1.0]])
             nef.decoder.layers[0].bias.uniform_(-0.05, 0.05)
+            for l in list(nef.decoder.layers)[1:]:
+                l.weight.mul_(0.05); l.weight[:6, :] = 0.0; l.weight[:6, :6] = torch.eye(6)
+                l.bias.uniform_(-0.05, 0.05); l.bias[:6] = 0.0
             nef.decoder.lout.weight.mul_(0.05); nef.decoder.lout.weight[0, :6] = 1.0 / np.sqrt(3.0)
             nef.decoder.lout.bias.fill_(-0.25)
         t = object.__new__(st.SDFTrainer)
@@ -106,7 +114,7 @@ def main():
         d[f"{name}_losses"] = np.asarray(losses, np.float64)
         out.update(d)
         print(name, "losses", losses, "params", len(_params(nef)), "grads", len(grads))
-    path = os.path.join(ROOT, "tests", "golden", "sdf_train.npz")
+    path = os.path.join(ROOT, "tests", "golden", "sdf_train_deep.npz" if deep else "sdf_train.npz")
     np.savez_compressed(path, **out)
     print(path)
 
