@@ -226,7 +226,9 @@ int wb_find_depth_bound(const float* query, const int32_t* curr_idxes, const flo
 /* ------------------------------------------------------------------------------------------------
  * NeuralSDF(OctreeGrid) and the sphere tracer of app/nglod (BASELINE config 3)
  *   wb_sdf_eval  replaces NeuralSDF.sdf (wisp/models/nefs/neural_sdf.py:120-155): OctreeGrid.interpolate
- *                (octree_grid.py:130-219) + position embedding + BasicDecoder, one launch, fp32 decoder.
+ *                (octree_grid.py:130-219) or HashGrid.interpolate (hash_grid.py:205-233, wb_sdf_desc.hash) + position
+ *                embedding + BasicDecoder, one launch, fp32 decoder.  Octree 'cat' grids: lod_idx = num_lods-1 only; hash grids:
+ *                any lod_idx.
  *   wb_sdf_trace replaces the whole loop of PackedSDFTracer.trace (wisp/tracers/packed_sdf_tracer.py:78-174) including
  *                wisp._C.render.find_depth_bound_cuda (find_depth_bound_cuda.cu:16-45) and finitediff_gradient
  *                (wisp/ops/differential/gradients.py:29-45): ONE persistent cooperative kernel.  Input: the nuggets of
@@ -247,7 +249,13 @@ typedef struct wb_sdf_desc {
     int32_t pos_mode, pos_freq;             /* 0 none, 1 identity, 2 positional, 3 positional+input  */
     int32_t num_layers, hidden_dim;         /* BasicDecoder(bias=True): num_layers hidden layers, relu, 1 output */
     const float* params;                    /* packed [W0, b0, ..., Wout, bout], nn.Linear layout      */
+    const wb_nef_desc* hash;  /* non-null: NeuralSDF(HashGrid); only the hash-grid fields are read; points/trinkets/feats/half_round unused */
 } wb_sdf_desc;
+/* A hash field (hash != NULL, HashGrid.interpolate, hash_grid.py:205-233): hash->feature_dim 4 or 8, 'cat' or 'sum', 3D; the
+ * table is codebook.feats [rows, F] fp32 (16-byte aligned), LOD l at rows begin_idxes[l] ..; feature_dim, num_lods and multiscale
+ * must equal the hash description's, base_lod is 0, and oct may be NULL.  'cat' features are L*F wide whatever lod_idx: the LODs
+ * >= lod_idx are zero (the reference's in-place write); 'sum' adds all L LODs whatever lod_idx.  No occupancy test: coordinates
+ * are clamped into each level's cells.  The table is read in fp32 (the reference's enable_amp fp16 table is not reproduced). */
 int wb_sdf_eval(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, const float* coords, int64_t N, float* sdf, wb_stream s);
 /* wb_sdf_train: one training launch of SDFTrainer.step (wisp/trainers/sdf_trainer.py:65-124) for the loss LOD lod_idx, over
  * NeuralSDF.sdf (wisp/models/nefs/neural_sdf.py:120-155): forward as wb_sdf_eval, loss and backward in the same kernel.
@@ -257,6 +265,8 @@ int wb_sdf_eval(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, c
  *   grad_params   += dL/d params, packed like nef->params [W0, b0, W1, b1, ..., Wout, bout] (nn.Linear layout: W_k [H, in])
  *   grad_feats[k] += dL/d feats[k] for k = 0 .. lod_idx (HOST array of device pointers, shapes of nef->feats), fp32, as
  *                    wb_octree_interp_bwd: no gradient to the coordinates, the fp16 rounding of the forward passed straight through.
+ *   hash field:   grad_feats[0] += dL/d codebook.feats [rows, F] (16-byte aligned), fp32, as wb_hashgrid_bwd; the zeroed 'cat'
+ *                    LODs receive nothing.
  * Everything accumulates: the caller zeroes loss_out and the gradients; a loss over several LODs is one call per LOD. */
 int wb_sdf_train(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, const float* coords, const float* sdf_gt, int64_t N,
                  float inv_count, float* const* grad_feats, float* grad_params, float* loss_out, wb_stream s);
@@ -281,9 +291,10 @@ int wb_sdf_trace(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, 
                  const float* nug_depth, int64_t Ng, const int64_t* ray_offsets,
                  int32_t num_steps, float step_size, float min_dis, int32_t want_normals, const wb_sdf_state* state,
                  float* xyz, float* depth, uint8_t* hit, float* normal, float* rgb, float* alpha, wb_stream s);
-/* The same state machine one phase per launch, for fields this library cannot evaluate itself (NeuralSDF over a hash or
- * triplanar grid, app/nglod/configs/nglod_hash.yaml): the caller evaluates its field at state->x of the alive packs and writes
- * state->dist between the phases.  phase 0: pack list (then read pack_off[R])  1: initial t, x, cursor, alive   2: step 1 of
+/* wb_sdf_trace takes octree fields only: a hash description returns WB_ERR_INVALID before anything is launched.
+ * The same state machine one phase per launch, for fields wb_sdf_trace does not trace (NeuralSDF over a hash grid,
+ * app/nglod/configs/nglod_hash.yaml, whose field the caller evaluates with wb_sdf_eval; or over a triplanar grid, evaluated outside
+ * this library): the caller evaluates its field at state->x of the alive packs and writes state->dist between the phases.  phase 0: pack list (then read pack_off[R])  1: initial t, x, cursor, alive   2: step 1 of
  * iteration `iteration` (packed_sdf_tracer.py:120-131)   3: step 2 (:133-141)   4: outputs of the packs that hit.
  * iterflags[2*iteration + (phase == 3)] != 0 afterwards iff a pack is still alive (the loop's `break` tests). */
 int wb_sdf_phase(int32_t phase, const wb_rays* rays, const float* nug_depth, int64_t Ng, const int64_t* ray_offsets,

@@ -57,7 +57,8 @@ class SdfDesc(C.Structure):
     """struct wb_sdf_desc."""
     _fields_ = [("points", C.c_void_p), ("trinkets", C.c_void_p), ("feats", C.POINTER(C.c_void_p)),
                 ("feature_dim", C.c_int32), ("base_lod", C.c_int32), ("num_lods", C.c_int32), ("multiscale", C.c_int32), ("half_round", C.c_int32),
-                ("pos_mode", C.c_int32), ("pos_freq", C.c_int32), ("num_layers", C.c_int32), ("hidden_dim", C.c_int32), ("params", C.c_void_p)]
+                ("pos_mode", C.c_int32), ("pos_freq", C.c_int32), ("num_layers", C.c_int32), ("hidden_dim", C.c_int32), ("params", C.c_void_p),
+                ("hash", C.POINTER(NefDesc))]
 
 
 class SdfState(C.Structure):

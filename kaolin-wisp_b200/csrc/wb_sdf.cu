@@ -1,8 +1,8 @@
 // wb_sdf.cu -- NeuralSDF(OctreeGrid) evaluation and the sphere tracer of app/nglod as ONE persistent kernel.
 //
-//   wb_sdf_eval   NeuralSDF.sdf (wisp/models/nefs/neural_sdf.py:120-155) = OctreeGrid.interpolate (octree_grid.py:130-219)
-//                 + [position embedding first, features second] + BasicDecoder (basic_decoders.py:73-101), one thread per
-//                 point, the decoder's weights staged in shared memory.  The reference runs a query, one Kaolin launch per
+//   wb_sdf_eval   NeuralSDF.sdf (wisp/models/nefs/neural_sdf.py:120-155) = OctreeGrid.interpolate (octree_grid.py:130-219) or
+//                 HashGrid.interpolate (hash_grid.py:205-233) + [position embedding first, features second] + BasicDecoder
+//                 (basic_decoders.py:73-101), one thread per point, the decoder's weights staged in shared memory.  The reference runs a query, one Kaolin launch per
 //                 LOD, a cat and two cuBLAS GEMMs per call.
 //   wb_sdf_trace  PackedSDFTracer.trace (wisp/tracers/packed_sdf_tracer.py:78-174) + find_depth_bound
 //                 (wisp/csrc/render/find_depth_bound_cuda.cu:16-45) + finitediff_gradient (wisp/ops/differential/gradients.py:29-45).
@@ -101,6 +101,46 @@ __device__ __forceinline__ float sdf_eval(const WbOct& oc, const WbSdf& m, const
     }
 }
 
+// BasicDecoder over the input vector in[0 .. in_dim) for the hash path: sdf_eval's generic chains restated (every unit seeded with
+// its bias, over its inputs in order; the output over the units in order), so eval and training give the same y.  sdf_eval keeps its
+// own copy: calling this from it moves the instruction schedule of the validated octree instances.
+__device__ __forceinline__ float sdf_decode(const WbSdf& m, const float* __restrict__ sw, const float* in)
+{
+    const int H = m.H;
+    float ha[WB_SDF_MAX_H], hb[WB_SDF_MAX_H];
+    const float* w = sw; const float* b = sw + H * m.in_pad;
+    for (int j = 0; j < H; ++j) {
+        float a = b[j];
+        for (int k = 0; k < m.in_dim; ++k) a = fmaf(w[j * m.in_pad + k], in[k], a);
+        ha[j] = fmaxf(a, 0.0f);
+    }
+    const float* p = b + H;
+    float* cur = ha; float* nxt = hb;
+    for (int l = 1; l < m.nh; ++l) {
+        const float* wl = p; const float* bl = p + H * H;
+        for (int j = 0; j < H; ++j) {
+            float a = bl[j];
+            for (int k = 0; k < H; ++k) a = fmaf(wl[j * H + k], cur[k], a);
+            nxt[j] = fmaxf(a, 0.0f);
+        }
+        p += H * H + H;
+        float* t = cur; cur = nxt; nxt = t;
+    }
+    float out = p[H];
+    for (int j = 0; j < H; ++j) out = fmaf(p[j], cur[j], out);
+    return out;
+}
+
+
+// NeuralSDF(HashGrid).sdf at one point: the generic path with the hash-grid gather
+__device__ __forceinline__ float sdf_eval_hash(const WbGrid& hg, const WbSdf& m, const float* __restrict__ sw, int nl, float x, float y, float z)
+{
+    float in[WB_SDF_MAX_IN];
+    const int pd = sdf_embed(m.pos_mode, m.pos_freq, x, y, z, in);
+    sdf_hash_features(hg, nl, x, y, z, in + pd);
+    return sdf_decode(m, sw, in);
+}
+
 template <int FT, int PT>
 __global__ void __launch_bounds__(WB_SDF_THREADS)
 wb_sdf_eval_kernel(WbOct oc, WbSdf m, int nl, const float* __restrict__ coords, int64_t N, float* __restrict__ out)
@@ -109,6 +149,17 @@ wb_sdf_eval_kernel(WbOct oc, WbSdf m, int nl, const float* __restrict__ coords, 
     sdf_stage(m, sw);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += (int64_t)gridDim.x * blockDim.x)
         out[i] = sdf_eval<FT, PT>(oc, m, sw, nl, __ldg(coords + 3 * i), __ldg(coords + 3 * i + 1), __ldg(coords + 3 * i + 2));
+}
+
+// the same loop for a hash field.  A kernel of its own: appending a WbGrid parameter to wb_sdf_eval_kernel moves the instruction
+// schedule of its <16,1> instance.
+__global__ void __launch_bounds__(WB_SDF_THREADS)
+wb_sdf_eval_hash_kernel(WbGrid hg, WbSdf m, int nl, const float* __restrict__ coords, int64_t N, float* __restrict__ out)
+{
+    extern __shared__ __align__(16) float sw[];
+    sdf_stage(m, sw);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += (int64_t)gridDim.x * blockDim.x)
+        out[i] = sdf_eval_hash(hg, m, sw, nl, __ldg(coords + 3 * i), __ldg(coords + 3 * i + 1), __ldg(coords + 3 * i + 2));
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -283,8 +334,8 @@ wb_sdf_trace_kernel(WbOct oc, WbSdf m, WbSdfTrace T)
     if ((threadIdx.x & 31) == 0 && evals) atomicAdd(T.S.iterflags + 2 * T.num_steps + 2, evals);
 }
 
-// The same state machine one phase per launch, for neural fields whose SDF is evaluated outside this library (NeuralSDF over a
-// hash or triplanar grid): the caller evaluates the field at S.x of the alive packs between the phases.
+// The same state machine one phase per launch, for neural fields this persistent kernel does not trace (NeuralSDF over a hash grid,
+// evaluated by wb_sdf_eval, or over a triplanar grid): the caller evaluates the field at S.x of the alive packs between the phases.
 //   phase 0: pack list   1: initial state   2: step 1 (march)   3: step 2 (jump)   4: outputs of the packs that hit
 __global__ void __launch_bounds__(WB_SDF_THREADS)
 wb_sdf_phase_kernel(WbSdfTrace T, int phase, int it, int cb)
@@ -311,13 +362,21 @@ wb_sdf_phase_kernel(WbSdfTrace T, int phase, int it, int cb)
 extern "C" int wb_sdf_eval(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, const float* coords, int64_t N, float* out, wb_stream s)
 {
     if (N == 0) return WB_OK;
-    WbSdf m; int rc = wb_make_sdf(nef, &m); if (rc) return rc;
+    WbSdf m; WbGrid hg; int rc = wb_make_sdf(nef, &m, &hg); if (rc) return rc;
+    const bool hash = hg.table != nullptr;
     WB_CHECK_ARG(lod_idx >= 0 && lod_idx < m.num_lods, "lod_idx out of range");
-    WB_CHECK_ARG(m.multiscale == 1 || lod_idx == m.num_lods - 1, "'cat' grids feed the decoder all LODs: lod_idx must be num_lods-1");
-    WbOct oc; rc = wb_make_oct(oct, m.base_lod + lod_idx, &oc); if (rc) return rc;
+    WB_CHECK_ARG(hash || m.multiscale == 1 || lod_idx == m.num_lods - 1, "'cat' octree grids feed the decoder all LODs: lod_idx must be num_lods-1");
+    WbOct oc; memset(&oc, 0, sizeof(oc));
+    if (!hash) { rc = wb_make_oct(oct, m.base_lod + lod_idx, &oc); if (rc) return rc; }
     WB_CHECK_ARG(coords && out, "null pointer");
     const int smem = m.smem_floats * 4;
     int64_t ctas = (N + WB_SDF_THREADS - 1) / WB_SDF_THREADS; const int64_t cap = (int64_t)wb_num_sms() * 8; if (ctas > cap) ctas = cap;
+    if (hash) {
+        if (smem > 48 * 1024) WB_CUDA(cudaFuncSetAttribute(wb_sdf_eval_hash_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        wb_sdf_eval_hash_kernel<<<(unsigned)ctas, WB_SDF_THREADS, smem, (cudaStream_t)s>>>(hg, m, lod_idx + 1, coords, N, out);
+        WB_LAUNCH_CHECK();
+        return WB_OK;
+    }
     auto kern = sdf_fast_shape(m) ? wb_sdf_eval_kernel<16, 1> : wb_sdf_eval_kernel<0, 0>;
     if (smem > 48 * 1024) WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     kern<<<(unsigned)ctas, WB_SDF_THREADS, smem, (cudaStream_t)s>>>(oc, m, lod_idx + 1, coords, N, out);
@@ -357,7 +416,8 @@ extern "C" int wb_sdf_trace(const wb_octree* oct, const wb_sdf_desc* nef, int32_
 {
     WB_CHECK_ARG(rays != nullptr, "null rays");
     if (rays->num_rays == 0 || Ng == 0) return WB_OK;
-    WbSdf m; int rc = wb_make_sdf(nef, &m); if (rc) return rc;
+    WbSdf m; WbGrid hg; int rc = wb_make_sdf(nef, &m, &hg); if (rc) return rc;
+    WB_CHECK_ARG(hg.table == nullptr, "hash fields are traced phase by phase (wb_sdf_phase + wb_sdf_eval)");
     WB_CHECK_ARG(lod_idx >= 0 && lod_idx < m.num_lods, "lod_idx out of range");
     WB_CHECK_ARG(m.multiscale == 1 || lod_idx == m.num_lods - 1, "'cat' grids feed the decoder all LODs: lod_idx must be num_lods-1");
     WbOct oc; rc = wb_make_oct(oct, m.base_lod + m.num_lods - 1, &oc); if (rc) return rc;

@@ -1,5 +1,6 @@
-// wb_sdf.cuh -- the NeuralSDF(OctreeGrid) field shared by wb_sdf.cu (evaluation, sphere tracing) and wb_sdf_train.cu (training
-// step): host-side description, the decoder's shared-memory image, the position embedding and the octree feature gather.
+// wb_sdf.cuh -- the NeuralSDF(OctreeGrid | HashGrid) field shared by wb_sdf.cu (evaluation, sphere tracing) and wb_sdf_train.cu
+// (training step): host-side description, the decoder's shared-memory image, the position embedding and the octree and hash-grid
+// feature gathers.
 #pragma once
 #include "wb_common.cuh"
 
@@ -20,17 +21,30 @@ struct WbSdf {
 
 static inline int sdf_embed_dim(int mode, int freq) { return mode == 0 ? 0 : mode == 1 ? 3 : mode == 2 ? 6 * freq : 3 + 6 * freq; }
 
-static inline int wb_make_sdf(const wb_sdf_desc* d, WbSdf* m)
+// hg: the hash grid of a hash field (d->hash != NULL), validated by wb_make_grid; hg->table == nullptr for an octree field
+static inline int wb_make_sdf(const wb_sdf_desc* d, WbSdf* m, WbGrid* hg)
 {
-    WB_CHECK_ARG(d != nullptr && d->points && d->trinkets && d->feats && d->params, "null pointer in wb_sdf_desc");
+    memset(hg, 0, sizeof(*hg));
+    WB_CHECK_ARG(d != nullptr && d->params && (d->hash || (d->points && d->trinkets && d->feats)), "null pointer in wb_sdf_desc");
+    if (d->hash) {
+        const int rc = wb_make_grid(d->hash, hg); if (rc) return rc;
+        WB_CHECK_ARG(d->hash->grid_kind == 0 && (hg->F == 4 || hg->F == 8), "hash field: a hash grid of 4 or 8 features per LOD");
+        WB_CHECK_ARG((reinterpret_cast<uintptr_t>(hg->table) & 15u) == 0, "hash field: the table must be 16-byte aligned");
+        WB_CHECK_ARG(d->feature_dim == hg->F && d->num_lods == hg->L && d->multiscale == hg->multiscale && d->base_lod == 0,
+                     "hash field: feature_dim / num_lods / multiscale differ from the hash description");
+    }
     WB_CHECK_ARG(d->num_lods >= 1 && d->num_lods <= WB_MAX_LODS && d->base_lod >= 0, "bad LOD range");
     WB_CHECK_ARG(d->feature_dim >= 1 && d->feature_dim <= 64, "feature_dim must be in [1,64]");
     WB_CHECK_ARG(d->multiscale == 0 || d->multiscale == 1, "multiscale must be 0 ('cat') or 1 ('sum')");
     WB_CHECK_ARG(d->num_layers >= 1 && d->num_layers <= 4 && d->hidden_dim >= 1 && d->hidden_dim <= WB_SDF_MAX_H, "decoder: 1..4 hidden layers, <= 128 wide");
     WB_CHECK_ARG(d->pos_mode >= 0 && d->pos_mode <= 3 && d->pos_freq >= 0 && d->pos_freq <= 10, "bad position embedding");
-    m->points = d->points; m->trinkets = d->trinkets;
-    for (int k = 0; k < d->num_lods; ++k) { WB_CHECK_ARG(d->feats[k] != nullptr, "null feature level"); m->feats[k] = d->feats[k]; }
-    m->F = d->feature_dim; m->base_lod = d->base_lod; m->num_lods = d->num_lods; m->multiscale = d->multiscale; m->half_round = d->half_round;
+    memset(m, 0, sizeof(*m));
+    if (!d->hash) {
+        m->points = d->points; m->trinkets = d->trinkets;
+        for (int k = 0; k < d->num_lods; ++k) { WB_CHECK_ARG(d->feats[k] != nullptr, "null feature level"); m->feats[k] = d->feats[k]; }
+        m->half_round = d->half_round;
+    }
+    m->F = d->feature_dim; m->base_lod = d->base_lod; m->num_lods = d->num_lods; m->multiscale = d->multiscale;
     m->pos_mode = d->pos_mode; m->pos_freq = d->pos_freq; m->pos_dim = sdf_embed_dim(d->pos_mode, d->pos_freq);
     m->feat_dim = d->multiscale ? d->feature_dim : d->feature_dim * d->num_lods;
     m->in_dim = m->pos_dim + m->feat_dim; m->in_pad = (m->in_dim + 3) & ~3;
@@ -149,6 +163,38 @@ __device__ __forceinline__ void sdf_features(const WbOct& oc, const WbSdf& m, in
             }
         }
         if (k == nl - 1) return;
+    }
+}
+
+// HashGrid.interpolate (hash_grid.py:205-233) for one point -> feat[0 .. F) ('sum') or feat[0 .. L*F) ('cat').  Per LOD the corners
+// of wb_corner_setup and wb_hashgrid_fwd's blend (v0 c0, then an fma over corners 1..7), so each LOD's features are bit-identical to
+// wb_hashgrid_fwd's; 'sum' adds all L LODs in LOD order whatever lod_idx, 'cat' writes zeros for the LODs >= lod_idx = nl - 1 (the
+// reference's in-place feats[..., lod_idx*F:] = 0).  F = 4 or 8: a row is one or two float4.
+__device__ __forceinline__ void sdf_hash_features(const WbGrid& g, int nl, float cx, float cy, float cz, float* feat)
+{
+    const int F = g.F, nq = F / 4;
+    const bool sum = g.multiscale != 0;
+    const int act = sum ? g.L : nl - 1;                 // LODs evaluated
+    for (int f = sum ? 0 : act * F; f < (sum ? F : g.L * F); ++f) feat[f] = 0.0f;
+    for (int l = 0; l < act; ++l) {
+        uint32_t idx[8]; float cf[8];
+        wb_corner_setup(g, l, cx, cy, cz, idx, cf);
+        const float4* tb = reinterpret_cast<const float4*>(g.table + g.begin[l] * F);
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+            if (q >= nq) break;
+            float4 v[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) v[j] = __ldg(tb + (int64_t)idx[j] * nq + q);
+            float a0 = v[0].x * cf[0], a1 = v[0].y * cf[0], a2 = v[0].z * cf[0], a3 = v[0].w * cf[0];
+#pragma unroll
+            for (int j = 1; j < 8; ++j) {
+                a0 = fmaf(v[j].x, cf[j], a0); a1 = fmaf(v[j].y, cf[j], a1); a2 = fmaf(v[j].z, cf[j], a2); a3 = fmaf(v[j].w, cf[j], a3);
+            }
+            float* o = feat + (sum ? 0 : l * F) + 4 * q;
+            if (sum) { o[0] += a0; o[1] += a1; o[2] += a2; o[3] += a3; }
+            else { o[0] = a0; o[1] = a1; o[2] = a2; o[3] = a3; }
+        }
     }
 }
 

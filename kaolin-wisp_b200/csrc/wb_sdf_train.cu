@@ -13,6 +13,8 @@
 //     dL/dW0[j,:] += da x, dL/db0[j] += da, dL/dwout[j] += dy relu(a), accumulated over all tiles of the CTA and added to
 //     grad_params once at the end (per-sample atomics into the decoder would serialise on a few thousand addresses).
 // fp32 SIMT throughout: ~15 kFLOP per sample against ~3 KB of feature gather and ~6 KB of scatter read-modify-write.
+// A hash field (NeuralSDF(HashGrid), the HASH instances) runs the same kernels with the hash-grid gather of wb_sdf.cuh and the
+// scatter below in place of the octree's; everything else (tiles, summation orders, footprint) is unchanged.
 #include "wb_sdf.cuh"
 #include "wb_featx.cuh"
 
@@ -42,9 +44,39 @@ __device__ __forceinline__ void sdf_scatter_sum(const WbGridX& x, float cx, floa
     });
 }
 
-template <int FT, int PT>
+// The scatter of a hash field (HashGrid.interpolate's backward, wb_hashgrid_bwd's products): per LOD and corner fl(g * c_j) added to
+// the table gradient gt [rows, F] with one float4 reduction per corner and quad of features; quads of zero gradients are skipped, and
+// the 'cat' LODs >= lod_idx = nl - 1, whose features the forward zeroed, get nothing.  grad(f): dL/dfeat of decoder-input feature f.
+template <class Grad>
+__device__ __forceinline__ void sdf_hash_scatter(const WbGrid& g, float* gt, int nl, float cx, float cy, float cz, Grad grad)
+{
+    const int F = g.F, nq = F / 4;
+    const bool sum = g.multiscale != 0;
+    const int act = sum ? g.L : nl - 1;
+    for (int l = 0; l < act; ++l) {
+        float gv[8];
+        bool any = false;
+#pragma unroll
+        for (int f = 0; f < 8; ++f) { gv[f] = f < F ? grad(sum ? f : l * F + f) : 0.0f; any |= gv[f] != 0.0f; }
+        if (!any) continue;
+        uint32_t idx[8]; float cf[8];
+        wb_corner_setup(g, l, cx, cy, cz, idx, cf);
+        float4* tb = reinterpret_cast<float4*>(gt + g.begin[l] * F);
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+            if (q >= nq) break;
+            const float g0 = gv[4 * q], g1 = gv[4 * q + 1], g2 = gv[4 * q + 2], g3 = gv[4 * q + 3];
+            if (g0 == 0.0f && g1 == 0.0f && g2 == 0.0f && g3 == 0.0f) continue;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) atomicAdd(tb + (int64_t)idx[j] * nq + q, make_float4(g0 * cf[j], g1 * cf[j], g2 * cf[j], g3 * cf[j]));
+        }
+    }
+}
+
+// HASH: a hash field, gathered from hg and scattered into gx.gptr[0] (the codebook gradient); gx's octree part is unused
+template <int FT, int PT, bool HASH = false>
 __global__ void __launch_bounds__(WB_SDF_TRAIN_TILE)
-wb_sdf_train_kernel(WbOct oc, WbSdf m, WbGridX gx, int nl, WbSdfTrain T)
+wb_sdf_train_kernel(WbOct oc, WbSdf m, WbGridX gx, int nl, WbSdfTrain T, WbGrid hg)
 {
     constexpr bool FAST = FT > 0 && PT == 1;             // dispatch guarantees nh == 1, 'sum', identity position input
     constexpr int INF = FAST ? ((3 + FT + 3) & ~3) : 1;  // compile-time in_pad of the fast shape
@@ -134,7 +166,8 @@ wb_sdf_train_kernel(WbOct oc, WbSdf m, WbGridX gx, int nl, WbSdfTrain T)
             } else {
                 float g[WB_SDF_MAX_IN];
                 const int pd = sdf_embed(m.pos_mode, m.pos_freq, x, y, z, xr);
-                sdf_features<0>(oc, m, nl, x, y, z, xr + pd);
+                if constexpr (HASH) sdf_hash_features(hg, nl, x, y, z, xr + pd);
+                else sdf_features<0>(oc, m, nl, x, y, z, xr + pd);
                 for (int k = IN; k < INP; ++k) xr[k] = 0.0f;
                 for (int k = pd; k < IN; ++k) g[k] = 0.0f;
                 float out = wo[H];
@@ -148,7 +181,8 @@ wb_sdf_train_kernel(WbOct oc, WbSdf m, WbGridX gx, int nl, WbSdfTrain T)
                 const float d = out - __ldg(T.gt + i);
                 lsum = fmaf(d, d, lsum);
                 dy = T.inv_count * (2.0f * d);
-                wb_featx_scatter(gx, x, y, z, [&](int f) { return dy * g[pd + f]; });
+                if constexpr (HASH) sdf_hash_scatter(hg, gx.gptr[0], nl, x, y, z, [&](int f) { return dy * g[pd + f]; });
+                else wb_featx_scatter(gx, x, y, z, [&](int f) { return dy * g[pd + f]; });
             }
         }
         dys[tid] = dy; dsum += dy;
@@ -333,8 +367,9 @@ __device__ __forceinline__ void sdf_deep_grad(float* G, int ldg, float* gb, int 
     }
 }
 
+template <bool HASH = false>      // as wb_sdf_train_kernel
 __global__ void __launch_bounds__(WB_SDF_DEEP_THREADS)
-wb_sdf_train_deep_kernel(WbOct oc, WbSdf m, WbGridX gx, int nl, WbSdfTrainDeep T)
+wb_sdf_train_deep_kernel(WbOct oc, WbSdf m, WbGridX gx, int nl, WbSdfTrainDeep T, WbGrid hg)
 {
     extern __shared__ __align__(16) float sw[];
     const int H = m.H, INP = m.in_pad, IN = m.in_dim, nh = m.nh, tid = threadIdx.x;
@@ -355,7 +390,8 @@ wb_sdf_train_deep_kernel(WbOct oc, WbSdf m, WbGridX gx, int nl, WbSdfTrainDeep T
             float* xr = xs + tid * SX;
             const float x = __ldg(T.coords + 3 * i), y = __ldg(T.coords + 3 * i + 1), z = __ldg(T.coords + 3 * i + 2);
             const int pd = sdf_embed(m.pos_mode, m.pos_freq, x, y, z, xr);
-            sdf_features<0>(oc, m, nl, x, y, z, xr + pd);
+            if constexpr (HASH) sdf_hash_features(hg, nl, x, y, z, xr + pd);
+            else sdf_features<0>(oc, m, nl, x, y, z, xr + pd);
             for (int k = IN; k < INP; ++k) xr[k] = 0.0f;
         }
         __syncthreads();
@@ -406,7 +442,9 @@ wb_sdf_train_deep_kernel(WbOct oc, WbSdf m, WbGridX gx, int nl, WbSdfTrainDeep T
         if (tid < cnt) {
             const int64_t i = base + tid;
             const float* gr = xs + tid * SX + m.pos_dim;
-            wb_featx_scatter(gx, __ldg(T.coords + 3 * i), __ldg(T.coords + 3 * i + 1), __ldg(T.coords + 3 * i + 2), [&](int f) { return gr[f]; });
+            const float x = __ldg(T.coords + 3 * i), y = __ldg(T.coords + 3 * i + 1), z = __ldg(T.coords + 3 * i + 2);
+            if constexpr (HASH) sdf_hash_scatter(hg, gx.gptr[0], nl, x, y, z, [&](int f) { return gr[f]; });
+            else wb_featx_scatter(gx, x, y, z, [&](int f) { return gr[f]; });
         }
         __syncthreads();
     }
@@ -452,7 +490,7 @@ static int sdf_train_plan(const WbSdf& m, int* tile)
 
 extern "C" int64_t wb_sdf_train_smem_bytes(const wb_sdf_desc* nef)
 {
-    WbSdf m; if (wb_make_sdf(nef, &m)) return -1;
+    WbSdf m; WbGrid hg; if (wb_make_sdf(nef, &m, &hg)) return -1;
     int tile = 0;
     return sdf_train_plan(m, &tile);
 }
@@ -460,23 +498,30 @@ extern "C" int64_t wb_sdf_train_smem_bytes(const wb_sdf_desc* nef)
 extern "C" int wb_sdf_train(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, const float* coords, const float* sdf_gt, int64_t N,
                             float inv_count, float* const* grad_feats, float* grad_params, float* loss_out, wb_stream s)
 {
-    WbSdf m; int rc = wb_make_sdf(nef, &m); if (rc) return rc;
+    WbSdf m; WbGrid hg; int rc = wb_make_sdf(nef, &m, &hg); if (rc) return rc;
+    const bool hash = hg.table != nullptr;
     int tile = 0; const int smem = sdf_train_plan(m, &tile);
     WB_CHECK_ARG(smem > 0, "decoder weights, their gradient accumulators and a 32-sample tile exceed shared memory (wb_sdf_train_smem_bytes < 0)");
     WB_CHECK_ARG(lod_idx >= 0 && lod_idx < m.num_lods, "lod_idx out of range");
-    WB_CHECK_ARG(m.multiscale == 1 || lod_idx == m.num_lods - 1, "'cat' grids feed the decoder all LODs: lod_idx must be num_lods-1");
+    WB_CHECK_ARG(hash || m.multiscale == 1 || lod_idx == m.num_lods - 1, "'cat' octree grids feed the decoder all LODs: lod_idx must be num_lods-1");
     WB_CHECK_ARG(coords && sdf_gt && grad_feats && grad_params && loss_out && N >= 0, "null pointer");
     if (N == 0) return WB_OK;
-    WbOct oc; rc = wb_make_oct(oct, m.base_lod + lod_idx, &oc); if (rc) return rc;
-    const bool fast = sdf_fast_shape(m);
+    WbOct oc; memset(&oc, 0, sizeof(oc));
+    const bool fast = !hash && sdf_fast_shape(m);
     WbGridX gx; memset(&gx, 0, sizeof(gx));
-    gx.kind = 2; gx.nl = lod_idx + 1; gx.sum = m.multiscale; gx.C = m.F;
-    gx.octree = oc.octree; gx.prefix = oc.prefix; gx.points = m.points; gx.trinkets = m.trinkets;
-    gx.base_lod = m.base_lod; gx.half_round = m.half_round;
-    for (int k = 0; k <= lod_idx; ++k) {
-        WB_CHECK_ARG(grad_feats[k] != nullptr, "null gradient level");
-        WB_CHECK_ARG(!fast || (reinterpret_cast<uintptr_t>(grad_feats[k]) & 15u) == 0, "gradient levels must be 16-byte aligned");
-        gx.ptr[k] = m.feats[k]; gx.gptr[k] = grad_feats[k];
+    if (hash) {                                            // kind 0: the hash grid of hg; its gradient is the one codebook table
+        WB_CHECK_ARG(grad_feats[0] != nullptr && (reinterpret_cast<uintptr_t>(grad_feats[0]) & 15u) == 0, "hash field: null or unaligned table gradient");
+        gx.gptr[0] = grad_feats[0];
+    } else {
+        rc = wb_make_oct(oct, m.base_lod + lod_idx, &oc); if (rc) return rc;
+        gx.kind = 2; gx.nl = lod_idx + 1; gx.sum = m.multiscale; gx.C = m.F;
+        gx.octree = oc.octree; gx.prefix = oc.prefix; gx.points = m.points; gx.trinkets = m.trinkets;
+        gx.base_lod = m.base_lod; gx.half_round = m.half_round;
+        for (int k = 0; k <= lod_idx; ++k) {
+            WB_CHECK_ARG(grad_feats[k] != nullptr, "null gradient level");
+            WB_CHECK_ARG(!fast || (reinterpret_cast<uintptr_t>(grad_feats[k]) & 15u) == 0, "gradient levels must be 16-byte aligned");
+            gx.ptr[k] = m.feats[k]; gx.gptr[k] = grad_feats[k];
+        }
     }
     int nl = lod_idx + 1;
     if (m.nh > 1) {
@@ -484,13 +529,13 @@ extern "C" int wb_sdf_train(const wb_octree* oct, const wb_sdf_desc* nef, int32_
         D.coords = coords; D.gt = sdf_gt; D.N = N; D.inv_count = inv_count; D.gparams = grad_params; D.loss = loss_out;
         D.T = tile; D.SX = sdf_deep_stride(m.in_pad); D.SH = sdf_deep_stride(m.H);
         D.acc_off = (m.smem_floats + 3) & ~3; D.tile_off = 2 * D.acc_off; D.red_off = D.tile_off + tile * (D.SX + m.nh * D.SH + 1);
-        const void* kern = (const void*)wb_sdf_train_deep_kernel;
+        const void* kern = hash ? (const void*)wb_sdf_train_deep_kernel<true> : (const void*)wb_sdf_train_deep_kernel<false>;
         WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         int per_sm = 0;
         WB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, WB_SDF_DEEP_THREADS, smem));
         WB_CHECK_ARG(per_sm >= 1, "training kernel does not fit on an SM");
         int64_t ctas = (N + tile - 1) / tile; const int64_t cap = (int64_t)wb_num_sms() * per_sm; if (ctas > cap) ctas = cap;
-        void* args[] = { &oc, &m, &gx, &nl, &D };
+        void* args[] = { &oc, &m, &gx, &nl, &D, &hg };
         WB_CUDA(cudaLaunchKernel(kern, dim3((unsigned)ctas), dim3(WB_SDF_DEEP_THREADS), args, (size_t)smem, (cudaStream_t)s));
         wb_count_launch();
         return WB_OK;
@@ -500,13 +545,13 @@ extern "C" int wb_sdf_train(const wb_octree* oct, const wb_sdf_desc* nef, int32_
     T.xs_off = (m.smem_floats + 3) & ~3;
     T.gw_off = T.xs_off + WB_SDF_TRAIN_TILE * m.in_pad + WB_SDF_TRAIN_TILE;
     T.red_off = T.gw_off + (fast ? 0 : m.H * (m.in_pad + 1));
-    const void* kern = fast ? (const void*)wb_sdf_train_kernel<16, 1> : (const void*)wb_sdf_train_kernel<0, 0>;
+    const void* kern = hash ? (const void*)wb_sdf_train_kernel<0, 0, true> : fast ? (const void*)wb_sdf_train_kernel<16, 1> : (const void*)wb_sdf_train_kernel<0, 0>;
     if (smem > 48 * 1024) WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     int per_sm = 0;
     WB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, WB_SDF_TRAIN_TILE, smem));
     WB_CHECK_ARG(per_sm >= 1, "training kernel does not fit on an SM");
     int64_t ctas = (N + WB_SDF_TRAIN_TILE - 1) / WB_SDF_TRAIN_TILE; const int64_t cap = (int64_t)wb_num_sms() * per_sm; if (ctas > cap) ctas = cap;
-    void* args[] = { &oc, &m, &gx, &nl, &T };
+    void* args[] = { &oc, &m, &gx, &nl, &T, &hg };
     WB_CUDA(cudaLaunchKernel(kern, dim3((unsigned)ctas), dim3(WB_SDF_TRAIN_TILE), args, (size_t)smem, (cudaStream_t)s));
     wb_count_launch();
     return WB_OK;

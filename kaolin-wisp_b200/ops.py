@@ -570,11 +570,19 @@ def _sdf_embed_mode(nef):
 
 
 def sdf_field(nef):
-    """-> (SdfDesc, OctreeTensors, keepalive) for a NeuralSDF over an OctreeGrid ('linear'), or None when the field is outside
-    what wb_sdf_eval / wb_sdf_trace evaluate natively (other grids, activations, skip connections, > 128 wide)."""
+    """-> (SdfDesc, OctreeTensors, keepalive) for a NeuralSDF over an OctreeGrid ('linear'), or (SdfDesc, None, keepalive) for a
+    NeuralSDF over a 3D HashGrid of 4 or 8 features per LOD; None when the field is outside what wb_sdf_eval / wb_sdf_train
+    evaluate natively (other grids, activations, skip connections, > 128 wide).  Only octree fields go to wb_sdf_trace."""
     g, dec = getattr(nef, "grid", None), getattr(nef, "decoder", None)
-    if g is None or dec is None or not all(hasattr(g, a) for a in ("trinkets", "features", "base_lod", "num_lods", "multiscale_type", "blas")):
+    if g is None or dec is None:
         return None
+    octree = all(hasattr(g, a) for a in ("trinkets", "features", "base_lod", "num_lods", "multiscale_type", "blas"))
+    if not octree:
+        # HashGrid (hash_grid.py:27-89): F = 4 or 8 rows are one or two float4; narrower tables (F = 2) keep the autograd route
+        if not all(hasattr(g, a) for a in ("codebook", "codebook_bitwidth", "resolutions", "multiscale_type", "feature_dim")):
+            return None
+        if int(getattr(g, "coord_dim", 3)) != 3 or int(g.feature_dim) not in (4, 8) or g.multiscale_type not in ('cat', 'sum'):
+            return None
     if getattr(g, "interpolation_type", "linear") != "linear" or getattr(dec, "skip", None):
         return None
     if getattr(nef, "activation_type", "relu") != "relu" or getattr(dec, "activation", torch.relu) not in (torch.relu, torch.nn.functional.relu):
@@ -590,6 +598,29 @@ def sdf_field(nef):
     em = _sdf_embed_mode(nef)
     if em is None or em[1] > 10 or g.feature_dim > 64:          # wb_make_sdf: pos_freq <= 10, feature_dim <= 64
         return None
+    num_lods = int(g.num_lods) if octree else len(g.resolutions)
+    pos_dim = 0 if em[0] == 0 else 3 if em[0] == 1 else 6 * em[1] + (3 if em[0] == 3 else 0)
+    in_dim = layers[0].in_features
+    if in_dim != pos_dim + (g.feature_dim if g.multiscale_type == 'sum' else g.feature_dim * num_lods):
+        return None
+    # the decoder input must be at most 132 wide and its shared-memory image must fit in 200 KB: the same limits and formula as
+    # wb_make_sdf (csrc/wb_sdf.cuh)
+    smem_floats = H * ((in_dim + 3) & ~3) + H + (nh - 1) * (H * H + H) + H + 4
+    if in_dim > 132 or smem_floats * 4 > 200 * 1024:
+        return None
+    params = torch.cat([t.detach().reshape(-1).float() for l in layers for t in (l.weight, l.bias)]).contiguous()
+    d = A.SdfDesc()
+    d.feature_dim, d.num_lods = int(g.feature_dim), num_lods
+    d.multiscale = 1 if g.multiscale_type == 'sum' else 0
+    d.pos_mode, d.pos_freq = em
+    d.num_layers, d.hidden_dim, d.params = nh, H, params.data_ptr()
+    if not octree:
+        # the whole codebook.feats [rows, F] as one table; LOD l at rows begin_idxes[l] .. (utils.py:13-71)
+        table = A.f32c(g.codebook.feats.detach())
+        res = [int(r) for r in torch.as_tensor(g.resolutions).reshape(-1).tolist()]
+        hd = A.make_grid_desc(table, res, _hash_begin(g), 2 ** int(g.codebook_bitwidth), g.multiscale_type)
+        d.hash = C.pointer(hd)
+        return d, None, [hd, table, params]
     dev = g.features[0].device
     blas = g.blas
     oct = blas.tensors() if hasattr(blas, "tensors") else None
@@ -599,25 +630,11 @@ def sdf_field(nef):
     if g.trinkets.device != dev:
         g.trinkets = g.trinkets.to(dev)
     feats = [A.f32c(f.detach()) for f in g.features]
-    params = torch.cat([t.detach().reshape(-1).float() for l in layers for t in (l.weight, l.bias)]).contiguous()
     trinkets = g.trinkets.int().contiguous()
-    d = A.SdfDesc()
     ptrs = (C.c_void_p * len(feats))(*[f.data_ptr() for f in feats])
     d.points, d.trinkets, d.feats = oct.points.data_ptr(), trinkets.data_ptr(), ptrs
-    d.feature_dim, d.base_lod, d.num_lods = int(g.feature_dim), int(g.base_lod), int(g.num_lods)
-    d.multiscale = 1 if g.multiscale_type == 'sum' else 0
+    d.base_lod = int(g.base_lod)
     d.half_round = int(getattr(g, "half_features", True))
-    d.pos_mode, d.pos_freq = em
-    d.num_layers, d.hidden_dim, d.params = nh, H, params.data_ptr()
-    pos_dim = 0 if em[0] == 0 else 3 if em[0] == 1 else 6 * em[1] + (3 if em[0] == 3 else 0)
-    in_dim = layers[0].in_features
-    if in_dim != pos_dim + (g.feature_dim if d.multiscale else g.feature_dim * g.num_lods):
-        return None
-    # the decoder input must be at most 132 wide and its shared-memory image must fit in 200 KB: the same limits and formula as
-    # wb_make_sdf (csrc/wb_sdf.cuh)
-    smem_floats = H * ((in_dim + 3) & ~3) + H + (nh - 1) * (H * H + H) + H + 4
-    if in_dim > 132 or smem_floats * 4 > 200 * 1024:
-        return None
     return d, oct, [ptrs, feats, params, trinkets]
 
 
@@ -629,15 +646,20 @@ def sdf_eval(nef, coords: torch.Tensor, lod_idx: Optional[int] = None) -> Option
     d, oct, keep = fd
     if lod_idx is None:
         lod_idx = d.num_lods - 1
-    if d.multiscale == 0 and lod_idx != d.num_lods - 1:
+    if d.multiscale == 0 and lod_idx != d.num_lods - 1 and not d.hash:    # an octree 'cat' grid below its finest LOD: nn.Linear raises
         return None
     A.require_device(coords)
     c = A.f32c(coords).reshape(-1, 3)
     out = torch.empty((c.shape[0], 1), dtype=torch.float32, device=c.device)
-    od = oct.desc()
+    od = _sdf_octree(oct)
     with _stage("sdf_eval"):
-        A.check(A.lib().wb_sdf_eval(C.byref(od), C.byref(d), C.c_int32(lod_idx), A.ptr(c), C.c_int64(c.shape[0]), A.ptr(out), A.stream()))
+        A.check(A.lib().wb_sdf_eval(od, C.byref(d), C.c_int32(lod_idx), A.ptr(c), C.c_int64(c.shape[0]), A.ptr(out), A.stream()))
     return out
+
+
+def _sdf_octree(oct):
+    """The wb_octree argument of wb_sdf_eval / wb_sdf_train: the octree grid's occupancy, NULL for a hash field."""
+    return None if oct is None else C.byref(oct.desc())
 
 
 def sdf_train_smem_bytes(fd) -> int:
@@ -651,7 +673,8 @@ def sdf_train(fd, coords: torch.Tensor, sdf_gt: torch.Tensor, lod_idx: int, inv_
     """Forward, L2 loss and backward of SDFTrainer.step (sdf_trainer.py:65-124) for one loss LOD in one launch (wb_sdf_train), for
     decoders of 1 to 4 hidden layers whose sdf_train_smem_bytes(fd) >= 0.  fd: sdf_field(nef) (its params pointer may be re-aimed
     at a flat decoder buffer); coords f32 [N,3], sdf_gt f32 [N] on the device.  Accumulates: loss_out[0] += sum (y - gt)^2 *
-    inv_count, grad_params (packed like the decoder: [W0, b0, W1, b1, ..., Wout, bout]) and grad_feats[k], k <= lod_idx."""
+    inv_count, grad_params (packed like the decoder: [W0, b0, W1, b1, ..., Wout, bout]) and grad_feats[k], k <= lod_idx (octree
+    grid); for a hash field grad_feats[0] is dL/d codebook.feats [rows, F]."""
     d, oct, _ = fd
     A.require_device(coords)
     if not (coords.dtype == sdf_gt.dtype == grad_params.dtype == loss_out.dtype == torch.float32 and coords.is_contiguous() and sdf_gt.is_contiguous()):
@@ -659,9 +682,9 @@ def sdf_train(fd, coords: torch.Tensor, sdf_gt: torch.Tensor, lod_idx: int, inv_
     if sdf_gt.numel() != coords.shape[0]:
         raise A.WispB200Error(f"sdf_gt has {sdf_gt.numel()} values for {coords.shape[0]} points")
     gptrs = (C.c_void_p * len(grad_feats))(*[g.data_ptr() for g in grad_feats])
-    od = oct.desc()
+    od = _sdf_octree(oct)
     with _stage("sdf_train"):
-        A.check(A.lib().wb_sdf_train(C.byref(od), C.byref(d), C.c_int32(lod_idx), A.ptr(coords), A.ptr(sdf_gt), C.c_int64(coords.shape[0]),
+        A.check(A.lib().wb_sdf_train(od, C.byref(d), C.c_int32(lod_idx), A.ptr(coords), A.ptr(sdf_gt), C.c_int64(coords.shape[0]),
                                      C.c_float(inv_count), gptrs, A.ptr(grad_params), A.ptr(loss_out), A.stream()))
 
 
@@ -697,7 +720,8 @@ def sdf_trace(nef, oct: OctreeTensors, origins, dirs, dist_max, level: int, lod_
               want_normals: bool):
     """PackedSDFTracer.trace (packed_sdf_tracer.py:78-174): raytrace + ONE persistent sphere-tracing kernel (wb_sdf_trace) when the
     field is a NeuralSDF(OctreeGrid); otherwise the same state machine phase by phase (wb_sdf_phase) with the field evaluated through
-    its own forward().  -> dict(xyz, depth, hit, normal, rgb, alpha) per ray."""
+    its own forward() (a NeuralSDF(HashGrid) in sdf_field's range: one wb_sdf_eval per evaluation).  -> dict(xyz, depth, hit,
+    normal, rgb, alpha) per ray."""
     A.require_device(origins)
     R, dev, L = origins.shape[0], origins.device, A.lib()
     _, _, nug_depth, ray_off = raytrace(oct, origins, dirs, level)
@@ -713,7 +737,7 @@ def sdf_trace(nef, oct: OctreeTensors, origins, dirs, dist_max, level: int, lod_
     st = _SdfState(R, num_steps, dev)
     od = oct.desc()
     fd = sdf_field(nef)
-    if fd is not None and not (fd[0].multiscale == 0 and lod_idx != fd[0].num_lods - 1):
+    if fd is not None and not fd[0].hash and not (fd[0].multiscale == 0 and lod_idx != fd[0].num_lods - 1):
         d, _, keep2 = fd
         with _stage("sdf_trace"):
             A.check(L.wb_sdf_trace(C.byref(od), C.byref(d), C.c_int32(lod_idx), C.byref(rays), A.ptr(nug_depth), C.c_int64(Ng), A.ptr(ray_off),
@@ -933,6 +957,18 @@ def raymarch_level(grid, lod_idx: int) -> int:
     return 0
 
 
+def _hash_begin(g) -> List[int]:
+    """MultiTable.begin_idxes of a hash grid as host ints: one device read, cached on the grid (the table layout never changes)."""
+    begin = getattr(g, "_wb_begin", None)
+    if begin is None or len(begin) != len(g.resolutions) + 1:
+        begin = [int(b) for b in g.codebook.begin_idxes.tolist()]
+        try:
+            g._wb_begin = begin
+        except Exception:
+            pass
+    return begin
+
+
 def nef_spec(nef, lod_idx: Optional[int] = None) -> Optional[NefSpec]:
     """Describe a NeuralRadianceField -- this package's mirror or the reference's own class (install()) -- for the fused path, or
     None when something is outside it (embedders other than none/identity/positional, activations other than relu, skip
@@ -958,13 +994,7 @@ def nef_spec(nef, lod_idx: Optional[int] = None) -> Optional[NefSpec]:
     if hasattr(g, "codebook"):                                   # HashGrid
         if g.feature_dim > 8 or getattr(g, "coord_dim", 3) != 3:
             return None
-        begin = getattr(g, "_wb_begin", None)
-        if begin is None or len(begin) != len(g.resolutions) + 1:
-            begin = [int(b) for b in g.codebook.begin_idxes.tolist()]       # one-off device read, cached on the grid
-            try:
-                g._wb_begin = begin
-            except Exception:
-                pass
+        begin = _hash_begin(g)
         return NefSpec(resolutions=[int(r) for r in g.resolutions], begin_idxes=begin, codebook_size=int(g.codebook_size),
                        feature_dim=int(g.feature_dim), lod_idx=lod_idx, kind="hash", num_lods=len(g.resolutions), **common)
     nl = lod_idx + 1

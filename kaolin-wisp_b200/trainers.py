@@ -255,12 +255,14 @@ class SDFStep:
     them), loss = sum over loss_lods of sum((pred - gt)^2), divided by the batch size.  loss_lods is the last LOD when
     `only_last` (nglod_octree.yaml), otherwise every LOD.
 
-    A NeuralSDF over an OctreeGrid with 1 to 4 hidden layers (every app/nglod octree config, with any nef.num_layers up to 4)
-    trains natively: per loss LOD one wb_sdf_train launch (forward, loss and backward, no autograd), then NativeAdam over every
-    parameter in one launch.  The decoder's parameters are flattened in place into one buffer [W0, b0, W1, b1, ..., Wout, bout],
-    which the kernel reads, whose gradient it writes and which is one Adam segment.  The decoder runs in fp32 whatever the
-    autocast state; the reference's enable_amp fp16 nn.Linear is not reproduced.  Every other field (NeuralSDF over a HashGrid
-    or TriplanarGrid, a deeper decoder whose weights, weight-gradient accumulators and smallest sample tile exceed an SM's shared
+    A NeuralSDF with 1 to 4 hidden layers over an OctreeGrid (every app/nglod octree config, with any nef.num_layers up to 4) or
+    over a 3D HashGrid of 4 or 8 features per LOD (nglod_hash.yaml) trains natively: per loss LOD one wb_sdf_train launch
+    (forward, loss and backward, no autograd), then NativeAdam over every parameter in one launch.  The decoder's parameters are
+    flattened in place into one buffer [W0, b0, W1, b1, ..., Wout, bout], which the kernel reads, whose gradient it writes and
+    which is one Adam segment; the grid's tensors (OctreeGrid.features, or the one HashGrid codebook.feats table) are the other
+    segments.  The decoder and the hash table run in fp32 whatever the autocast state; the reference's enable_amp fp16
+    nn.Linear and fp16 table are not reproduced.  Every other field (NeuralSDF over a TriplanarGrid, a hash grid of F = 2 or over
+    8 features, a deeper decoder whose weights, weight-gradient accumulators and smallest sample tile exceed an SM's shared
     memory: wb_sdf_train_smem_bytes < 0) takes autograd plus the same NativeAdam."""
 
     def __init__(self, pipeline, lr: float = 1e-3, eps: float = 1e-15, weight_decay: float = 0.0, grid_lr_weight: float = 1.0,
@@ -277,7 +279,7 @@ class SDFStep:
         self.fd = self._fused_field(nef, [p for _, p in named])
         self.fused = self.fd is not None
         if self.fused:
-            feats = list(nef.grid.features)
+            feats = self._grid_tensors(nef.grid)
             tensors = [(f.data, lr * grid_lr_weight, 0.0) for f in feats] + [(self.dec_flat, lr, weight_decay)]
             self.g_feats = [torch.zeros_like(f.data) for f in feats]
             self.g_dec = torch.zeros_like(self.dec_flat)
@@ -288,14 +290,22 @@ class SDFStep:
         self.opt = NativeAdam(tensors, betas=betas, eps=eps)
         self.loss_buf = torch.zeros(1, dtype=torch.float32, device=self.device)
 
+    @staticmethod
+    def _grid_tensors(grid):
+        """The grid tensors wb_sdf_train writes gradients for: OctreeGrid.features, or HashGrid's one codebook.feats table."""
+        cb = getattr(grid, "codebook", None)
+        if hasattr(cb, "feats") and not hasattr(grid, "features"):
+            return [cb.feats]
+        return list(getattr(grid, "features", []))
+
     def _fused_field(self, nef, params):
         """ops.sdf_field of the field with the decoder flattened in place and the description aimed at that buffer, or None when
-        the field is outside wb_sdf_train (not an OctreeGrid, a decoder whose training footprint exceeds shared memory, or
-        trainable parameters beyond grid and decoder)."""
+        the field is outside wb_sdf_train (neither an OctreeGrid nor a hash grid in ops.sdf_field's range, a decoder whose
+        training footprint exceeds shared memory, or trainable parameters beyond grid and decoder)."""
         grid, dec = getattr(nef, "grid", None), getattr(nef, "decoder", None)
         if grid is None or dec is None or getattr(grid, "dictionary", None) is not None:
             return None
-        feats = list(getattr(grid, "features", []))
+        feats = self._grid_tensors(grid)
         if not feats or any(not isinstance(f, torch.Tensor) or f.dim() != 2 or f.shape[1] != grid.feature_dim or f.dtype != torch.float32 or not f.is_contiguous() for f in feats):
             return None
         dparams = ops.decoder_params(dec)
@@ -307,14 +317,15 @@ class SDFStep:
         self.dec_flat = _flatten_in_place(dparams)
         fd = ops.sdf_field(nef)
         d, oct, keep = fd
-        if any(d.feats[k] != f.data_ptr() for k, f in enumerate(feats)):
+        if (d.hash.contents.table != feats[0].data_ptr()) if d.hash else any(d.feats[k] != f.data_ptr() for k, f in enumerate(feats)):
             return None
         d.params = self.dec_flat.data_ptr()
         return d, oct, keep + [self.dec_flat]
 
     def _lod_check(self, N: int) -> None:
         g = self.nef.grid
-        if self.fused and g.multiscale_type == 'cat' and min(self.loss_lods) < g.num_lods - 1:
+        # an octree 'cat' grid feeds the decoder only LODs 0..lod_idx; a hash 'cat' grid keeps its width and zeroes LODs >= lod_idx
+        if self.fused and not self.fd[0].hash and g.multiscale_type == 'cat' and min(self.loss_lods) < g.num_lods - 1:
             lin = self.nef.decoder.layers[0]
             pd = lin.in_features - g.feature_dim * g.num_lods
             k = min(self.loss_lods)

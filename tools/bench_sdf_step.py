@@ -6,9 +6,13 @@ size, the device name and power limit, and a parity block (SDFStep's gradients a
 parity failure fails the run).
 
     python tools/bench_sdf_step.py [--steps 200] [--warmup 20] [--batches 512,65536,1048576] [--num-layers 1] [--hidden-dim 128]
+                                   [--grid octree|hash]
 
 --num-layers / --hidden-dim replace config 3's decoder (19-128-1) by one with that many hidden layers of that width
 (oracle.sdf_reference.random_decoder, seeded); the grid and the samples stay config 3's.
+--grid hash replaces config 3's OctreeGrid by the nglod_hash.yaml grid (HashGrid.from_geometric: 'cat', F = 8, 4 LODs of 16 .. 2048,
+2^19 rows per level, feature_std 0.01, seeded) with identity position input and a decoder of --num-layers x --hidden-dim (torch's
+default init, seeded); octree and samples stay config 3's.
 """
 from __future__ import annotations
 
@@ -70,6 +74,7 @@ def main():
     ap.add_argument("--batches", default="512,65536,1048576")
     ap.add_argument("--num-layers", type=int, default=1)
     ap.add_argument("--hidden-dim", type=int, default=128)
+    ap.add_argument("--grid", choices=["octree", "hash"], default="octree")
     args = ap.parse_args()
     import wisp_b200 as W
     from oracle import octree_grid as OG
@@ -82,8 +87,17 @@ def main():
         case["W"], case["b"] = S.random_decoder(np.random.default_rng(4), 19, 1, args.hidden_dim, args.num_layers, scale=0.2)
     lr, eps = 1e-3, 1e-15
 
+    def make_nef():
+        if args.grid == "octree":
+            return sdf_nef_from_case(case)
+        torch.manual_seed(0)
+        blas = W.OctreeAS(torch.from_numpy(case["octree"]).cuda())
+        grid = W.HashGrid.from_geometric(blas, feature_dim=8, num_lods=4, multiscale_type='cat', feature_std=0.01, codebook_bitwidth=19,
+                                         min_grid_res=16, max_grid_res=2048)
+        return W.NeuralSDF(grid, pos_embedder='none', position_input=True, hidden_dim=args.hidden_dim, num_layers=args.num_layers).cuda()
+
     # parity: SDFStep's gradients and loss against the autograd route at batch 65 536
-    nef = sdf_nef_from_case(case)
+    nef = make_nef()
     step = W.SDFStep(W.Pipeline(nef), lr=lr, eps=eps)
     c, gt = _points(case, 65536, 1)
     loss = float(step.step(c, gt, update=False))
@@ -93,7 +107,7 @@ def main():
     ref.backward()
     ref = ref.detach()
     got = list(step.g_feats) + [step.g_dec]
-    refs = [f.grad for f in nef.grid.features] + [torch.cat([p.grad.reshape(-1) for p in W.ops.decoder_params(nef.decoder)])]
+    refs = [f.grad for f in W.SDFStep._grid_tensors(nef.grid)] + [torch.cat([p.grad.reshape(-1) for p in W.ops.decoder_params(nef.decoder)])]
     grad_err = max(float((a - b).abs().max() / b.abs().max().clamp_min(1e-30)) for a, b in zip(got, refs))
     loss_err = abs(loss - float(ref)) / abs(float(ref))
     parity = dict(batch=65536, loss=loss, loss_autograd=float(ref), loss_relerr=loss_err, grad_relerr_of_max=grad_err,
@@ -102,7 +116,7 @@ def main():
 
     arms = {}
     for B in [int(b) for b in args.batches.split(",")]:
-        nef_n, nef_a = sdf_nef_from_case(case), sdf_nef_from_case(case)
+        nef_n, nef_a = make_nef(), make_nef()
         native = W.SDFStep(W.Pipeline(nef_n), lr=lr, eps=eps)
         opt = _torch_adam(nef_a, lr, eps)
         coords, gts = _points(case, B, 2)
@@ -130,7 +144,7 @@ def main():
                         for k, v in res.items()}
         arms[str(B)]["speedup"] = arms[str(B)]["autograd"]["ms_per_step"] / arms[str(B)]["native"]["ms_per_step"]
     name, power = _gpu_info()
-    print(json.dumps(dict(workload="sdf_step_config3", num_layers=args.num_layers, hidden_dim=args.hidden_dim, fused=step.fused, device=name, power_limit=power, steps=args.steps, warmup=args.warmup,
+    print(json.dumps(dict(workload="sdf_step_config3" if args.grid == "octree" else "sdf_step_nglod_hash", num_layers=args.num_layers, hidden_dim=args.hidden_dim, fused=step.fused, device=name, power_limit=power, steps=args.steps, warmup=args.warmup,
                           batches=arms, parity=parity)))
     if not parity["ok"]:
         sys.exit(1)

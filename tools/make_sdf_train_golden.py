@@ -3,9 +3,9 @@
 (wisp/trainers/sdf_trainer.py:65-124) with the optimiser of its BaseTrainer.init_optimizer (wisp/trainers/base_trainer.py:205-239),
 run on CPU from an UNMODIFIED kaolin-wisp checkout (TEST INFRASTRUCTURE).
 
-    python tools/make_sdf_train_golden.py [--deep] [path/to/kaolin-wisp]
+    python tools/make_sdf_train_golden.py [--deep | --hash] [path/to/kaolin-wisp]
 
-Writes only sdf_train.npz, or with --deep only sdf_train_deep.npz.  Kaolin calls are answered by the oracle (oracle/ref_import.py).  The two trainer modules are loaded
+Writes only sdf_train.npz, or with --deep only sdf_train_deep.npz, or with --hash only sdf_train_hash.npz.  Kaolin calls are answered by the oracle (oracle/ref_import.py).  The two trainer modules are loaded
 from their files; the trainer object is created without its constructor and given what step() and init_optimizer() read.
 init_optimizer's `instantiate(cfg.optimizer, params=groups)` is answered by torch.optim.Adam(groups, lr, betas, eps): the decoder
 group carries its weight decay, the grid and rest groups Adam's default of none (the reference's instantiate would also pass
@@ -13,7 +13,10 @@ cfg.optimizer.weight_decay as that default; the nglod configs train with weight_
 
 Cases (the octahedron model of oracle/make_golden.py:gen_sdf at level 5, 3 LODs, F = 8, H = 16): 'sum' and 'cat' with only_last,
 and 'sum' over all LODs, with one hidden layer; --deep: 'sum' only_last with 2 hidden layers, 'cat' only_last with 3, and 'sum'
-over all LODs with 2 (the deeper layers pass the six |x|-units through unchanged, as oracle.sdf_reference.random_decoder).  grid_lr_weight = 5 and weight_decay = 1e-2 so that every group is pinned.  Recorded per case: the initial
+over all LODs with 2 (the deeper layers pass the six |x|-units through unchanged, as oracle.sdf_reference.random_decoder);
+--hash: the reference's NeuralSDF(HashGrid.from_geometric(4 LODs, 4 .. 32, codebook_bitwidth 10: dense levels 4 and 8, hashed
+levels 16 and 32 with collisions)), 'cat' F = 8 only_last, 'sum' F = 4 only_last, 'cat' F = 8 over all LODs, and 'cat' F = 8 with
+2 hidden layers (the hash kernels answered by the oracle).  grid_lr_weight = 5 and weight_decay = 1e-2 so that every group is pinned.  Recorded per case: the initial
 parameters, the loss of each step, the gradients of step 1 (after backward(), before optimizer.step()) and the parameters after
 steps 1 and 3."""
 from __future__ import annotations
@@ -33,6 +36,7 @@ sys.path.insert(0, ROOT)
 LR, EPS, WD, GRID_LR_WEIGHT, STEPS, N = 1e-3, 1e-15, 1e-2, 5.0, 3, 256
 CASES = {"sum": ("sum", True, 1), "cat": ("cat", True, 1), "sum_all": ("sum", False, 1)}
 DEEP_CASES = {"sum": ("sum", True, 2), "cat": ("cat", True, 3), "sum_all": ("sum", False, 2)}
+HASH_CASES = {"cat": ("cat", True, 1, 8), "sum": ("sum", True, 1, 4), "cat_all": ("cat", False, 1, 8), "cat_l2": ("cat", True, 2, 8)}
 
 
 def _load(name, path):
@@ -50,15 +54,15 @@ def main():
     from oracle import oracle as O
     from oracle import ref_import
     args = sys.argv[1:]
-    deep = "--deep" in args
-    args = [a for a in args if a != "--deep"]
+    deep, hashed = "--deep" in args, "--hash" in args
+    args = [a for a in args if a not in ("--deep", "--hash")]
     if args:
         ref_import.REF_ROOT = args[0]
     warnings.filterwarnings("ignore")
     ref_import.install()
     import wisp.models, wisp.models.pipeline, wisp.framework, wisp.datasets, wisp.trainers     # noqa: F401
     from wisp.accelstructs import OctreeAS
-    from wisp.models.grids import OctreeGrid
+    from wisp.models.grids import HashGrid, OctreeGrid
     from wisp.models.nefs import NeuralSDF
     from wisp.models import Pipeline
     from oracle.make_golden import octahedron_points
@@ -71,10 +75,16 @@ def main():
     coords = rng.uniform(-0.7, 0.7, (N, 3)).astype(np.float32)
     sdf = ((np.abs(coords).sum(-1, keepdims=True) - 0.3) / np.sqrt(3.0) + rng.normal(0.0, 0.01, (N, 1))).astype(np.float32)
     out = dict(octree=oct_np, level=level, coords=coords, sdf=sdf, lr=LR, eps=EPS, weight_decay=WD, grid_lr_weight=GRID_LR_WEIGHT)
-    for name, (ms, only_last, layers) in (DEEP_CASES if deep else CASES).items():
+    cases = HASH_CASES if hashed else {k: v + (8,) for k, v in (DEEP_CASES if deep else CASES).items()}
+    for name, (ms, only_last, layers, F) in cases.items():
         torch.manual_seed(7)
         blas = OctreeAS(torch.from_numpy(oct_np))
-        grid = OctreeGrid(blas, feature_dim=8, num_lods=3, interpolation_type='linear', multiscale_type=ms, feature_std=0.05)
+        if hashed:
+            grid = HashGrid.from_geometric(blas, feature_dim=F, num_lods=4, multiscale_type=ms, feature_std=0.05, feature_bias=0.0,
+                                           codebook_bitwidth=10, min_grid_res=4, max_grid_res=32)
+        else:
+            grid = OctreeGrid(blas, feature_dim=8, num_lods=3, interpolation_type='linear', multiscale_type=ms, feature_std=0.05)
+        nl = grid.num_lods
         nef = NeuralSDF(grid, pos_embedder='none', position_input=True, hidden_dim=16, num_layers=layers)
         with torch.no_grad():       # sdf ~ (|x|+|y|+|z|)/sqrt(3) - 0.3 + small learned perturbation (as gen_sdf)
             W0 = nef.decoder.layers[0].weight; W0.mul_(0.05)
@@ -88,7 +98,7 @@ def main():
         t = object.__new__(st.SDFTrainer)
         t.pipeline = Pipeline(nef=nef, tracer=None)
         t.device = 'cpu'
-        t.loss_lods = [2] if only_last else [0, 1, 2]
+        t.loss_lods = [nl - 1] if only_last else list(range(nl))
         t.tracker = SimpleNamespace(metrics=SimpleNamespace(total_loss=0., l2_loss=0., rgb_loss=0., num_samples=0))
         t.train_dataset = [None]
         t.cfg = SimpleNamespace(optimizer=SimpleNamespace(lr=LR, eps=EPS, weight_decay=WD, betas=(0.9, 0.999)), grid_lr_weight=GRID_LR_WEIGHT,
@@ -101,6 +111,9 @@ def main():
                 grads.update({n: p.grad.numpy().copy() for n, p in nef.named_parameters() if p.grad is not None})
         t.optimizer.register_step_pre_hook(record_first_grads)
         d = {f"{name}_multiscale": ms, f"{name}_loss_lods": np.asarray(t.loss_lods)}
+        if hashed:
+            d.update({f"{name}_feature_dim": F, f"{name}_num_layers": layers, f"{name}_resolutions": np.asarray(grid.resolutions),
+                      f"{name}_codebook_bitwidth": 10})
         d.update({f"{name}_init_{k}": v for k, v in _params(nef).items()})
         losses = []
         for s in range(STEPS):
@@ -114,7 +127,7 @@ def main():
         d[f"{name}_losses"] = np.asarray(losses, np.float64)
         out.update(d)
         print(name, "losses", losses, "params", len(_params(nef)), "grads", len(grads))
-    path = os.path.join(ROOT, "tests", "golden", "sdf_train_deep.npz" if deep else "sdf_train.npz")
+    path = os.path.join(ROOT, "tests", "golden", "sdf_train_hash.npz" if hashed else "sdf_train_deep.npz" if deep else "sdf_train.npz")
     np.savez_compressed(path, **out)
     print(path)
 

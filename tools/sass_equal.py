@@ -1,10 +1,13 @@
 #!/usr/bin/env python
 """Compare the SASS of the kernels in two object files / shared libraries instruction by instruction.
 
-    python tools/sass_equal.py OLD.o NEW.o [substring ...]
+    python tools/sass_equal.py OLD.o NEW.o [--appended TYPE ...] [substring ...]
 
 Used when a change must leave GPU-validated kernels untouched (no GPU at hand): template parameters with a `false` default are
-folded away, so `kernel<3>` in OLD is matched with `kernel<3, false>` in NEW.  Exit code 1 if any matched kernel differs."""
+folded away, so `kernel<3>` in OLD is matched with `kernel<3, false>` in NEW, and a kernel that only gained that parameter
+(`kernel` -> `kernel<false>`) with its old self.  --appended TYPE folds away a trailing parameter of struct type TYPE that NEW's
+kernels gained (`kernel(a, b)` -> `kernel(a, b, TYPE)`); such a kernel's SASS can only be identical when the instance ignores it.
+Exit code 1 if any matched kernel differs or is missing."""
 import re
 import subprocess
 import sys
@@ -24,12 +27,24 @@ def functions(path):
 
 def main():
     old, new = functions(sys.argv[1]), functions(sys.argv[2])
-    want = sys.argv[3:]
+    rest, appended = sys.argv[3:], []
+    while "--appended" in rest:
+        i = rest.index("--appended")
+        appended.append(rest[i + 1]); del rest[i:i + 2]
+    want = rest
+    tails = [f"{len(t)}{t}" for t in appended]
+
+    def fold(kk):
+        kk = re.sub(r"I(Lb0E)+Ev", "", re.sub(r"(ELb0)+EE", "EE", kk))
+        for t in tails:
+            if kk.endswith(t):
+                kk = kk[:-len(t)]
+        return kk
     bad = 0
     for k, v in sorted(old.items()):
         if want and not any(w in k for w in want):
             continue
-        match = [kk for kk in new if kk == k or re.sub(r"(ELb0)+EE", "EE", kk) == k]
+        match = [kk for kk in new if kk == k or fold(kk) == k]
         if not match:
             print(f"{k[:70]:70s} MISSING in {sys.argv[2]}"); bad += 1; continue
         same = v == new[match[0]]
