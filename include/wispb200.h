@@ -403,8 +403,8 @@ int wb_codebook_rows_bwd(const float* logits, const float* dictionary, const flo
  *       sum * inv_count; *loss_out (device float, zeroed by the caller) receives the loss value.
  *   wb_adam_step : torch.optim.Adam (amsgrad off) over up to 64 tensors in one launch; per-segment lr and weight decay carry the
  *       reference's parameter groups; grad_scale multiplies every gradient first (1/world after an all-reduce(sum)); zero_grad != 0
- *       clears each gradient as it is consumed.  desc_dev: device scratch, desc_pinned: page-locked host scratch, both
- *       wb_adam_desc_bytes() bytes, owned by the caller for as long as steps are in flight.
+ *       clears each gradient as it is consumed.  The step's description (segments, bias corrections, scales) is passed to the
+ *       kernel by value, so segs may be reused as soon as the call returns, however far the host runs ahead of the stream.
  * ---------------------------------------------------------------------------------------------- */
 int wb_composite_bwd_loss(const float* shaded, const float* depth, const float* deltas, const int64_t* offsets, int64_t R,
                           const float* bg, const float* rgb_pred, const float* target, int32_t loss_type, float inv_count,
@@ -414,9 +414,8 @@ typedef struct wb_adam_segment {
     int64_t numel;
     float lr, weight_decay;
 } wb_adam_segment;
-int64_t wb_adam_desc_bytes(void);
 int wb_adam_step(const wb_adam_segment* segs, int32_t nseg, float beta1, float beta2, float eps, int32_t step, float grad_scale,
-                 int32_t zero_grad, void* desc_dev, void* desc_pinned, wb_stream s);
+                 int32_t zero_grad, wb_stream s);
 
 /* ------------------------------------------------------------------------------------------------
  * Ray generation (camera -> rays on the device); origin/view/right/up/cam_pos/rotation are HOST pointers (launch parameters).

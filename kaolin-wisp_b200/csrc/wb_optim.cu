@@ -12,13 +12,16 @@
 #define WB_ADAM_MAX_SEG 64
 struct WbAdamSeg { float* p; float* g; float* m; float* v; int64_t n; float lr, wd; };
 struct WbAdam { WbAdamSeg seg[WB_ADAM_MAX_SEG]; int nseg; float b1, b2, eps, bc1, bc2_sqrt, grad_scale; int zero_grad; };
+// The step description travels as a kernel parameter: the launch copies it, so the host may build the next step's description
+// while this one is still queued (a host staging buffer + cudaMemcpyAsync would be overwritten by a host running steps ahead).
+static_assert(sizeof(WbAdam) <= 4096, "WbAdam must fit the 4 KB kernel parameter space");
 
 __global__ void __launch_bounds__(256)
-wb_adam_kernel(const WbAdam* __restrict__ A)
+wb_adam_kernel(const __grid_constant__ WbAdam A)
 {
-    const float b1 = A->b1, b2 = A->b2, eps = A->eps, bc1 = A->bc1, bc2s = A->bc2_sqrt, gs = A->grad_scale;
-    for (int k = 0; k < A->nseg; ++k) {
-        const WbAdamSeg sg = A->seg[k];
+    const float b1 = A.b1, b2 = A.b2, eps = A.eps, bc1 = A.bc1, bc2s = A.bc2_sqrt, gs = A.grad_scale;
+    for (int k = 0; k < A.nseg; ++k) {
+        const WbAdamSeg sg = A.seg[k];
         const float step_size = sg.lr / bc1;
         const int64_t n4 = ((reinterpret_cast<uintptr_t>(sg.p) | reinterpret_cast<uintptr_t>(sg.g) | reinterpret_cast<uintptr_t>(sg.m) |
                              reinterpret_cast<uintptr_t>(sg.v)) & 15u) == 0 ? sg.n / 4 : 0;
@@ -34,40 +37,36 @@ wb_adam_kernel(const WbAdam* __restrict__ A)
                 pp[c] -= step_size * (mp[c] / (sqrtf(vp[c]) / bc2s + eps));
             }
             reinterpret_cast<float4*>(sg.p)[i] = p; reinterpret_cast<float4*>(sg.m)[i] = m; reinterpret_cast<float4*>(sg.v)[i] = v;
-            if (A->zero_grad) reinterpret_cast<float4*>(sg.g)[i] = make_float4(0, 0, 0, 0);
+            if (A.zero_grad) reinterpret_cast<float4*>(sg.g)[i] = make_float4(0, 0, 0, 0);
         }
         for (int64_t i = n4 * 4 + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < sg.n; i += (int64_t)gridDim.x * blockDim.x) {
             float gg = sg.g[i] * gs; if (sg.wd != 0.0f) gg = fmaf(sg.wd, sg.p[i], gg);
             const float m = fmaf(b1, sg.m[i], (1.0f - b1) * gg), v = fmaf(b2, sg.v[i], (1.0f - b2) * gg * gg);
             sg.m[i] = m; sg.v[i] = v;
             sg.p[i] -= step_size * (m / (sqrtf(v) / bc2s + eps));
-            if (A->zero_grad) sg.g[i] = 0.0f;
+            if (A.zero_grad) sg.g[i] = 0.0f;
         }
     }
 }
 
-// segs: HOST array of nseg wb_adam_segment; desc_dev: device scratch of wb_adam_desc_bytes() bytes (the segment table is copied
-// there with cudaMemcpyAsync: > 4 KB of launch parameters otherwise)
-extern "C" int64_t wb_adam_desc_bytes(void) { return (int64_t)sizeof(WbAdam); }
+// segs: HOST array of nseg wb_adam_segment, read before this call returns
 extern "C" int wb_adam_step(const wb_adam_segment* segs, int32_t nseg, float beta1, float beta2, float eps, int32_t step, float grad_scale,
-                            int32_t zero_grad, void* desc_dev, void* desc_pinned, wb_stream s)
+                            int32_t zero_grad, wb_stream s)
 {
-    WB_CHECK_ARG(segs && desc_dev && desc_pinned, "null pointer");
+    WB_CHECK_ARG(segs, "null pointer");
     WB_CHECK_ARG(nseg >= 1 && nseg <= WB_ADAM_MAX_SEG && step >= 1, "nseg must be 1..64 and step >= 1");
-    WbAdam* A = reinterpret_cast<WbAdam*>(desc_pinned);
+    WbAdam A{};
     int64_t total = 0;
     for (int k = 0; k < nseg; ++k) {
         WB_CHECK_ARG(segs[k].param && segs[k].grad && segs[k].exp_avg && segs[k].exp_avg_sq && segs[k].numel >= 0, "bad segment");
-        A->seg[k] = WbAdamSeg{ segs[k].param, segs[k].grad, segs[k].exp_avg, segs[k].exp_avg_sq, segs[k].numel, segs[k].lr, segs[k].weight_decay };
+        A.seg[k] = WbAdamSeg{ segs[k].param, segs[k].grad, segs[k].exp_avg, segs[k].exp_avg_sq, segs[k].numel, segs[k].lr, segs[k].weight_decay };
         total += segs[k].numel;
     }
-    A->nseg = nseg; A->b1 = beta1; A->b2 = beta2; A->eps = eps; A->grad_scale = grad_scale; A->zero_grad = zero_grad;
-    A->bc1 = (float)(1.0 - pow((double)beta1, (double)step));
-    A->bc2_sqrt = (float)sqrt(1.0 - pow((double)beta2, (double)step));
-    cudaStream_t st = (cudaStream_t)s;
-    WB_CUDA(cudaMemcpyAsync(desc_dev, A, sizeof(WbAdam), cudaMemcpyHostToDevice, st));
+    A.nseg = nseg; A.b1 = beta1; A.b2 = beta2; A.eps = eps; A.grad_scale = grad_scale; A.zero_grad = zero_grad;
+    A.bc1 = (float)(1.0 - pow((double)beta1, (double)step));
+    A.bc2_sqrt = (float)sqrt(1.0 - pow((double)beta2, (double)step));
     int64_t ctas = (total / 4 + 255) / 256; const int64_t cap = (int64_t)wb_num_sms() * 8; if (ctas > cap) ctas = cap; if (ctas < 1) ctas = 1;
-    wb_adam_kernel<<<(unsigned)ctas, 256, 0, st>>>(reinterpret_cast<const WbAdam*>(desc_dev));
+    wb_adam_kernel<<<(unsigned)ctas, 256, 0, (cudaStream_t)s>>>(A);
     WB_LAUNCH_CHECK();
     return WB_OK;
 }

@@ -34,12 +34,8 @@ class NativeAdam:
     def __init__(self, entries, betas=(0.9, 0.999), eps=1e-8):
         self.entries = [(p, float(lr), float(wd)) for p, lr, wd in entries]
         self.betas, self.eps, self.t = betas, float(eps), 0
-        dev = self.entries[0][0].device
         self.exp_avg = [torch.zeros_like(p, dtype=torch.float32) for p, _, _ in self.entries]
         self.exp_avg_sq = [torch.zeros_like(p, dtype=torch.float32) for p, _, _ in self.entries]
-        nb = int(A.lib().wb_adam_desc_bytes())
-        self._dev = torch.empty(nb, dtype=torch.uint8, device=dev)
-        self._pinned = [torch.empty(nb, dtype=torch.uint8).pin_memory() for _ in range(4)]      # ring: a step's table is read by an async copy
 
     def step(self, grads, grad_scale: float = 1.0, zero_grad: bool = True):
         self.t += 1
@@ -49,9 +45,8 @@ class NativeAdam:
             assert g.is_contiguous() and p.is_contiguous() and g.numel() == p.numel() and p.dtype == torch.float32 and g.dtype == torch.float32
             segs[k].param, segs[k].grad, segs[k].exp_avg, segs[k].exp_avg_sq = p.data_ptr(), g.data_ptr(), self.exp_avg[k].data_ptr(), self.exp_avg_sq[k].data_ptr()
             segs[k].numel, segs[k].lr, segs[k].weight_decay = p.numel(), lr, wd
-        pin = self._pinned[self.t % len(self._pinned)]
         A.check(A.lib().wb_adam_step(segs, C.c_int32(n), C.c_float(self.betas[0]), C.c_float(self.betas[1]), C.c_float(self.eps), C.c_int32(self.t),
-                                     C.c_float(grad_scale), C.c_int32(int(zero_grad)), A.ptr(self._dev), C.c_void_p(pin.data_ptr()), A.stream()))
+                                     C.c_float(grad_scale), C.c_int32(int(zero_grad)), A.stream()))
 
 
 def _flatten_in_place(module_params):
