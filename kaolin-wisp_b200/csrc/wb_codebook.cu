@@ -22,15 +22,18 @@ __device__ __forceinline__ float wb_warp_max(float v) {
     return v;
 }
 
-// softmax statistics + argmax (lowest index among equal maxima, as torch.max) of one row held as KPL values per lane
+// softmax statistics + argmax (lowest index among equal maxima, as torch.max) of one row held as KPL values per lane.
+// Seeded with -inf, so every finite logit, -FLT_MAX included, can be a lane's maximum; padding lanes (k >= K) hold -inf and
+// never win, and a lane without logits keeps mi = K and mx = -inf != gmx.  For any finite row amax lies in [0, K) and the
+// maximum's expf(0) = 1 keeps the sum >= 1.
 template <int KPL>
 __device__ __forceinline__ void cb_row_softmax(const float* __restrict__ row, int K, int lane, float y[KPL], int& amax)
 {
-    float mx = -3.0e38f; int mi = 0x7fffffff;
+    float mx = -INFINITY; int mi = K;
 #pragma unroll
     for (int i = 0; i < KPL; ++i) {
         const int k = lane + 32 * i;
-        y[i] = k < K ? __ldg(row + k) : -3.0e38f;
+        y[i] = k < K ? __ldg(row + k) : -INFINITY;
         if (y[i] > mx) { mx = y[i]; mi = k; }
     }
     const float gmx = wb_warp_max(mx);
