@@ -274,6 +274,17 @@ int wb_sdf_train(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, 
  * wb_sdf_eval refuses, or a decoder with more than one hidden layer whose weights, weight-gradient accumulators and a 32-sample
  * tile exceed 227 KB).  Host only: no device is touched. */
 int64_t wb_sdf_train_smem_bytes(const wb_sdf_desc* nef);
+/* wb_sdf_train_tc: wb_sdf_train with the reference's enable_amp arithmetic (torch.cuda.amp.autocast around SDFTrainer.step,
+ * wisp/trainers/base_trainer.py:338; sdf_trainer.py:65-124) on the tensor cores: every decoder nn.Linear takes fp16 inputs, weights
+ * and biases, accumulates in fp32 and rounds its output (the prediction included) to fp16; the loss is fp32.  Same arguments and
+ * accumulate-into semantics as wb_sdf_train, gradients in fp32.  Deviations: the hash table is read in fp32, the output gradient
+ * carries a power-of-two loss scale (removed exactly in fp32), weight gradients accumulate in fp32 over the batch.  Decoders with
+ * 1 to 4 hidden layers whose footprint fits (wb_sdf_train_tc_smem_bytes(nef) >= 0; otherwise the call fails). */
+int wb_sdf_train_tc(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, const float* coords, const float* sdf_gt, int64_t N,
+                    float inv_count, float* const* grad_feats, float* grad_params, float* loss_out, wb_stream s);
+/* Dynamic shared memory (bytes) of a wb_sdf_train_tc launch: fp16 weight packs, fp32 weight-gradient accumulators and one 64-sample
+ * tile; < 0 when that exceeds 227 KB or wb_sdf_eval refuses the description.  Host only. */
+int64_t wb_sdf_train_tc_smem_bytes(const wb_sdf_desc* nef);
 /* Per-pack state of the sphere tracer (pack = ray with >= 1 nugget).  All device pointers, allocated by the caller for R rays;
  * nothing needs initialising.  state bit 0 = alive (the reference's `mask`), bit 1 = hit. */
 typedef struct wb_sdf_state {

@@ -80,7 +80,7 @@ EXPORTS = [
     "wb_raymarch_ray_count", "wb_scan_workspace_bytes", "wb_scan_counts", "wb_raymarch_ray_fill",
     "wb_raytrace_count", "wb_raytrace_fill", "wb_raytrace_cache_bytes", "wb_raytrace_count_cached", "wb_raytrace_fill_cached", "wb_raymarch_voxel_fill", "wb_raymarch_uniform_count", "wb_raymarch_uniform_fill",
     "wb_hashgrid_fwd", "wb_hashgrid_bwd", "wb_triplane_fwd", "wb_triplane_bwd", "wb_triplane_relayout",
-    "wb_octree_interp_fwd", "wb_octree_interp_bwd", "wb_find_depth_bound", "wb_sdf_eval", "wb_sdf_train", "wb_sdf_train_smem_bytes", "wb_sdf_trace", "wb_sdf_phase", "wb_composite_fwd", "wb_composite_bwd",
+    "wb_octree_interp_fwd", "wb_octree_interp_bwd", "wb_find_depth_bound", "wb_sdf_eval", "wb_sdf_train", "wb_sdf_train_smem_bytes", "wb_sdf_train_tc", "wb_sdf_train_tc_smem_bytes", "wb_sdf_trace", "wb_sdf_phase", "wb_composite_fwd", "wb_composite_bwd",
     "wb_rf_march_fill", "wb_rf_param_blob_floats", "wb_rf_precision_supported", "wb_rf_pack_params", "wb_rf_shade_fwd", "wb_rf_shade_bwd",
     "wb_rf_workspace_bytes", "wb_rf_feat_bytes", "wb_rf_decoder_bwd", "wb_rf_table_scatter", "wb_rf_loss_scale", "wb_rf_workspace_holds_ray_rows", "wb_prune_samples", "wb_prune_update", "wb_raygen_lookat", "wb_raygen_pinhole", "wb_codebook_rows_fwd", "wb_codebook_rows_bwd", "wb_composite_bwd_loss", "wb_adam_step", "wb_tc_selftest",
 ]
@@ -113,6 +113,7 @@ def lib() -> C.CDLL:
         L.wb_rf_feat_bytes.restype = C.c_int64
         L.wb_raytrace_cache_bytes.restype = C.c_int64
         L.wb_sdf_train_smem_bytes.restype = C.c_int64
+        L.wb_sdf_train_tc_smem_bytes.restype = C.c_int64
         _lib = L
     return _lib
 

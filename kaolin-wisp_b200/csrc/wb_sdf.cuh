@@ -198,5 +198,35 @@ __device__ __forceinline__ void sdf_hash_features(const WbGrid& g, int nl, float
     }
 }
 
+// The scatter of a hash field (HashGrid.interpolate's backward, wb_hashgrid_bwd's products): per LOD and corner fl(g * c_j) added to
+// the table gradient gt [rows, F] with one float4 reduction per corner and quad of features; quads of zero gradients are skipped, and
+// the 'cat' LODs >= lod_idx = nl - 1, whose features the forward zeroed, get nothing.  grad(f): dL/dfeat of decoder-input feature f.
+// Shared by the training kernels of wb_sdf_train.cu and wb_sdf_train_tc.cu.
+template <class Grad>
+__device__ __forceinline__ void sdf_hash_scatter(const WbGrid& g, float* gt, int nl, float cx, float cy, float cz, Grad grad)
+{
+    const int F = g.F, nq = F / 4;
+    const bool sum = g.multiscale != 0;
+    const int act = sum ? g.L : nl - 1;
+    for (int l = 0; l < act; ++l) {
+        float gv[8];
+        bool any = false;
+#pragma unroll
+        for (int f = 0; f < 8; ++f) { gv[f] = f < F ? grad(sum ? f : l * F + f) : 0.0f; any |= gv[f] != 0.0f; }
+        if (!any) continue;
+        uint32_t idx[8]; float cf[8];
+        wb_corner_setup(g, l, cx, cy, cz, idx, cf);
+        float4* tb = reinterpret_cast<float4*>(gt + g.begin[l] * F);
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+            if (q >= nq) break;
+            const float g0 = gv[4 * q], g1 = gv[4 * q + 1], g2 = gv[4 * q + 2], g3 = gv[4 * q + 3];
+            if (g0 == 0.0f && g1 == 0.0f && g2 == 0.0f && g3 == 0.0f) continue;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) atomicAdd(tb + (int64_t)idx[j] * nq + q, make_float4(g0 * cf[j], g1 * cf[j], g2 * cf[j], g3 * cf[j]));
+        }
+    }
+}
+
 // the app/nglod shape (nglod_octree.yaml): 'sum' grid of 16 features, identity position input, one hidden layer
 static inline bool sdf_fast_shape(const WbSdf& m) { return m.multiscale == 1 && m.F == 16 && m.pos_mode == 1 && m.nh == 1; }

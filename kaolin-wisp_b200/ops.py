@@ -668,13 +668,23 @@ def sdf_train_smem_bytes(fd) -> int:
     return int(A.lib().wb_sdf_train_smem_bytes(C.byref(fd[0])))
 
 
+def sdf_train_tc_smem_bytes(fd) -> int:
+    """Shared memory of a wb_sdf_train_tc launch (precision 1: fp16 weight packs, fp32 weight-gradient accumulators and one
+    64-sample tile) for the field fd = sdf_field(nef), or < 0 when the tensor-core step cannot train it."""
+    return int(A.lib().wb_sdf_train_tc_smem_bytes(C.byref(fd[0])))
+
+
 def sdf_train(fd, coords: torch.Tensor, sdf_gt: torch.Tensor, lod_idx: int, inv_count: float, grad_feats: Sequence[torch.Tensor],
-              grad_params: torch.Tensor, loss_out: torch.Tensor) -> None:
+              grad_params: torch.Tensor, loss_out: torch.Tensor, precision: int = 0) -> None:
     """Forward, L2 loss and backward of SDFTrainer.step (sdf_trainer.py:65-124) for one loss LOD in one launch (wb_sdf_train), for
     decoders of 1 to 4 hidden layers whose sdf_train_smem_bytes(fd) >= 0.  fd: sdf_field(nef) (its params pointer may be re-aimed
     at a flat decoder buffer); coords f32 [N,3], sdf_gt f32 [N] on the device.  Accumulates: loss_out[0] += sum (y - gt)^2 *
     inv_count, grad_params (packed like the decoder: [W0, b0, W1, b1, ..., Wout, bout]) and grad_feats[k], k <= lod_idx (octree
-    grid); for a hash field grad_feats[0] is dL/d codebook.feats [rows, F]."""
+    grid); for a hash field grad_feats[0] is dL/d codebook.feats [rows, F].  precision 1: the reference's enable_amp arithmetic on
+    the tensor cores (wb_sdf_train_tc: fp16 decoder operands and outputs, fp32 gradients), for fields whose
+    sdf_train_tc_smem_bytes(fd) >= 0."""
+    if precision not in (0, 1):
+        raise A.WispB200Error(f"sdf_train: precision must be 0 (fp32) or 1 (fp16 tensor cores), got {precision!r}")
     d, oct, _ = fd
     A.require_device(coords)
     if not (coords.dtype == sdf_gt.dtype == grad_params.dtype == loss_out.dtype == torch.float32 and coords.is_contiguous() and sdf_gt.is_contiguous()):
@@ -683,8 +693,9 @@ def sdf_train(fd, coords: torch.Tensor, sdf_gt: torch.Tensor, lod_idx: int, inv_
         raise A.WispB200Error(f"sdf_gt has {sdf_gt.numel()} values for {coords.shape[0]} points")
     gptrs = (C.c_void_p * len(grad_feats))(*[g.data_ptr() for g in grad_feats])
     od = _sdf_octree(oct)
+    fn = A.lib().wb_sdf_train_tc if precision == 1 else A.lib().wb_sdf_train
     with _stage("sdf_train"):
-        A.check(A.lib().wb_sdf_train(od, C.byref(d), C.c_int32(lod_idx), A.ptr(coords), A.ptr(sdf_gt), C.c_int64(coords.shape[0]),
+        A.check(fn(od, C.byref(d), C.c_int32(lod_idx), A.ptr(coords), A.ptr(sdf_gt), C.c_int64(coords.shape[0]),
                                      C.c_float(inv_count), gptrs, A.ptr(grad_params), A.ptr(loss_out), A.stream()))
 
 

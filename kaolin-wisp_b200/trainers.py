@@ -15,6 +15,7 @@ Fields outside the fused path (ops.nef_spec is None) fall back to autograd + the
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 from typing import Optional
 
@@ -255,13 +256,26 @@ class SDFStep:
     (forward, loss and backward, no autograd), then NativeAdam over every parameter in one launch.  The decoder's parameters are
     flattened in place into one buffer [W0, b0, W1, b1, ..., Wout, bout], which the kernel reads, whose gradient it writes and
     which is one Adam segment; the grid's tensors (OctreeGrid.features, or the one HashGrid codebook.feats table) are the other
-    segments.  The decoder and the hash table run in fp32 whatever the autocast state; the reference's enable_amp fp16
-    nn.Linear and fp16 table are not reproduced.  Every other field (NeuralSDF over a TriplanarGrid, a hash grid of F = 2 or over
-    8 features, a deeper decoder whose weights, weight-gradient accumulators and smallest sample tile exceed an SM's shared
-    memory: wb_sdf_train_smem_bytes < 0) takes autograd plus the same NativeAdam."""
+    segments.  Every other field (NeuralSDF over a TriplanarGrid, a hash grid of F = 2 or over 8 features, a deeper decoder whose
+    weights, weight-gradient accumulators and smallest sample tile exceed an SM's shared memory: wb_sdf_train_smem_bytes < 0)
+    takes autograd plus the same NativeAdam.
+
+    `precision` picks the arithmetic, whatever the autocast state:
+      0  fp32 decoder (wb_sdf_train; autograd in fp32); the reference's enable_amp fp16 nn.Linear is not reproduced.
+      1  the reference's enable_amp arithmetic (every app/nglod config sets enable_amp: True; BaseTrainer runs the step under
+         torch.cuda.amp.autocast, base_trainer.py:338): hash fields the native route trains whose tensor-core footprint fits
+         (wb_sdf_train_tc_smem_bytes >= 0: one or two hidden layers of 128, any 1-4 layers narrower) take one wb_sdf_train_tc
+         launch per loss LOD (fp16 decoder operands and outputs on the tensor cores, fp32 gradients), then the same NativeAdam;
+         the hash table stays fp32 (the reference casts it to fp16).  Every other field, octree fields included (the kernel
+         trains them through ops.sdf_train, but measured slower than autocast autograd at large batches), takes autograd inside
+         torch.autocast("cuda", torch.float16) plus NativeAdam.
+    `fused` tells which route was chosen."""
 
     def __init__(self, pipeline, lr: float = 1e-3, eps: float = 1e-15, weight_decay: float = 0.0, grid_lr_weight: float = 1.0,
-                 betas=(0.9, 0.999), only_last: bool = True):
+                 betas=(0.9, 0.999), only_last: bool = True, precision: int = 0):
+        if precision not in (0, 1) or isinstance(precision, bool):
+            raise ValueError(f"SDFStep: precision must be 0 (fp32) or 1 (fp16 autocast arithmetic), got {precision!r}")
+        self.precision = int(precision)
         self.pipeline, self.nef = pipeline, pipeline.nef
         nef = self.nef
         n = int(nef.grid.num_lods)
@@ -295,8 +309,8 @@ class SDFStep:
 
     def _fused_field(self, nef, params):
         """ops.sdf_field of the field with the decoder flattened in place and the description aimed at that buffer, or None when
-        the field is outside wb_sdf_train (neither an OctreeGrid nor a hash grid in ops.sdf_field's range, a decoder whose
-        training footprint exceeds shared memory, or trainable parameters beyond grid and decoder)."""
+        the field is outside wb_sdf_train (precision 1: wb_sdf_train_tc): neither an OctreeGrid nor a hash grid in ops.sdf_field's
+        range, a decoder whose training footprint exceeds shared memory, or trainable parameters beyond grid and decoder."""
         grid, dec = getattr(nef, "grid", None), getattr(nef, "decoder", None)
         if grid is None or dec is None or getattr(grid, "dictionary", None) is not None:
             return None
@@ -307,8 +321,11 @@ class SDFStep:
         if {id(p) for p in params} != {id(p) for p in feats + dparams} or any(p.dtype != torch.float32 for p in dparams):
             return None
         fd = ops.sdf_field(nef)
-        if fd is None or ops.sdf_train_smem_bytes(fd) < 0:
+        smem = ops.sdf_train_tc_smem_bytes if self.precision == 1 else ops.sdf_train_smem_bytes
+        if fd is None or smem(fd) < 0:
             return None
+        if self.precision == 1 and not fd[0].hash:
+            return None               # octree fields: wb_sdf_train_tc is slower than autograd under autocast (DESIGN section 7)
         self.dec_flat = _flatten_in_place(dparams)
         fd = ops.sdf_field(nef)
         d, oct, keep = fd
@@ -341,7 +358,7 @@ class SDFStep:
         c, g = A.f32c(pts).reshape(-1, 3), A.f32c(gts).reshape(-1)
         self.loss_buf.zero_()
         for lod in self.loss_lods:
-            ops.sdf_train(self.fd, c, g, lod, 1.0 / N, self.g_feats, self.g_dec, self.loss_buf)
+            ops.sdf_train(self.fd, c, g, lod, 1.0 / N, self.g_feats, self.g_dec, self.loss_buf, precision=self.precision)
         loss = self.loss_buf.clone()
         if update:
             with ops._stage("adam"):
@@ -361,10 +378,12 @@ class SDFStep:
         for p in self.params:
             p.grad = None                                                     # self.pipeline.zero_grad() (:77)
         loss = 0.0
-        for lod in self.loss_lods:
-            pred = self.nef(coords=pts, lod_idx=lod, channels="sdf")
-            loss = loss + ((pred - 1.0 * gts) ** 2).sum()
-        loss = loss / N
+        amp = torch.autocast("cuda", torch.float16) if self.precision == 1 else contextlib.nullcontext()
+        with amp:                                                             # base_trainer.py:338 with enable_amp
+            for lod in self.loss_lods:
+                pred = self.nef(coords=pts, lod_idx=lod, channels="sdf")
+                loss = loss + ((pred - 1.0 * gts) ** 2).sum()
+            loss = loss / N
         loss.backward()
         if update:
             grads = [(p.grad if p.grad is not None else torch.zeros_like(p)).contiguous() for p in self.params]
