@@ -40,7 +40,7 @@ class OctreeAS:
         self.points, self.pyramid, self.prefix = spc.octree_to_spc(octree)
         self.max_level = self.pyramid.shape[-1] - 2
         self.extent = dict()
-        self._tensors: Optional[ops.OctreeTensors] = None
+        self._wb_tensors: Optional[ops.OctreeTensors] = None        # ops.octree_tensors' cache
 
     # --- constructors (octree_as.py:122-144) ---------------------------------------------------------------
     @classmethod
@@ -57,15 +57,11 @@ class OctreeAS:
 
     # --- native handle ---------------------------------------------------------------------------------------
     def tensors(self) -> ops.OctreeTensors:
-        t = self._tensors
-        if t is None or t.octree.data_ptr() != self.octree.data_ptr():
-            t = ops.OctreeTensors(self.octree.contiguous(), self.prefix.contiguous(), self.points.contiguous(), self.pyramid.cpu(), self.max_level)
-            self._tensors = t
-        return t
+        return ops.octree_tensors(self)
 
     def to(self, device) -> "OctreeAS":
         self.octree, self.points, self.prefix = self.octree.to(device), self.points.to(device), self.prefix.to(device)
-        self._tensors = None
+        self._wb_tensors = None
         return self
 
     # --- queries (octree_as.py:146-163) ----------------------------------------------------------------------

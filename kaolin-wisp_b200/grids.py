@@ -209,13 +209,15 @@ class OctreeGrid(nn.Module):
             f.requires_grad_(False)
 
     def interpolate(self, coords, lod_idx):
-        """octree_grid.py:165-219."""
+        """octree_grid.py:165-219.  install() runs this body on the reference's OctreeGrid too, which has no `half_features` and
+        always rounds the features to half (octree_grid.py:149)."""
         output_shape = coords.shape[:-1]
         dev = self.features[0].device
         if self.trinkets.device != dev:
             self.trinkets = self.trinkets.to(dev)
-        feats = ops.OctreeInterpolate.apply(coords.reshape(-1, 3), self.blas.tensors(), self.trinkets, self.base_lod, self.multiscale_type if lod_idx > 0 else 'cat',
-                                            self.half_features, *[self.features[i] for i in range(lod_idx + 1)])
+        feats = ops.OctreeInterpolate.apply(coords.reshape(-1, 3), ops.octree_tensors(self.blas), self.trinkets.int(), self.base_lod,
+                                            self.multiscale_type if lod_idx > 0 else 'cat', getattr(self, "half_features", True),
+                                            *[self.features[i] for i in range(lod_idx + 1)])
         return feats.reshape(*output_shape, feats.shape[-1])
 
     def raymarch(self, rays, raymarch_type, num_samples, level=None, **kw) -> ASRaymarchResults:
@@ -255,7 +257,7 @@ class CodebookOctreeGrid(OctreeGrid):
         if self.trinkets.device != dev:
             self.trinkets = self.trinkets.to(dev)
         rows = [ops.CodebookRows.apply(self.features[i], self.dictionary[i], self.training) for i in range(lod_idx + 1)]
-        feats = ops.OctreeInterpolate.apply(coords.reshape(-1, 3), self.blas.tensors(), self.trinkets, self.base_lod,
+        feats = ops.OctreeInterpolate.apply(coords.reshape(-1, 3), ops.octree_tensors(self.blas), self.trinkets, self.base_lod,
                                             self.multiscale_type if lod_idx > 0 else 'cat', False, *rows)
         return feats.reshape(*output_shape, feats.shape[-1])
 

@@ -13,6 +13,8 @@ What is patched (reference file:line -> native replacement):
   NeuralRadianceField.prune                     (nerf.py:175-212)                  ops.prune_field
 Every replacement keeps the reference signature, falls back to the original method for configurations outside the native
 path (unknown embedders, activations, grids), and keeps the attributes other wisp code reads (`prev_num_samples`, `bg_color`).
+The grid and SDF-tracer replacements run the methods of this package's mirror classes (grids.py, tracers.py); the rest share
+their host logic with the mirrors through ops (octree_tensors, march, resolve_precision, sdf_channel).
 """
 from __future__ import annotations
 
@@ -20,17 +22,9 @@ import os
 
 import torch
 
-from . import ops
+from . import grids, ops, tracers
 
 _ORIG = {}          # (class name, method) -> original function, for uninstall() and the fall-backs
-
-
-def _octree_tensors(blas) -> ops.OctreeTensors:
-    t = getattr(blas, "_wb_tensors", None)
-    if t is None or t.octree.data_ptr() != blas.octree.data_ptr():
-        t = ops.OctreeTensors(blas.octree.contiguous(), blas.prefix.contiguous().int(), blas.points.contiguous(), blas.pyramid.cpu().int(), blas.max_level)
-        blas._wb_tensors = t
-    return t
 
 
 def _seed() -> int:
@@ -71,20 +65,20 @@ def install() -> bool:
 
     # ---- OctreeAS ------------------------------------------------------------------------------------------------
     def query(self, coords, level=None, with_parents=False):
-        return ASQueryResults(pidx=ops.query(_octree_tensors(self), coords, self.max_level if level is None else level, with_parents))
+        return ASQueryResults(pidx=ops.query(ops.octree_tensors(self), coords, self.max_level if level is None else level, with_parents))
 
     def raytrace(self, rays, level=None, with_exit=False):
-        ridx, pidx, depth, _ = ops.raytrace(_octree_tensors(self), rays.origins, rays.dirs, self.max_level if level is None else level)
+        ridx, pidx, depth, _ = ops.raytrace(ops.octree_tensors(self), rays.origins, rays.dirs, self.max_level if level is None else level)
         return ASRaytraceResults(ridx=ridx, pidx=pidx, depth=depth if with_exit else depth[:, 0:1].contiguous())
 
     def _raymarch_ray(self, rays, num_samples, level=None):
-        ms = ops.march_count(_octree_tensors(self), rays.origins, rays.dirs, rays.dist_min, rays.dist_max, num_samples,
+        ms = ops.march_count(ops.octree_tensors(self), rays.origins, rays.dirs, rays.dist_min, rays.dist_max, num_samples,
                              self.max_level if level is None else level, seed=_seed())
         ridx, samples, depth, deltas, boundary = ops.march_fill_reference_layout(ms, rays.origins.device)
         return ASRaymarchResults(ridx=ridx, samples=samples, depth_samples=depth, deltas=deltas, boundary=boundary, pack_info=None)
 
     def _nuggets(self, rays, num_samples, level, kind):
-        _, ref = ops.march_nuggets(_octree_tensors(self), rays.origins, rays.dirs, self.max_level if level is None else level, num_samples, kind,
+        _, ref = ops.march_nuggets(ops.octree_tensors(self), rays.origins, rays.dirs, self.max_level if level is None else level, num_samples, kind,
                                    reference_layout=True, seed=_seed())
         return ASRaymarchResults(pack_info=None, **ref)
 
@@ -100,31 +94,14 @@ def install() -> bool:
 
     # ---- grids ---------------------------------------------------------------------------------------------------
     def triplanar_interpolate(self, coords, lod_idx):
-        output_shape = coords.shape[:-1]
-        if coords.ndim < 3:
-            coords = coords[:, None]
-        planes = []
-        for i in range(lod_idx + 1):
-            f = self.features[i]
-            planes += [f.fmx, f.fmy, f.fmz]
         if self.interpolation_type != 'linear' or any(getattr(self.features[i], "padding_mode", "reflection") != "reflection" for i in range(lod_idx + 1)):
-            return _ORIG[("TriplanarGrid", "interpolate")][1](self, coords.reshape(*output_shape, coords.shape[-1]), lod_idx)
-        feats = ops.TriplaneInterpolate.apply(coords.reshape(-1, 3), lod_idx + 1, *planes)
-        feats = feats.reshape(*coords.shape[:-1], feats.shape[-1])
-        if self.multiscale_type == 'sum':
-            feats = feats.reshape(*output_shape, lod_idx + 1, feats.shape[-1] // (lod_idx + 1)).sum(-2)
-        return feats
+            return _ORIG[("TriplanarGrid", "interpolate")][1](self, coords, lod_idx)
+        return grids.TriplanarGrid.interpolate(self, coords, lod_idx)
 
     def octree_interpolate(self, coords, lod_idx):
         if self.interpolation_type != 'linear':
             return _ORIG[("OctreeGrid", "interpolate")][1](self, coords, lod_idx)
-        output_shape = coords.shape[:-1]
-        dev = self.features[0].device
-        if self.trinkets.device != dev:
-            self.trinkets = self.trinkets.to(dev)
-        feats = ops.OctreeInterpolate.apply(coords.reshape(-1, 3), _octree_tensors(self.blas), self.trinkets.int(), self.base_lod,
-                                            self.multiscale_type if lod_idx > 0 else 'cat', True, *[self.features[i] for i in range(lod_idx + 1)])
-        return feats.reshape(*output_shape, feats.shape[-1])
+        return grids.OctreeGrid.interpolate(self, coords, lod_idx)
 
     _patch(TriplanarGrid, "interpolate", triplanar_interpolate)
     _patch(OctreeGrid, "interpolate", octree_interpolate)
@@ -142,52 +119,26 @@ def install() -> bool:
             return orig_trace(self, nef, rays, channels, extra_channels, lod_idx=lod_idx, raymarch_type=raymarch_type,
                               num_steps=num_steps, step_size=step_size, bg_color=bg_color)
         self.bg_color = self.bg_color.to(rays.origins.device)
-        blas = nef.grid.blas
-        oct = _octree_tensors(blas)
-        level = ops.raymarch_level(nef.grid, lod_idx)
-        if raymarch_type == 'ray':
-            ms = ops.march_count(oct, rays.origins, rays.dirs, rays.dist_min, rays.dist_max, num_steps, level, seed=_seed())
-        else:
-            ms, _ = ops.march_nuggets(oct, rays.origins, rays.dirs, level, num_steps, raymarch_type, reference_layout=False, seed=_seed())
+        ms = ops.march(nef.grid, lod_idx, rays, raymarch_type, num_steps, seed=_seed())
         self.prev_num_samples = ms.total
         need_bwd = torch.is_grad_enabled() and any(p.requires_grad for p in nef.parameters())
-        precision = 1 if (torch.is_autocast_enabled() and ops.precision_supported(spec, nef, 1, need_bwd)) else 0
-        rgb, depth, alpha, hit = ops.rf_trace_nef(ms, spec, nef, self.bg_color, precision=precision)
+        rgb, depth, alpha, hit = ops.rf_trace_nef(ms, spec, nef, self.bg_color, precision=ops.resolve_precision(None, spec, nef, need_bwd))
         return RenderBuffer(depth=depth if "depth" in channels else None, hit=hit, rgb=rgb, alpha=alpha)
 
     _patch(PackedRFTracer, "trace", rf_trace)
 
     # ---- SDF tracer ----------------------------------------------------------------------------------------------
     def sdf_trace(self, nef, rays, channels, extra_channels, lod_idx=None, num_steps=64, step_size=1.0, min_dis=1e-4):
-        if lod_idx is None:
-            lod_idx = nef.grid.num_lods - 1
-        want_normals = "rgb" in channels or "normal" in channels
-        out, st = ops.sdf_trace(nef, _octree_tensors(nef.grid.blas), rays.origins, rays.dirs, rays.dist_max, nef.grid.active_lods[lod_idx], lod_idx,
-                                num_steps, step_size, min_dis, want_normals)
-        hit = out["hit"]
-        self.prev_num_evals = out.get("_evals")                          # device int32 [1] (fused kernel only): field evaluations of the trace
-        if st is not None and want_normals and bool(hit.any()):
-            grad = ops.finitediff_gradient(out["xyz"][hit], nef.get_forward_function("sdf"))
-            out["normal"][hit] = torch.nn.functional.normalize(grad, p=2, dim=-1, eps=1e-5)
-            out["rgb"] = (out["normal"] + 1.0) / 2.0
-        extra_outputs = {}
-        for channel in extra_channels:
-            feats = nef(coords=out["xyz"][hit], lod_idx=lod_idx, channels=channel)
-            buf = torch.zeros(*rays.origins.shape[:-1], feats.shape[-1], device=feats.device)
-            buf[hit] = feats.to(buf.dtype)
-            extra_outputs[channel] = buf
-        return RenderBuffer(xyz=out["xyz"], depth=out["depth"], hit=hit, normal=out["normal"], rgb=out["rgb"], alpha=out["alpha"], **extra_outputs)
+        rb = tracers.PackedSDFTracer.trace(self, nef, rays, channels, extra_channels, lod_idx, num_steps, step_size, min_dis)
+        # wisp code calls wisp's RenderBuffer methods (blend, image, exr_dict ...); the keyword order sets its fields' order
+        return RenderBuffer(**{c: getattr(rb, c) for c in ("xyz", "depth", "hit", "normal", "rgb", "alpha", *extra_channels)})
 
     _patch(PackedSDFTracer, "trace", sdf_trace)
 
     orig_sdf = NeuralSDF.sdf
 
     def sdf(self, coords, lod_idx=None):
-        if coords.shape[0] > 0 and coords.is_cuda and not torch.is_grad_enabled() and not torch.is_autocast_enabled():
-            fused = ops.sdf_eval(self, coords, lod_idx)
-            if fused is not None:
-                return dict(sdf=fused.reshape(*coords.shape[:-1], 1))
-        return orig_sdf(self, coords, lod_idx)
+        return ops.sdf_channel(self, coords, lod_idx) or orig_sdf(self, coords, lod_idx)
 
     _patch(NeuralSDF, "sdf", sdf)
 

@@ -168,7 +168,7 @@ class NeuralRadianceField(BaseNeuralField):
         """Prunes the blas based on the current state (nerf.py:175-212): decay the running occupancy, probe the density at one
         jittered point per finest-level cell, keep the cells above `prune_min_density`, rebuild the occupancy structure from them.
         All of it runs on the native path (ops.prune_field: probe points, fused gather + decoders, occupancy update); the next
-        raymarch rebuilds the native bit masks (OctreeAS.tensors()).  `jitter` ([cells, 3] in [0,1)) replays a given draw; `seed`
+        raymarch rebuilds the native bit masks (ops.octree_tensors).  `jitter` ([cells, 3] in [0,1)) replays a given draw; `seed`
         selects the counter-based stream (default: the prune-call count, identical on all ranks)."""
         if self.prune_density_decay is None or self.prune_min_density is None or self.grid is None:
             return
@@ -252,10 +252,9 @@ class NeuralSDF(BaseNeuralField):
             return dict(sdf=torch.zeros_like(coords)[..., 0:1])
         if lod_idx is None:
             lod_idx = self.grid.num_lods - 1
-        if not torch.is_grad_enabled() and coords.is_cuda and not torch.is_autocast_enabled():
-            fused = ops.sdf_eval(self, coords, lod_idx)
-            if fused is not None:
-                return dict(sdf=fused.reshape(*shape[:-1], 1))
+        fused = ops.sdf_channel(self, coords, lod_idx)
+        if fused is not None:
+            return fused
         if len(shape) == 2:
             coords = coords[:, None]
         num_samples = coords.shape[1]

@@ -90,6 +90,16 @@ class OctreeTensors:
             self.bbox = ([2.0 * m / res - 1.0 for m in mn], [2.0 * (m + 1) / res - 1.0 for m in mx])
 
 
+def octree_tensors(blas) -> OctreeTensors:
+    """The OctreeTensors of an OctreeAS (this package's or the reference's), cached on the BLAS and rebuilt when its octree tensor
+    is replaced.  prefix and pyramid are cast to int32 (the C ABI's type; already so for spc.scan_octree's)."""
+    t = getattr(blas, "_wb_tensors", None)
+    if t is None or t.octree.data_ptr() != blas.octree.data_ptr():
+        t = OctreeTensors(blas.octree.contiguous(), blas.prefix.contiguous().int(), blas.points.contiguous(), blas.pyramid.cpu().int(), blas.max_level)
+        blas._wb_tensors = t
+    return t
+
+
 def query(oct: OctreeTensors, coords: torch.Tensor, level: int, with_parents: bool = False) -> torch.Tensor:
     """spc_ops.unbatched_query(octree, prefix, coords, level, with_parents)  (octree_as.py:162)."""
     A.require_device(coords)
@@ -382,6 +392,14 @@ def march_nuggets(oct: OctreeTensors, origins, dirs, level: int, num_samples: in
     return ms, ref
 
 
+def march(grid, lod_idx: int, rays, raymarch_type: str, num_steps: int, jitter: Optional[torch.Tensor] = None, seed: int = 0) -> MarchState:
+    """The march of a fused trace at `lod_idx` over the grid's BLAS: 'ray' -> march_count, 'voxel' / 'uniform' -> march_nuggets."""
+    oct, level = octree_tensors(grid.blas), raymarch_level(grid, lod_idx)
+    if raymarch_type == 'ray':
+        return march_count(oct, rays.origins, rays.dirs, rays.dist_min, rays.dist_max, num_steps, level, jitter=jitter, seed=seed)
+    return march_nuggets(oct, rays.origins, rays.dirs, level, num_steps, raymarch_type, reference_layout=False, jitter=jitter, seed=seed)[0]
+
+
 # --------------------------------------------------------------------------------------------------------------
 # hash grid interpolate (unfused drop-in for wisp.ops.grid.hashgrid)
 # --------------------------------------------------------------------------------------------------------------
@@ -556,19 +574,6 @@ def finitediff_gradient(x: torch.Tensor, f, eps: float = 0.005) -> torch.Tensor:
 # --------------------------------------------------------------------------------------------------------------
 # NeuralSDF(OctreeGrid) + sphere tracing (app/nglod)
 # --------------------------------------------------------------------------------------------------------------
-def _sdf_embed_mode(nef):
-    """(pos_mode, pos_freq) of a NeuralSDF (neural_sdf.py:86-99): 0 none, 1 identity, 2 positional, 3 positional + input."""
-    pe = getattr(nef, "pos_embedder", None)
-    if pe is None:
-        return 0, 0
-    if isinstance(pe, torch.nn.Identity):
-        return 1, 0
-    nf = int(getattr(pe, "num_freq", 0))
-    if nf <= 0 or not getattr(pe, "log_sampling", True) or int(round(float(getattr(pe, "max_freq_log2", nf - 1)))) != nf - 1:
-        return None                                        # only get_positional_embedder(frequencies) bands (2^0 .. 2^(f-1))
-    return (3 if getattr(pe, "include_input", True) else 2), nf
-
-
 def sdf_field(nef):
     """-> (SdfDesc, OctreeTensors, keepalive) for a NeuralSDF over an OctreeGrid ('linear'), or (SdfDesc, None, keepalive) for a
     NeuralSDF over a 3D HashGrid of 4 or 8 features per LOD; None when the field is outside what wb_sdf_eval / wb_sdf_train
@@ -583,25 +588,22 @@ def sdf_field(nef):
             return None
         if int(getattr(g, "coord_dim", 3)) != 3 or int(g.feature_dim) not in (4, 8) or g.multiscale_type not in ('cat', 'sum'):
             return None
-    if getattr(g, "interpolation_type", "linear") != "linear" or getattr(dec, "skip", None):
+    if getattr(g, "interpolation_type", "linear") != "linear" or getattr(nef, "activation_type", "relu") != "relu":
         return None
-    if getattr(nef, "activation_type", "relu") != "relu" or getattr(dec, "activation", torch.relu) not in (torch.relu, torch.nn.functional.relu):
-        return None
-    layers = list(dec.layers) + [dec.lout]
-    if not all(isinstance(l, torch.nn.Linear) and l.bias is not None for l in layers):
+    layers = _decoder_layers(dec)
+    if layers is None or any(l.bias is None for l in layers):       # the SDF decoder: bias on every layer, equal widths, one output
         return None
     H, nh = layers[0].out_features, len(layers) - 1
     if not (1 <= nh <= 4 and H <= 128 and layers[-1].out_features == 1 and all(l.out_features == H for l in layers[:-1])):
         return None
     if nh > 1 and H % 4:
         return None
-    em = _sdf_embed_mode(nef)
+    em = _embedder_mode(getattr(nef, "pos_embedder", None))
     if em is None or em[1] > 10 or g.feature_dim > 64:          # wb_make_sdf: pos_freq <= 10, feature_dim <= 64
         return None
     num_lods = int(g.num_lods) if octree else len(g.resolutions)
-    pos_dim = 0 if em[0] == 0 else 3 if em[0] == 1 else 6 * em[1] + (3 if em[0] == 3 else 0)
     in_dim = layers[0].in_features
-    if in_dim != pos_dim + (g.feature_dim if g.multiscale_type == 'sum' else g.feature_dim * num_lods):
+    if in_dim != _embed_width(*em) + (g.feature_dim if g.multiscale_type == 'sum' else g.feature_dim * num_lods):
         return None
     # the decoder input must be at most 132 wide and its shared-memory image must fit in 200 KB: the same limits and formula as
     # wb_make_sdf (csrc/wb_sdf.cuh)
@@ -622,11 +624,7 @@ def sdf_field(nef):
         d.hash = C.pointer(hd)
         return d, None, [hd, table, params]
     dev = g.features[0].device
-    blas = g.blas
-    oct = blas.tensors() if hasattr(blas, "tensors") else None
-    if oct is None:                                        # a reference OctreeAS patched by install()
-        from .install import _octree_tensors
-        oct = _octree_tensors(blas)
+    oct = octree_tensors(g.blas)
     if g.trinkets.device != dev:
         g.trinkets = g.trinkets.to(dev)
     feats = [A.f32c(f.detach()) for f in g.features]
@@ -655,6 +653,15 @@ def sdf_eval(nef, coords: torch.Tensor, lod_idx: Optional[int] = None) -> Option
     with _stage("sdf_eval"):
         A.check(A.lib().wb_sdf_eval(od, C.byref(d), C.c_int32(lod_idx), A.ptr(c), C.c_int64(c.shape[0]), A.ptr(out), A.stream()))
     return out
+
+
+def sdf_channel(nef, coords: torch.Tensor, lod_idx: Optional[int] = None) -> Optional[dict]:
+    """NeuralSDF.sdf's native route: {"sdf": [..., 1]} from sdf_eval for a non-empty CUDA batch outside autograd and autocast (the
+    sphere tracer, the trainer's validation slices); None otherwise or when sdf_eval declines the field (the caller's own body runs)."""
+    if coords.shape[0] == 0 or not coords.is_cuda or torch.is_grad_enabled() or torch.is_autocast_enabled():
+        return None
+    fused = sdf_eval(nef, coords, lod_idx)
+    return None if fused is None else dict(sdf=fused.reshape(*coords.shape[:-1], 1))
 
 
 def _sdf_octree(oct):
@@ -881,18 +888,23 @@ class NefSpec:
                 keep.append(od)
                 d.oct, d.points, d.trinkets = C.addressof(od), oct.points.data_ptr(), trinkets.data_ptr()
                 d.base_lod, d.half_round = self.base_lod, int(self.half_round)
+        if not self.fill_decoders(d, dens_flat.data_ptr(), col_flat.data_ptr()):
+            raise A.WispB200Error("decoder too deep for the fused path")
+        return d, keep
+
+    def fill_decoders(self, d, dens_params: int, col_params: int) -> bool:
+        """The embedding and decoder fields of NefDesc `d`; False (nothing written) when a decoder is deeper than WB_MAX_LAYERS."""
+        if len(self.dens_dims) - 1 > A.WB_MAX_LAYERS or len(self.col_dims) - 1 > A.WB_MAX_LAYERS:
+            return False
         d.pos_mode, d.pos_freq, d.view_mode, d.view_freq = self.pos_mode, self.pos_freq, self.view_mode, self.view_freq
         d.has_bias = int(self.has_bias)
-        d.dens_layers = len(self.dens_dims) - 1
-        d.col_layers = len(self.col_dims) - 1
-        if d.dens_layers > A.WB_MAX_LAYERS or d.col_layers > A.WB_MAX_LAYERS:
-            raise A.WispB200Error("decoder too deep for the fused path")
+        d.dens_layers, d.col_layers = len(self.dens_dims) - 1, len(self.col_dims) - 1
         for i, v in enumerate(self.dens_dims):
             d.dens_dims[i] = v
         for i, v in enumerate(self.col_dims):
             d.col_dims[i] = v
-        d.dens_params, d.col_params = dens_flat.data_ptr(), col_flat.data_ptr()
-        return d, keep
+        d.dens_params, d.col_params = dens_params, col_params
+        return True
 
 
 def triplane_wants_channel_last(spec: "NefSpec") -> bool:
@@ -936,6 +948,11 @@ def _embedder_mode(emb):
     if nf < 1 or int(round(float(getattr(emb, "max_freq_log2", nf - 1)))) != nf - 1 or int(getattr(emb, "out_dim", 0)) not in (6 * nf, 3 + 6 * nf):
         return None
     return (3 if getattr(emb, "include_input", True) else 2), nf
+
+
+def _embed_width(mode: int, freq: int) -> int:
+    """Width of an embedding of _embedder_mode (mode, freq)."""
+    return 0 if mode == 0 else 3 if mode == 1 else 6 * freq + (3 if mode == 3 else 0)
 
 
 def _decoder_layers(dec):
@@ -1025,8 +1042,7 @@ def nef_spec(nef, lod_idx: Optional[int] = None) -> Optional[NefSpec]:
     else:
         return None
     feat = spec.feature_dim if (g.multiscale_type == "sum" or (spec.kind == "octree" and nl == 1)) else nl * spec.feature_dim
-    pos_dim = 0 if pe[0] == 0 else 3 if pe[0] == 1 else 6 * pe[1] + (3 if pe[0] == 3 else 0)
-    if spec.dens_dims[0] != feat + pos_dim:                      # e.g. 'cat' evaluated below its finest LOD: the reference fails in nn.Linear
+    if spec.dens_dims[0] != feat + _embed_width(*pe):                    # e.g. 'cat' evaluated below its finest LOD: the reference fails in nn.Linear
         return None
     return spec
 
@@ -1053,13 +1069,7 @@ def _grid_context(nef, spec: NefSpec):
     dev = g.features[0].device
     if g.trinkets.device != dev:
         g.trinkets = g.trinkets.to(dev)
-    blas = g.blas
-    if hasattr(blas, "tensors"):
-        oct = blas.tensors()
-    else:
-        from .install import _octree_tensors
-        oct = _octree_tensors(blas)
-    return oct, g.trinkets.int().contiguous()
+    return octree_tensors(g.blas), g.trinkets.int().contiguous()
 
 
 class RFTraceFn(torch.autograd.Function):
@@ -1188,18 +1198,20 @@ def precision_supported(spec: NefSpec, nef, precision: int, backward: bool) -> b
         d.num_lods = spec.num_lods if spec.kind != "hash" else len(spec.resolutions)
         d.feature_dim, d.multiscale = spec.feature_dim, (0 if spec.multiscale == "cat" else 1)
         d.lod_idx = spec.lod_idx if spec.kind == "hash" else d.num_lods
-        d.pos_mode, d.pos_freq, d.view_mode, d.view_freq, d.has_bias = spec.pos_mode, spec.pos_freq, spec.view_mode, spec.view_freq, int(spec.has_bias)
-        d.dens_layers, d.col_layers = len(spec.dens_dims) - 1, len(spec.col_dims) - 1
-        if d.dens_layers > A.WB_MAX_LAYERS or d.col_layers > A.WB_MAX_LAYERS:
+        if not spec.fill_decoders(d, dummy.data_ptr(), dummy.data_ptr()):
             return False
-        for i, v in enumerate(spec.dens_dims):
-            d.dens_dims[i] = v
-        for i, v in enumerate(spec.col_dims):
-            d.col_dims[i] = v
-        d.dens_params = d.col_params = dummy.data_ptr()
         ans = bool(A.lib().wb_rf_precision_supported(C.byref(d), C.c_int32(precision), C.c_int32(1 if backward else 0)))
         _SUPPORT_CACHE[key] = ans
     return ans
+
+
+def resolve_precision(precision: Optional[int], spec: NefSpec, nef, backward: bool) -> int:
+    """Decoder arithmetic of a fused trace: 0 = fp32, 1 = fp16 tensor cores with fp32 accumulation.  An explicit precision is taken
+    literally (an unsupported configuration raises); None follows autocast and quietly stays on the fp32 kernels when the decoders
+    do not fit the tensor-core path (both are native CUDA)."""
+    if precision is not None:
+        return int(precision)
+    return 1 if (torch.is_autocast_enabled() and precision_supported(spec, nef, 1, backward)) else 0
 
 
 def rf_trace_nef(ms: MarchState, spec: NefSpec, nef, bg, precision: int = 0):

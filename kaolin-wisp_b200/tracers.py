@@ -1,7 +1,8 @@
-"""PackedRFTracer: host-side mirror of wisp.tracers.PackedRFTracer (wisp/tracers/packed_rf_tracer.py:20-181) and
-wisp.tracers.BaseTracer.forward (wisp/tracers/base_tracer.py:99-162).  trace() runs the fused native pipeline when
-the neural field is a NeuralRadianceField(HashGrid) with the 'ray' sampler, and otherwise the unfused route
-(native raymarch + nef forward + native compositing)."""
+"""PackedRFTracer / PackedSDFTracer: host-side mirrors of wisp.tracers.PackedRFTracer (wisp/tracers/packed_rf_tracer.py:20-181),
+wisp.tracers.PackedSDFTracer (wisp/tracers/packed_sdf_tracer.py:20-174) and wisp.tracers.BaseTracer.forward
+(wisp/tracers/base_tracer.py:99-162).  PackedRFTracer.trace() runs the fused native pipeline when the neural field is a
+NeuralRadianceField(HashGrid) with the 'ray' sampler, and otherwise the unfused route (native raymarch + nef forward + native
+compositing)."""
 from __future__ import annotations
 
 import inspect
@@ -14,7 +15,30 @@ from . import ops
 from .core import RenderBuffer
 
 
-class PackedRFTracer(nn.Module):
+class BaseTracer(nn.Module):
+    def forward(self, nef, rays, channels=None, **kwargs):
+        """base_tracer.py:99-162: channel negotiation, kwargs default to tracer attributes of the same name."""
+        nef_channels = nef.get_supported_channels()
+        unsupported_inputs = self.get_required_nef_channels() - nef_channels
+        if unsupported_inputs:
+            raise Exception(f"The neural field class {type(nef)} does not output the required channels {unsupported_inputs}.")
+        requested = self.get_supported_channels() if channels is None else {channels} if isinstance(channels, str) else set(channels)
+        extra = requested - self.get_supported_channels()
+        unsupported_outputs = extra - nef_channels
+        if unsupported_outputs:
+            raise Exception(f"Channels {unsupported_outputs} are not supported in the tracer {type(self)} or neural field {type(nef)}.")
+        input_args = {}
+        for a in list(inspect.signature(self.trace).parameters)[4:]:
+            if a in kwargs:
+                input_args[a] = kwargs[a]
+            else:
+                d = getattr(self, a, None)
+                if d is not None:
+                    input_args[a] = d
+        return self.trace(nef, rays, requested, extra, **input_args)
+
+
+class PackedRFTracer(BaseTracer):
     def __init__(self, raymarch_type='ray', num_steps=1024, step_size=1.0, bg_color=(1.0, 1.0, 1.0)):
         super().__init__()
         self.raymarch_type, self.num_steps, self.step_size = raymarch_type, num_steps, step_size
@@ -27,16 +51,6 @@ class PackedRFTracer(nn.Module):
         self.jitter = None          # optional explicit [R, num_steps] jitter (parity tests)
         self._pending = {}          # pre-marched batches (premarch), keyed by (origins ptr, dirs ptr, num rays, seed, num_steps)
         self._march_stream = None
-
-    def _resolve_precision(self, spec, nef) -> int:
-        """Explicit precision is taken literally (an unsupported configuration raises); `None` follows autocast and quietly
-        stays on the fp32 kernels when the decoders do not fit the tensor-core path (both are native CUDA)."""
-        if self.precision is not None:
-            return int(self.precision)
-        if not torch.is_autocast_enabled():
-            return 0
-        need_bwd = torch.is_grad_enabled() and any(p.requires_grad for p in nef.parameters())
-        return 1 if ops.precision_supported(spec, nef, 1, need_bwd) else 0
 
     def __getstate__(self):                                  # deepcopy / pickle: streams and in-flight marches are not state
         d = self.__dict__.copy()
@@ -55,7 +69,8 @@ class PackedRFTracer(nn.Module):
             self._march_stream = torch.cuda.Stream(device=dev)
         cur = torch.cuda.current_stream(dev)
         level = ops.raymarch_level(nef.grid, nef.grid.num_lods - 1)
-        blas.tensors().ensure_bits(level)                   # built on the caller's stream BEFORE the side stream starts waiting on it
+        oct = ops.octree_tensors(blas)
+        oct.ensure_bits(level)                              # built on the caller's stream BEFORE the side stream starts waiting on it
         self._march_stream.wait_stream(cur)                 # the rays (and octree masks) are ready on the caller's stream ...
         if ready is not None:
             self._march_stream.wait_event(ready)            # ... or when `ready` fires (e.g. HostPrefetcher.staged_event)
@@ -70,7 +85,7 @@ class PackedRFTracer(nn.Module):
                           torch.empty(R + 1, dtype=torch.int64, device=dev)) for _ in range(4)]
                 del spare
                 self._primed = key
-            pm = ops.march_count(blas.tensors(), rays.origins, rays.dirs, rays.dist_min, rays.dist_max, n, level,
+            pm = ops.march_count(oct, rays.origins, rays.dirs, rays.dist_min, rays.dist_max, n, level,
                                  seed=seed, defer_total=True)
         for t in (rays.origins, rays.dirs):
             t.record_stream(self._march_stream)
@@ -95,27 +110,6 @@ class PackedRFTracer(nn.Module):
     def get_required_nef_channels(self):
         return {"rgb", "density"}
 
-    def forward(self, nef, rays, channels=None, **kwargs):
-        """base_tracer.py:99-162: channel negotiation, kwargs default to tracer attributes of the same name."""
-        nef_channels = nef.get_supported_channels()
-        unsupported_inputs = self.get_required_nef_channels() - nef_channels
-        if unsupported_inputs:
-            raise Exception(f"The neural field class {type(nef)} does not output the required channels {unsupported_inputs}.")
-        requested = self.get_supported_channels() if channels is None else {channels} if isinstance(channels, str) else set(channels)
-        extra = requested - self.get_supported_channels()
-        unsupported_outputs = extra - nef_channels
-        if unsupported_outputs:
-            raise Exception(f"Channels {unsupported_outputs} are not supported in the tracer {type(self)} or neural field {type(nef)}.")
-        input_args = {}
-        for a in list(inspect.signature(self.trace).parameters)[4:]:
-            if a in kwargs:
-                input_args[a] = kwargs[a]
-            else:
-                d = getattr(self, a, None)
-                if d is not None:
-                    input_args[a] = d
-        return self.trace(nef, rays, requested, extra, **input_args)
-
     def trace(self, nef, rays, channels, extra_channels, lod_idx=None, raymarch_type='voxel', num_steps=64, step_size=1.0, bg_color='white'):
         """packed_rf_tracer.py:84-181.  Like the reference, the body reads self.bg_color, not the bg_color argument."""
         assert nef.grid is not None and "this tracer requires a grid"
@@ -130,18 +124,14 @@ class PackedRFTracer(nn.Module):
         if raymarch_type not in ('ray', 'voxel', 'uniform'):
             raise TypeError(f"Raymarch sampler type: {raymarch_type} is not supported by OctreeAS.")       # octree_as.py:427
         if spec is not None and not extra_channels:
-            blas = nef.grid.blas
-            level = ops.raymarch_level(nef.grid, lod_idx)
-            if raymarch_type == 'ray':
-                pm = self._pending.pop(self._march_key(rays, seed, num_steps, blas), None) if (self._pending and jitter is None) else None
-                ms = pm.finalize() if pm is not None else \
-                    ops.march_count(blas.tensors(), rays.origins, rays.dirs, rays.dist_min, rays.dist_max, num_steps, level,
-                                    jitter=jitter, seed=seed)
-            else:
-                ms, _ = ops.march_nuggets(blas.tensors(), rays.origins, rays.dirs, level, num_steps, raymarch_type,
-                                          reference_layout=False, jitter=jitter, seed=seed)
+            pm = None
+            if raymarch_type == 'ray' and self._pending and jitter is None:
+                pm = self._pending.pop(self._march_key(rays, seed, num_steps, nef.grid.blas), None)
+            ms = pm.finalize() if pm is not None else ops.march(nef.grid, lod_idx, rays, raymarch_type, num_steps, jitter=jitter, seed=seed)
             self.prev_num_samples = ms.total
-            rgb, depth, alpha, hit = ops.rf_trace_nef(ms, spec, nef, self.bg_color, precision=self._resolve_precision(spec, nef))
+            # read by resolve_precision only when it follows autocast: the parameter scan runs only then
+            need_bwd = self.precision is None and torch.is_autocast_enabled() and torch.is_grad_enabled() and any(p.requires_grad for p in nef.parameters())
+            rgb, depth, alpha, hit = ops.rf_trace_nef(ms, spec, nef, self.bg_color, precision=ops.resolve_precision(self.precision, spec, nef, need_bwd))
             return RenderBuffer(depth=depth if "depth" in channels else None, hit=hit, rgb=rgb, alpha=alpha)
 
         # ---- unfused route: same operators, nef evaluated through its own forward() ----
@@ -172,7 +162,7 @@ class PackedRFTracer(nn.Module):
         return RenderBuffer(depth=depth if "depth" in channels else None, hit=hit, rgb=rgb, alpha=alpha, **extra_outputs)
 
 
-class PackedSDFTracer(nn.Module):
+class PackedSDFTracer(BaseTracer):
     """wisp.tracers.PackedSDFTracer (packed_sdf_tracer.py:20-174): sphere tracing over the nugget list of OctreeAS.raytrace with
     find_depth_bound jumping between occupied cells; normals by central differences.  The reference's Python loop of masked
     torch ops is one persistent cooperative kernel here (csrc/wb_sdf.cu)."""
@@ -187,33 +177,16 @@ class PackedSDFTracer(nn.Module):
     def get_required_nef_channels(self):
         return {"sdf"}
 
-    def forward(self, nef, rays, channels=None, **kwargs):
-        nef_channels = nef.get_supported_channels()
-        unsupported_inputs = self.get_required_nef_channels() - nef_channels
-        if unsupported_inputs:
-            raise Exception(f"The neural field class {type(nef)} does not output the required channels {unsupported_inputs}.")
-        requested = self.get_supported_channels() if channels is None else {channels} if isinstance(channels, str) else set(channels)
-        extra = requested - self.get_supported_channels()
-        if extra - nef_channels:
-            raise Exception(f"Channels {extra - nef_channels} are not supported in the tracer {type(self)} or neural field {type(nef)}.")
-        args = {}
-        for a in ("lod_idx", "num_steps", "step_size", "min_dis"):
-            if a in kwargs:
-                args[a] = kwargs[a]
-            elif getattr(self, a, None) is not None:
-                args[a] = getattr(self, a)
-        return self.trace(nef, rays, requested, extra, **args)
-
     def trace(self, nef, rays, channels, extra_channels, lod_idx=None, num_steps=64, step_size=1.0, min_dis=1e-4):
         """packed_sdf_tracer.py:57-174.  The nuggets come from the native raytrace; the sphere-tracing loop, the nugget cursor
         and the finite-difference normals are ONE persistent kernel (ops.sdf_trace -> wb_sdf_trace) for NeuralSDF(OctreeGrid);
-        for other fields the per-pack state machine still runs natively and only the field is evaluated through its forward()."""
+        for other fields the per-pack state machine still runs natively and only the field is evaluated through its forward().
+        install() runs this body on the reference's PackedSDFTracer too."""
         assert nef.grid is not None and "this tracer requires a grid"
         if lod_idx is None:
             lod_idx = nef.grid.num_lods - 1
         want_normals = "rgb" in channels or "normal" in channels
-        blas = nef.grid.blas
-        out, st = ops.sdf_trace(nef, blas.tensors(), rays.origins, rays.dirs, rays.dist_max, nef.grid.active_lods[lod_idx], lod_idx,
+        out, st = ops.sdf_trace(nef, ops.octree_tensors(nef.grid.blas), rays.origins, rays.dirs, rays.dist_max, nef.grid.active_lods[lod_idx], lod_idx,
                                 num_steps, step_size, min_dis, want_normals)
         hit = out["hit"]
         self.prev_num_evals = out.get("_evals")                          # device int32 [1] (fused kernel only): field evaluations of the trace

@@ -102,23 +102,9 @@ class MultiviewStep:
         return dist.get_world_size(self.group) if (dist.is_available() and dist.is_initialized()) else 1
 
     def _march(self, rays: Rays, seed: int):
-        nef, tr = self.nef, self.tracer
-        blas = nef.grid.blas
-        level = ops.raymarch_level(nef.grid, len(nef.grid.active_lods) - 1)
-        if tr.raymarch_type == 'ray':
-            pm = tr._pending.pop(tr._march_key(rays, seed, tr.num_steps, blas), None) if tr._pending else None
-            if pm is not None:
-                return pm.finalize()
-            return ops.march_count(blas.tensors(), rays.origins, rays.dirs, rays.dist_min, rays.dist_max, tr.num_steps, level, seed=seed)
-        ms, _ = ops.march_nuggets(blas.tensors(), rays.origins, rays.dirs, level, tr.num_steps, tr.raymarch_type, reference_layout=False, seed=seed)
-        return ms
-
-    def _precision(self) -> int:
-        if self.precision is not None:
-            return int(self.precision)
-        if self.tracer.precision is not None:
-            return int(self.tracer.precision)
-        return 1 if (torch.is_autocast_enabled() and ops.precision_supported(self.spec, self.nef, 1, True)) else 0
+        grid, tr = self.nef.grid, self.tracer
+        pm = tr._pending.pop(tr._march_key(rays, seed, tr.num_steps, grid.blas), None) if (tr.raymarch_type == 'ray' and tr._pending) else None
+        return pm.finalize() if pm is not None else ops.march(grid, len(grid.active_lods) - 1, rays, tr.raymarch_type, tr.num_steps, seed=seed)
 
     # ---- the step ------------------------------------------------------------------------------------------------------
     def step(self, rays: Rays, img_gts: torch.Tensor, seed: Optional[int] = None, next_rays: Optional[Rays] = None, next_seed: Optional[int] = None,
@@ -141,7 +127,7 @@ class MultiviewStep:
         ms = self._march(rays, seed)
         tr.prev_num_samples = ms.total
         S, R = ms.total, ms.rays.num_rays
-        precision = self._precision()
+        precision = ops.resolve_precision(self.precision if self.precision is not None else tr.precision, spec, nef, True)
         gt = [t.data for t in self.grid]
         g_used = self.g_grid
         layout = 1 if ops.triplane_wants_channel_last(spec) else 0

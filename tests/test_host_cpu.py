@@ -224,8 +224,9 @@ def test_install_patches_the_real_wisp_classes():
     """wisp_b200.install.install() against the UNMODIFIED reference classes (imported on CPU through oracle/ref_import.py, in a
     subprocess because the import stubs are process-wide): every patched method keeps its signature, the tracer keeps the
     attributes other wisp code reads and survives copy.deepcopy, ops.nef_spec / ops.sdf_field read the reference's own
-    NeuralRadianceField / NeuralSDF objects, unsupported configurations are declined (-> original method), wide decoders
-    under autocast resolve to the fp32 kernels, and uninstall() restores the originals."""
+    NeuralRadianceField / NeuralSDF objects, unsupported configurations are declined (-> original method), deep decoders
+    under autocast resolve to the fp32 kernels, ops.octree_tensors caches one handle per octree on either OctreeAS, the grid
+    and SDF-tracer patches run the mirror classes' methods, and uninstall() restores the originals."""
     import subprocess
     code = r"""
 import copy, inspect, sys, warnings
@@ -267,6 +268,15 @@ sw = ops.nef_spec(wide, 3)
 assert sw is not None and not sw.has_bias and ops.precision_supported(sw, wide, 1, False) and ops.precision_supported(sw, wide, 1, True)
 deep = NeuralRadianceField(hg, view_embedder='positional', view_multires=4, hidden_dim=128, num_layers=2, bias=True)
 assert ops.precision_supported(ops.nef_spec(deep, 3), deep, 1, False) and not ops.precision_supported(ops.nef_spec(deep, 3), deep, 1, True)
+# the precision rule of both tracers and MultiviewStep: an explicit precision is literal, None follows autocast where supported
+sd = ops.nef_spec(deep, 3)
+assert [ops.resolve_precision(None, s, n, True) for s, n in ((spec, nef), (sw, wide), (sd, deep))] == [0, 0, 0]
+torch.set_autocast_enabled("cuda", True)
+try:
+    assert [ops.resolve_precision(None, s, n, b) for s, n, b in ((spec, nef, True), (sw, wide, True), (sd, deep, True), (sd, deep, False))] == [1, 1, 0, 1]
+    assert ops.resolve_precision(0, spec, nef, True) == 0 and ops.resolve_precision(1, sd, deep, True) == 1
+finally:
+    torch.set_autocast_enabled("cuda", False)
 ident = NeuralRadianceField(hg, view_embedder='none', pos_embedder='positional', pos_multires=3, position_input=True, hidden_dim=32)
 si = ops.nef_spec(ident, 3)
 assert si.view_mode == 1 and si.pos_mode == 3 and si.pos_freq == 3 and si.dens_dims[0] == 8 + 3 + 18
@@ -283,8 +293,51 @@ sdf = NeuralSDF(OctreeGrid(blas, feature_dim=16, num_lods=2, multiscale_type='su
 fd = ops.sdf_field(sdf)
 assert fd is not None and fd[0].hidden_dim == 128 and fd[0].feature_dim == 16 and fd[0].pos_mode == 1 and fd[0].multiscale == 1
 assert ops.sdf_field(NeuralSDF(hg, pos_embedder='none', position_input=True, hidden_dim=32)) is None       # SDF over a hash grid: phase-by-phase route
+# one octree handle for the reference's and the mirror's OctreeAS: cached on the BLAS, rebuilt when the octree tensor is replaced
+mb = W.OctreeAS(torch.from_numpy(O.dense_octree(3)))
+for b in (blas, mb):
+    t = ops.octree_tensors(b)
+    assert ops.octree_tensors(b) is t and t.prefix.dtype == t.pyramid.dtype == torch.int32
+    b.octree = b.octree.clone()
+    t2 = ops.octree_tensors(b)
+    assert t2 is not t and ops.octree_tensors(b) is t2
+assert mb.tensors() is t2
+mb.to("cpu")
+assert mb.tensors() is not t2
+# the grid and SDF-tracer patches run the mirror classes' methods; the triplanar fall-back (non-'reflection' padding) stays
+from wisp.core import Rays, RenderBuffer
+x = torch.zeros(4, 3)
+rb = W.RenderBuffer(rgb=x, alpha=x[:, :1], depth=x[:, :1], hit=x[:, 0] > 0, xyz=x, normal=x)
+calls = []
+def recorder(name, result):
+    def fn(self, *a):
+        calls.append((name, self, a))
+        return result
+    return fn
+mirror = (W.grids.TriplanarGrid.interpolate, W.grids.OctreeGrid.interpolate, W.tracers.PackedSDFTracer.trace)
+W.grids.TriplanarGrid.interpolate, W.grids.OctreeGrid.interpolate = recorder("tri", x), recorder("oct", x)
+W.tracers.PackedSDFTracer.trace = recorder("sdf", rb)
+try:
+    st_ = PackedSDFTracer()
+    assert tg.interpolate(x, 1) is x and og.interpolate(x, 1) is x
+    out = st_.trace(sdf, Rays(origins=x, dirs=x), {"rgb"}, set(), 1, 8, 0.5, 1e-3)
+    tg.features[1].padding_mode = 'zeros'
+    assert tg.interpolate(x, 1) is not x and len(calls) == 3
+    tg.features[1].padding_mode = 'reflection'
+finally:
+    W.grids.TriplanarGrid.interpolate, W.grids.OctreeGrid.interpolate, W.tracers.PackedSDFTracer.trace = mirror
+assert [c[0] for c in calls] == ["tri", "oct", "sdf"] and calls[0][1] is tg and calls[1][1] is og and calls[2][1] is st_
+assert all(c[2][0] is x and c[2][1] == 1 for c in calls[:2])
+assert calls[2][2][0] is sdf and calls[2][2][2] == {"rgb"} and calls[2][2][3:] == (set(), 1, 8, 0.5, 1e-3)
+assert isinstance(out, RenderBuffer) and all(getattr(out, c) is getattr(rb, c) for c in ("rgb", "alpha", "depth", "hit", "xyz", "normal"))
+# the real mirror bodies on the reference grids (no `half_features` on its OctreeGrid) get as far as the device check
+for g in (tg, og):
+    try:
+        g.interpolate(x, 1)
+        raise SystemExit("interpolate on CPU tensors must raise")
+    except W.WispB200Error:
+        pass
 # no CPU fallback behind the patches either
-from wisp.core import Rays
 try:
     blas.query(torch.zeros(4, 3))
     raise SystemExit("query on CPU tensors must raise")
