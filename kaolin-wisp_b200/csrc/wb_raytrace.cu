@@ -21,7 +21,7 @@ __device__ __forceinline__ bool wb_slab(const float o[3], const float d[3], int 
         if (d[a] != 0.0f) {
             const float ta = __fdiv_rn(__fsub_rn(lo, o[a]), d[a]), tb = __fdiv_rn(__fsub_rn(hi, o[a]), d[a]);
             te = fmaxf(te, fminf(ta, tb)); tx = fminf(tx, fmaxf(ta, tb));
-        } else if (o[a] < lo || o[a] > hi) return false;
+        } else if (o[a] < lo || o[a] >= hi) return false;     // parallel axis: the cell's points, [lo, hi) as in wb_quantize
     }
     const float en = fmaxf(te, 0.0f);
     if (!(tx > en)) return false;

@@ -127,7 +127,7 @@ def test_raytrace_against_brute_force():
         with np.errstate(divide="ignore", invalid="ignore"):
             ta, tb = (lo - o[r]) / d[r], (hi - o[r]) / d[r]
             te = np.where(d[r] != 0, np.minimum(ta, tb), -np.inf).max(1); tx = np.where(d[r] != 0, np.maximum(ta, tb), np.inf).min(1)
-        inside_zero = np.all((d[r] != 0) | ((o[r] >= lo) & (o[r] <= hi)), axis=1)
+        inside_zero = np.all((d[r] != 0) | ((o[r] >= lo) & (o[r] < hi)), axis=1)
         hit = (tx > np.maximum(te, 0)) & inside_zero
         mine = rt["pidx"][rt["ridx"] == r] - spc.pyramid[1, 4]
         assert set(mine.tolist()) == set(np.nonzero(hit)[0].tolist()), r
