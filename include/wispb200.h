@@ -416,6 +416,15 @@ int wb_codebook_rows_bwd(const float* logits, const float* dictionary, const flo
  *       reference's parameter groups; grad_scale multiplies every gradient first (1/world after an all-reduce(sum)); zero_grad != 0
  *       clears each gradient as it is consumed.  The step's description (segments, bias corrections, scales) is passed to the
  *       kernel by value, so segs may be reused as soon as the call returns, however far the host runs ahead of the stream.
+ *   wb_adamw_step : torch.optim.AdamW (amsgrad off; what apex FusedAdam computes by default) with wb_adam_step's contract and
+ *       segments: p *= 1 - lr * weight_decay (the factor formed in double, one fp32 multiply), then Adam's moments and update
+ *       without the L2 term.
+ *   wb_rmsprop_step : torch.optim.RMSprop (centered off) with wb_adam_step's contract: g = grad * grad_scale (+ weight_decay * p);
+ *       square_avg = alpha * square_avg + (1 - alpha) g^2; q = g / (sqrt(square_avg) + eps); momentum == 0: p -= lr * q, and
+ *       momentum_buffer is neither read nor written (it may be null); momentum > 0: buf = momentum * buf + q, p -= lr * buf.
+ *   Roundings of the two (ours, not torch's, which runs one kernel per operation): every product, quotient and square root is
+ *   rounded once; the moment updates and the final parameter update are single fused multiply-adds (b * state + fl(..),
+ *   p - lr * q); wb_optim.cu lists the chains.  fp32 parameters and state.
  * ---------------------------------------------------------------------------------------------- */
 int wb_composite_bwd_loss(const float* shaded, const float* depth, const float* deltas, const int64_t* offsets, int64_t R,
                           const float* bg, const float* rgb_pred, const float* target, int32_t loss_type, float inv_count,
@@ -427,6 +436,15 @@ typedef struct wb_adam_segment {
 } wb_adam_segment;
 int wb_adam_step(const wb_adam_segment* segs, int32_t nseg, float beta1, float beta2, float eps, int32_t step, float grad_scale,
                  int32_t zero_grad, wb_stream s);
+int wb_adamw_step(const wb_adam_segment* segs, int32_t nseg, float beta1, float beta2, float eps, int32_t step, float grad_scale,
+                  int32_t zero_grad, wb_stream s);
+typedef struct wb_rmsprop_segment {
+    float* param; float* grad; float* square_avg; float* momentum_buffer;      /* momentum_buffer: null when momentum == 0 */
+    int64_t numel;
+    float lr, weight_decay;
+} wb_rmsprop_segment;
+int wb_rmsprop_step(const wb_rmsprop_segment* segs, int32_t nseg, float alpha, float eps, float momentum, float grad_scale,
+                    int32_t zero_grad, wb_stream s);
 
 /* ------------------------------------------------------------------------------------------------
  * Ray generation (camera -> rays on the device); origin/view/right/up/cam_pos/rotation are HOST pointers (launch parameters).

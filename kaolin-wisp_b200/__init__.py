@@ -13,6 +13,6 @@ from .nefs import NeuralRadianceField, NeuralSDF, BasicDecoder, PositionalEmbedd
 from .tracers import PackedRFTracer, PackedSDFTracer                                             # noqa: F401
 from .pipeline import Pipeline                                                  # noqa: F401
 from . import trainers                                                          # noqa: F401
-from .trainers import MultiviewStep, NativeAdam, SDFStep                        # noqa: F401
+from .trainers import MultiviewStep, NativeAdam, NativeAdamW, NativeRMSprop, SDFStep   # noqa: F401
 
 __version__ = "0.1.0"

@@ -74,6 +74,12 @@ class AdamSegment(C.Structure):
                 ("lr", C.c_float), ("weight_decay", C.c_float)]
 
 
+class RMSpropSegment(C.Structure):
+    """struct wb_rmsprop_segment."""
+    _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("square_avg", C.c_void_p), ("momentum_buffer", C.c_void_p), ("numel", C.c_int64),
+                ("lr", C.c_float), ("weight_decay", C.c_float)]
+
+
 EXPORTS = [
     "wb_last_error", "wb_version", "wb_device_check", "wb_launch_count",
     "wb_octree_generate_points", "wb_octree_build_bits", "wb_octree_build_coarse", "wb_query",
@@ -82,7 +88,7 @@ EXPORTS = [
     "wb_hashgrid_fwd", "wb_hashgrid_bwd", "wb_triplane_fwd", "wb_triplane_bwd", "wb_triplane_relayout",
     "wb_octree_interp_fwd", "wb_octree_interp_bwd", "wb_find_depth_bound", "wb_sdf_eval", "wb_sdf_train", "wb_sdf_train_smem_bytes", "wb_sdf_train_tc", "wb_sdf_train_tc_smem_bytes", "wb_sdf_trace", "wb_sdf_phase", "wb_composite_fwd", "wb_composite_bwd",
     "wb_rf_march_fill", "wb_rf_param_blob_floats", "wb_rf_precision_supported", "wb_rf_pack_params", "wb_rf_shade_fwd", "wb_rf_shade_bwd",
-    "wb_rf_workspace_bytes", "wb_rf_feat_bytes", "wb_rf_decoder_bwd", "wb_rf_table_scatter", "wb_rf_loss_scale", "wb_rf_workspace_holds_ray_rows", "wb_prune_samples", "wb_prune_update", "wb_raygen_lookat", "wb_raygen_pinhole", "wb_codebook_rows_fwd", "wb_codebook_rows_bwd", "wb_composite_bwd_loss", "wb_adam_step", "wb_tc_selftest",
+    "wb_rf_workspace_bytes", "wb_rf_feat_bytes", "wb_rf_decoder_bwd", "wb_rf_table_scatter", "wb_rf_loss_scale", "wb_rf_workspace_holds_ray_rows", "wb_prune_samples", "wb_prune_update", "wb_raygen_lookat", "wb_raygen_pinhole", "wb_codebook_rows_fwd", "wb_codebook_rows_bwd", "wb_composite_bwd_loss", "wb_adam_step", "wb_adamw_step", "wb_rmsprop_step", "wb_tc_selftest",
 ]
 
 _lib: Optional[C.CDLL] = None

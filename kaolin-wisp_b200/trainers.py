@@ -6,7 +6,8 @@ optimiser set-up of BaseTrainer.init_optimizer (wisp/trainers/base_trainer.py:20
     composite backward WITH the image loss and its gradient inside (wb_composite_bwd_loss)       [torch: 6 launches + a [R,3] tensor]
     device loss scale -> decoder backward -> grid scatter, into persistent gradient buffers
     [N > 1: NCCL all-reduce(sum) of the gradient buffers; the 1/world is folded into the optimiser]
-    Adam over grid + decoders in one launch that also clears the gradients (wb_adam_step)          [torch: zero_grad + fused Adam]
+    Adam / AdamW / RMSprop over grid + decoders in one launch that also clears the gradients        [torch: zero_grad + fused Adam]
+    (wb_adam_step / wb_adamw_step / wb_rmsprop_step), at the learning rate MultiStepLR would have reached
 
 What the reference does around it and this keeps: parameter groups by name ('decoder' -> weight decay, 'grid' -> lr * grid_lr_weight),
 rgb_loss_type l2 / l1 / huber, rgb_loss_denom rays / samples, tracer.prev_num_samples for the adaptive ray budget.  What it drops:
@@ -29,25 +30,87 @@ from .core import Rays
 LOSS_TYPES = {"l2": 0, "l1": 1, "huber": 2}
 
 
+def _fill_segments(segs, entries, grads, lr_scale, **state):
+    """Fill the C segment array of one step; state: the two state fields of the segment struct by name, each a list of tensors or
+    None.  lr_scale multiplies every learning rate in double before the fp32 conversion (1.0: the rate as constructed)."""
+    if entries:
+        A.require_device(entries[0][0])                                       # no CPU fallback
+    for k, ((p, lr, wd), g) in enumerate(zip(entries, grads)):
+        assert g.is_contiguous() and p.is_contiguous() and g.numel() == p.numel() and p.dtype == torch.float32 and g.dtype == torch.float32
+        sg = segs[k]
+        sg.param, sg.grad, sg.numel, sg.lr, sg.weight_decay = p.data_ptr(), g.data_ptr(), p.numel(), lr * lr_scale, wd
+        for name, tensors in state.items():
+            setattr(sg, name, tensors[k].data_ptr() if tensors is not None else None)
+
+
 class NativeAdam:
-    """torch.optim.Adam (amsgrad off) over a list of (tensor, lr, weight_decay) in one launch; see wb_adam_step."""
+    """torch.optim.Adam (amsgrad off) over a list of (tensor, lr, weight_decay) in one launch; see wb_adam_step.
+    `lr_scale` (an attribute, 1.0 unless set) multiplies every entry's learning rate in the steps that follow: a schedule's factor."""
+    _entry = "wb_adam_step"
 
     def __init__(self, entries, betas=(0.9, 0.999), eps=1e-8):
         self.entries = [(p, float(lr), float(wd)) for p, lr, wd in entries]
-        self.betas, self.eps, self.t = betas, float(eps), 0
+        self.betas, self.eps, self.t, self.lr_scale = betas, float(eps), 0, 1.0
         self.exp_avg = [torch.zeros_like(p, dtype=torch.float32) for p, _, _ in self.entries]
         self.exp_avg_sq = [torch.zeros_like(p, dtype=torch.float32) for p, _, _ in self.entries]
 
     def step(self, grads, grad_scale: float = 1.0, zero_grad: bool = True):
-        self.t += 1
         n = len(self.entries)
         segs = (A.AdamSegment * n)()
-        for k, ((p, lr, wd), g) in enumerate(zip(self.entries, grads)):
-            assert g.is_contiguous() and p.is_contiguous() and g.numel() == p.numel() and p.dtype == torch.float32 and g.dtype == torch.float32
-            segs[k].param, segs[k].grad, segs[k].exp_avg, segs[k].exp_avg_sq = p.data_ptr(), g.data_ptr(), self.exp_avg[k].data_ptr(), self.exp_avg_sq[k].data_ptr()
-            segs[k].numel, segs[k].lr, segs[k].weight_decay = p.numel(), lr, wd
-        A.check(A.lib().wb_adam_step(segs, C.c_int32(n), C.c_float(self.betas[0]), C.c_float(self.betas[1]), C.c_float(self.eps), C.c_int32(self.t),
-                                     C.c_float(grad_scale), C.c_int32(int(zero_grad)), A.stream()))
+        _fill_segments(segs, self.entries, grads, self.lr_scale, exp_avg=self.exp_avg, exp_avg_sq=self.exp_avg_sq)
+        self.t += 1
+        A.check(getattr(A.lib(), self._entry)(segs, C.c_int32(n), C.c_float(self.betas[0]), C.c_float(self.betas[1]), C.c_float(self.eps), C.c_int32(self.t),
+                                              C.c_float(grad_scale), C.c_int32(int(zero_grad)), A.stream()))
+
+
+class NativeAdamW(NativeAdam):
+    """torch.optim.AdamW (amsgrad off; apex FusedAdam's default adam_w_mode) with NativeAdam's interface: the entries' weight decay
+    is decoupled, p *= 1 - lr * weight_decay before the Adam update; see wb_adamw_step."""
+    _entry = "wb_adamw_step"
+
+
+class NativeRMSprop:
+    """torch.optim.RMSprop (centered off) over a list of (tensor, lr, weight_decay) in one launch, with NativeAdam's step and
+    lr_scale; see wb_rmsprop_step.  momentum_buffer is None when momentum == 0."""
+
+    def __init__(self, entries, alpha=0.99, eps=1e-8, momentum=0.0):
+        self.entries = [(p, float(lr), float(wd)) for p, lr, wd in entries]
+        self.alpha, self.eps, self.momentum, self.t, self.lr_scale = float(alpha), float(eps), float(momentum), 0, 1.0
+        if self.momentum < 0.0:
+            raise ValueError(f"NativeRMSprop: momentum must be >= 0, got {momentum!r}")
+        self.square_avg = [torch.zeros_like(p, dtype=torch.float32) for p, _, _ in self.entries]
+        self.momentum_buffer = [torch.zeros_like(p, dtype=torch.float32) for p, _, _ in self.entries] if self.momentum > 0.0 else None
+
+    def step(self, grads, grad_scale: float = 1.0, zero_grad: bool = True):
+        n = len(self.entries)
+        segs = (A.RMSpropSegment * n)()
+        _fill_segments(segs, self.entries, grads, self.lr_scale, square_avg=self.square_avg, momentum_buffer=self.momentum_buffer)
+        self.t += 1
+        A.check(A.lib().wb_rmsprop_step(segs, C.c_int32(n), C.c_float(self.alpha), C.c_float(self.eps), C.c_float(self.momentum),
+                                        C.c_float(grad_scale), C.c_int32(int(zero_grad)), A.stream()))
+
+
+OPTIMIZERS = ("adam", "adamw", "rmsprop")
+
+
+def _make_optimizer(optimizer, tensors, betas, eps, alpha, momentum):
+    """The native optimiser MultiviewStep / SDFStep step with: cfg.optimizer.constructor 'Adam' | 'AdamW' (and apex 'FusedAdam')
+    | 'RMSprop' of the reference's configs (wisp/config/presets/torch.py:37-67) as "adam" | "adamw" | "rmsprop"."""
+    if optimizer not in OPTIMIZERS:
+        raise ValueError(f"optimizer must be one of {OPTIMIZERS}, got {optimizer!r}")
+    if optimizer == "rmsprop":
+        return NativeRMSprop(tensors, alpha=alpha, eps=eps, momentum=momentum)
+    return (NativeAdamW if optimizer == "adamw" else NativeAdam)(tensors, betas=betas, eps=eps)
+
+
+def multistep_factor(milestones, gamma: float, t: int) -> float:
+    """Learning-rate factor of optimiser step t (1-based) under torch.optim.lr_scheduler.MultiStepLR stepped once after every
+    optimiser step: gamma^k, k = the number of milestones <= t - 1 counted with multiplicity, multiplied up in double."""
+    f = 1.0
+    for m in milestones:
+        if m <= t - 1:
+            f *= gamma
+    return f
 
 
 def _flatten_in_place(module_params):
@@ -64,7 +127,18 @@ def _flatten_in_place(module_params):
 
 class MultiviewStep:
     def __init__(self, pipeline, lr: float = 1e-3, eps: float = 1e-15, weight_decay: float = 0.0, grid_lr_weight: float = 1.0, betas=(0.9, 0.999),
-                 rgb_loss_type: str = "huber", rgb_loss_denom: str = "rays", precision: Optional[int] = None, group=None):
+                 rgb_loss_type: str = "huber", rgb_loss_denom: str = "rays", precision: Optional[int] = None, group=None,
+                 optimizer: str = "adam", alpha: float = 0.99, momentum: float = 0.0, scheduler_milestones=(), scheduler_gamma: float = 0.333):
+        """`optimizer`: "adam" | "adamw" | "rmsprop", the rule cfg.optimizer.constructor names (apex FusedAdam: "adamw"); `betas`
+        belong to the first two, `alpha` and `momentum` to RMSprop.  The parameter groups are the same under every rule.
+
+        `scheduler_milestones` / `scheduler_gamma`: the MultiStepLR the reference steps after every optimiser step
+        (multiview_trainer.py:179-180).  The milestones are ITERATION NUMBERS (ints): optimiser step t (1-based) runs at
+        lr * gamma^k, k = the number of milestones <= t - 1, a repeated milestone counted each time.  step(update=False) does
+        not advance the schedule.  The reference's own milestones are not these numbers: init_optimizer hands MultiStepLR the
+        floats max_steps * x (max_steps = len(train_dataset) * max_epochs, x in cfg.scheduler_milestones; base_trainer.py:237-246),
+        and MultiStepLR.step tests `last_epoch in milestones`, so a milestone fires only when that product is integer-valued
+        (8 steps with (0.5, 0.75, 0.9): 4.0 and 6.0 fire, 7.2 never does).  Pass the iterations that do fire.  Empty: no schedule."""
         if rgb_loss_type not in LOSS_TYPES or rgb_loss_denom not in ("rays", "samples"):
             raise NotImplementedError                                                        # multiview_trainer.py:147,157
         self.pipeline, self.nef, self.tracer = pipeline, pipeline.nef, pipeline.tracer
@@ -89,7 +163,10 @@ class MultiviewStep:
             tensors = [(p.data, lr * grid_lr_weight if ("grid" in n and "decoder" not in n) else lr, weight_decay if "decoder" in n else 0.0)
                        for n, p in named if p.requires_grad]
             self.params = [p for _, p in named if p.requires_grad]
-        self.opt = NativeAdam(tensors, betas=betas, eps=eps)
+        self.opt = _make_optimizer(optimizer, tensors, betas, eps, alpha, momentum)
+        self.milestones, self.gamma = [int(m) for m in scheduler_milestones], float(scheduler_gamma)
+        if any(m != f for m, f in zip(self.milestones, scheduler_milestones)):
+            raise ValueError(f"scheduler_milestones are iteration numbers (ints), got {scheduler_milestones!r}")
         dev = tensors[0][0].device
         self._scalars = torch.zeros(2, dtype=torch.float32, device=dev)       # loss accumulator | max |g_shaded|: cleared by ONE fill per step
         self.loss_buf, self.absmax = self._scalars[0:1], self._scalars[1:2]
@@ -185,6 +262,7 @@ class MultiviewStep:
             with ops._stage("all_reduce"):
                 self._all_reduce(loss)
         if update:
+            self.opt.lr_scale = multistep_factor(self.milestones, self.gamma, self.opt.t + 1)
             with ops._stage("adam"):
                 self.opt.step(self.g_grid + [self.g_dens, self.g_col] + self.g_rest, grad_scale=1.0, zero_grad=zero_grad)
             if layout and zero_grad:
@@ -226,6 +304,7 @@ class MultiviewStep:
         if world > 1:
             for g in grads:
                 dist.all_reduce(g, op=dist.ReduceOp.SUM, group=self.group)
+        self.opt.lr_scale = multistep_factor(self.milestones, self.gamma, self.opt.t + 1)
         self.opt.step(grads, grad_scale=1.0 / world, zero_grad=False)
         return loss.detach()
 
@@ -255,10 +334,13 @@ class SDFStep:
          the hash table stays fp32 (the reference casts it to fp16).  Every other field, octree fields included (the kernel
          trains them through ops.sdf_train, but measured slower than autocast autograd at large batches), takes autograd inside
          torch.autocast("cuda", torch.float16) plus NativeAdam.
+    `optimizer`: "adam" | "adamw" | "rmsprop" replaces NativeAdam by NativeAdamW or NativeRMSprop(alpha, momentum) on either route,
+    with the same parameter groups.  No learning-rate schedule: SDFTrainer.step never steps one.
     `fused` tells which route was chosen."""
 
     def __init__(self, pipeline, lr: float = 1e-3, eps: float = 1e-15, weight_decay: float = 0.0, grid_lr_weight: float = 1.0,
-                 betas=(0.9, 0.999), only_last: bool = True, precision: int = 0):
+                 betas=(0.9, 0.999), only_last: bool = True, precision: int = 0, optimizer: str = "adam", alpha: float = 0.99,
+                 momentum: float = 0.0):
         if precision not in (0, 1) or isinstance(precision, bool):
             raise ValueError(f"SDFStep: precision must be 0 (fp32) or 1 (fp16 autocast arithmetic), got {precision!r}")
         self.precision = int(precision)
@@ -282,7 +364,7 @@ class SDFStep:
             tensors = [(p.data, lr if "decoder" in k or "grid" not in k else lr * grid_lr_weight, weight_decay if "decoder" in k else 0.0)
                        for k, p in named]
             self.params = [p for _, p in named]
-        self.opt = NativeAdam(tensors, betas=betas, eps=eps)
+        self.opt = _make_optimizer(optimizer, tensors, betas, eps, alpha, momentum)
         self.loss_buf = torch.zeros(1, dtype=torch.float32, device=self.device)
 
     @staticmethod

@@ -50,6 +50,27 @@ def _params(nef):
     return {k: p.detach().numpy().copy() for k, p in nef.named_parameters() if p.requires_grad}
 
 
+def init_decoder(nef):
+    """sdf ~ (|x|+|y|+|z|)/sqrt(3) - 0.3 + small learned perturbation (as gen_sdf)."""
+    with torch.no_grad():
+        W0 = nef.decoder.layers[0].weight; W0.mul_(0.05)
+        W0[:6, :3] = torch.tensor([[1, 0, 0], [-1, 0, 0], [0, 1, 0], [0, -1, 0], [0, 0, 1], [0, 0, -1.0]])
+        nef.decoder.layers[0].bias.uniform_(-0.05, 0.05)
+        for l in list(nef.decoder.layers)[1:]:
+            l.weight.mul_(0.05); l.weight[:6, :] = 0.0; l.weight[:6, :6] = torch.eye(6)
+            l.bias.uniform_(-0.05, 0.05); l.bias[:6] = 0.0
+        nef.decoder.lout.weight.mul_(0.05); nef.decoder.lout.weight[0, :6] = 1.0 / np.sqrt(3.0)
+        nef.decoder.lout.bias.fill_(-0.25)
+
+
+def batch():
+    """The training batch of every case: N points around the octahedron with its noisy distance."""
+    rng = np.random.default_rng(17)
+    coords = rng.uniform(-0.7, 0.7, (N, 3)).astype(np.float32)
+    sdf = ((np.abs(coords).sum(-1, keepdims=True) - 0.3) / np.sqrt(3.0) + rng.normal(0.0, 0.01, (N, 1))).astype(np.float32)
+    return coords, sdf
+
+
 def main():
     from oracle import oracle as O
     from oracle import ref_import
@@ -71,9 +92,7 @@ def main():
     bt.instantiate = lambda cfg, params: torch.optim.Adam(params, lr=cfg.lr, betas=cfg.betas, eps=cfg.eps)
     level = 5
     oct_np = O.points_to_octree(octahedron_points(level), level)
-    rng = np.random.default_rng(17)
-    coords = rng.uniform(-0.7, 0.7, (N, 3)).astype(np.float32)
-    sdf = ((np.abs(coords).sum(-1, keepdims=True) - 0.3) / np.sqrt(3.0) + rng.normal(0.0, 0.01, (N, 1))).astype(np.float32)
+    coords, sdf = batch()
     out = dict(octree=oct_np, level=level, coords=coords, sdf=sdf, lr=LR, eps=EPS, weight_decay=WD, grid_lr_weight=GRID_LR_WEIGHT)
     cases = HASH_CASES if hashed else {k: v + (8,) for k, v in (DEEP_CASES if deep else CASES).items()}
     for name, (ms, only_last, layers, F) in cases.items():
@@ -86,15 +105,7 @@ def main():
             grid = OctreeGrid(blas, feature_dim=8, num_lods=3, interpolation_type='linear', multiscale_type=ms, feature_std=0.05)
         nl = grid.num_lods
         nef = NeuralSDF(grid, pos_embedder='none', position_input=True, hidden_dim=16, num_layers=layers)
-        with torch.no_grad():       # sdf ~ (|x|+|y|+|z|)/sqrt(3) - 0.3 + small learned perturbation (as gen_sdf)
-            W0 = nef.decoder.layers[0].weight; W0.mul_(0.05)
-            W0[:6, :3] = torch.tensor([[1, 0, 0], [-1, 0, 0], [0, 1, 0], [0, -1, 0], [0, 0, 1], [0, 0, -1.0]])
-            nef.decoder.layers[0].bias.uniform_(-0.05, 0.05)
-            for l in list(nef.decoder.layers)[1:]:
-                l.weight.mul_(0.05); l.weight[:6, :] = 0.0; l.weight[:6, :6] = torch.eye(6)
-                l.bias.uniform_(-0.05, 0.05); l.bias[:6] = 0.0
-            nef.decoder.lout.weight.mul_(0.05); nef.decoder.lout.weight[0, :6] = 1.0 / np.sqrt(3.0)
-            nef.decoder.lout.bias.fill_(-0.25)
+        init_decoder(nef)
         t = object.__new__(st.SDFTrainer)
         t.pipeline = Pipeline(nef=nef, tracer=None)
         t.device = 'cpu'
