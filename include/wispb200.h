@@ -300,7 +300,7 @@ typedef struct wb_sdf_state {
 } wb_sdf_state;
 int wb_sdf_trace(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, const wb_rays* rays,
                  const float* nug_depth, int64_t Ng, const int64_t* ray_offsets,
-                 int32_t num_steps, float step_size, float min_dis, int32_t want_normals, const wb_sdf_state* state,
+                 int32_t num_steps, float step_size, double min_dis, int32_t want_normals, const wb_sdf_state* state,
                  float* xyz, float* depth, uint8_t* hit, float* normal, float* rgb, float* alpha, wb_stream s);
 /* wb_sdf_trace takes octree fields only: a hash description returns WB_ERR_INVALID before anything is launched.
  * The same state machine one phase per launch, for fields wb_sdf_trace does not trace (NeuralSDF over a hash grid,
@@ -309,7 +309,7 @@ int wb_sdf_trace(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, 
  * iteration `iteration` (packed_sdf_tracer.py:120-131)   3: step 2 (:133-141)   4: outputs of the packs that hit.
  * iterflags[2*iteration + (phase == 3)] != 0 afterwards iff a pack is still alive (the loop's `break` tests). */
 int wb_sdf_phase(int32_t phase, const wb_rays* rays, const float* nug_depth, int64_t Ng, const int64_t* ray_offsets,
-                 int32_t num_steps, int32_t iteration, float min_dis, const wb_sdf_state* state,
+                 int32_t num_steps, int32_t iteration, double min_dis, const wb_sdf_state* state,
                  float* xyz, float* depth, uint8_t* hit, float* alpha, wb_stream s);
 
 /* ------------------------------------------------------------------------------------------------

@@ -385,7 +385,7 @@ extern "C" int wb_sdf_eval(const wb_octree* oct, const wb_sdf_desc* nef, int32_t
 }
 
 static int sdf_make_trace(const wb_rays* rays, const float* nug_depth, int64_t Ng, const int64_t* ray_offsets, int32_t num_steps, float step_size,
-                          float min_dis, const wb_sdf_state* st, WbSdfTrace* T)
+                          double min_dis, const wb_sdf_state* st, WbSdfTrace* T)
 {
     WB_CHECK_ARG(rays != nullptr && rays->origins && rays->dirs && nug_depth && ray_offsets, "null pointer");
     WB_CHECK_ARG(rays->near_v == nullptr, "the SDF tracer compares t with a scalar dist_max (packed_sdf_tracer.py:127)");
@@ -397,7 +397,9 @@ static int sdf_make_trace(const wb_rays* rays, const float* nug_depth, int64_t N
     T->origins = rays->origins; T->dirs = rays->dirs; T->R = rays->num_rays; T->dist_max = rays->dist_max;
     T->nug_depth = reinterpret_cast<const float2*>(nug_depth); T->Ng = Ng; T->ray_offsets = ray_offsets; T->S = *st;
     T->num_steps = num_steps; T->step_size = step_size;
-    T->min_dis = (float)((double)min_dis * 1.0); T->min_dis5 = (float)(((double)min_dis * 5.0) * 1.0);     // min_dis * invres, (min_dis*5) * invres (:123-126)
+    // min_dis * invres, (min_dis*5) * invres (:123-126): Python doubles, each rounded once to fp32 where torch compares them with
+    // the fp32 distances (min_dis arrives as a double: fp32(fp32(1e-3) * 5) is one ulp above fp32(1e-3 * 5))
+    T->min_dis = (float)(min_dis * 1.0); T->min_dis5 = (float)((min_dis * 5.0) * 1.0);
     return WB_OK;
 }
 // rays with nuggets -> exclusive scan (pack_off); iteration flags cleared
@@ -411,7 +413,7 @@ static int sdf_scan_packs(const WbSdfTrace& T, int32_t num_steps, cudaStream_t s
 
 extern "C" int wb_sdf_trace(const wb_octree* oct, const wb_sdf_desc* nef, int32_t lod_idx, const wb_rays* rays,
                             const float* nug_depth, int64_t Ng, const int64_t* ray_offsets,
-                            int32_t num_steps, float step_size, float min_dis, int32_t want_normals, const wb_sdf_state* state,
+                            int32_t num_steps, float step_size, double min_dis, int32_t want_normals, const wb_sdf_state* state,
                             float* xyz, float* depth, uint8_t* hit, float* normal, float* rgb, float* alpha, wb_stream s)
 {
     WB_CHECK_ARG(rays != nullptr, "null rays");
@@ -442,7 +444,7 @@ extern "C" int wb_sdf_trace(const wb_octree* oct, const wb_sdf_desc* nef, int32_
 }
 
 extern "C" int wb_sdf_phase(int32_t phase, const wb_rays* rays, const float* nug_depth, int64_t Ng, const int64_t* ray_offsets,
-                            int32_t num_steps, int32_t iteration, float min_dis, const wb_sdf_state* state,
+                            int32_t num_steps, int32_t iteration, double min_dis, const wb_sdf_state* state,
                             float* xyz, float* depth, uint8_t* hit, float* alpha, wb_stream s)
 {
     WB_CHECK_ARG(rays != nullptr, "null rays");

@@ -172,7 +172,8 @@ class TriplanarGrid(nn.Module):
         return self.blas.raymarch(rays, raymarch_type=raymarch_type, num_samples=num_samples, level=0, **kw)
 
     def raytrace(self, rays, level=None, with_exit=False):
-        return self.blas.raytrace(rays, level=level, with_exit=with_exit)
+        """triplanar_grid.py:152-157: the blas is only used as an AABB tracer (level 0)."""
+        return self.blas.raytrace(rays, level=0, with_exit=with_exit)
 
     def query(self, coords, level=None, with_parents=False):
         return self.blas.query(coords, level=level, with_parents=with_parents)

@@ -759,7 +759,7 @@ def sdf_trace(nef, oct: OctreeTensors, origins, dirs, dist_max, level: int, lod_
         d, _, keep2 = fd
         with _stage("sdf_trace"):
             A.check(L.wb_sdf_trace(C.byref(od), C.byref(d), C.c_int32(lod_idx), C.byref(rays), A.ptr(nug_depth), C.c_int64(Ng), A.ptr(ray_off),
-                                   C.c_int32(num_steps), C.c_float(step_size), C.c_float(min_dis), C.c_int32(int(want_normals)), C.byref(st.c),
+                                   C.c_int32(num_steps), C.c_float(step_size), C.c_double(min_dis), C.c_int32(int(want_normals)), C.byref(st.c),
                                    A.ptr(out["xyz"]), A.ptr(out["depth"]), A.ptr(out["hit"]), A.ptr(out["normal"]), A.ptr(out["rgb"]), A.ptr(out["alpha"]), A.stream()))
         out["_evals"] = st.iterflags[2 * num_steps + 2: 2 * num_steps + 3]      # device counter: field evaluations of this launch
         return out, None
@@ -767,7 +767,7 @@ def sdf_trace(nef, oct: OctreeTensors, origins, dirs, dist_max, level: int, lod_
     # ---- generic field: the state machine runs natively, the field through its own forward() between the phases ----
     def phase(ph, it=0):
         A.check(L.wb_sdf_phase(C.c_int32(ph), C.byref(rays), A.ptr(nug_depth), C.c_int64(Ng), A.ptr(ray_off), C.c_int32(num_steps), C.c_int32(it),
-                               C.c_float(min_dis), C.byref(st.c), A.ptr(out["xyz"]), A.ptr(out["depth"]), A.ptr(out["hit"]), A.ptr(out["alpha"]), A.stream()))
+                               C.c_double(min_dis), C.byref(st.c), A.ptr(out["xyz"]), A.ptr(out["depth"]), A.ptr(out["hit"]), A.ptr(out["alpha"]), A.stream()))
 
     def field(x):
         return nef(coords=x, lod_idx=lod_idx, channels="sdf").reshape(-1).float() * 1.0 * step_size
@@ -982,6 +982,14 @@ def raymarch_level(grid, lod_idx: int) -> int:
         return grid.blas.max_level
     if hasattr(grid, "trinkets"):
         return grid.base_lod
+    return 0
+
+
+def raytrace_level(grid, lod_idx: int) -> int:
+    """Octree level PackedSDFTracer raytraces (packed_sdf_tracer.py:86 asks for active_lods[lod_idx]; BLASGrid.raytrace passes it
+    through, blas_grid.py:42-45, and TriplanarGrid.raytrace traces level 0 of its AABB blas instead, triplanar_grid.py:152-157)."""
+    if hasattr(grid, "codebook") or hasattr(grid, "trinkets"):
+        return grid.active_lods[lod_idx]
     return 0
 
 

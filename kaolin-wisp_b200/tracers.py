@@ -186,7 +186,7 @@ class PackedSDFTracer(BaseTracer):
         if lod_idx is None:
             lod_idx = nef.grid.num_lods - 1
         want_normals = "rgb" in channels or "normal" in channels
-        out, st = ops.sdf_trace(nef, ops.octree_tensors(nef.grid.blas), rays.origins, rays.dirs, rays.dist_max, nef.grid.active_lods[lod_idx], lod_idx,
+        out, st = ops.sdf_trace(nef, ops.octree_tensors(nef.grid.blas), rays.origins, rays.dirs, rays.dist_max, ops.raytrace_level(nef.grid, lod_idx), lod_idx,
                                 num_steps, step_size, min_dis, want_normals)
         hit = out["hit"]
         self.prev_num_evals = out.get("_evals")                          # device int32 [1] (fused kernel only): field evaluations of the trace

@@ -77,7 +77,7 @@ def test_sdf_trace_refuses_hash_fields():
     rays.num_rays = 1
     st = A.SdfState()
     rc = A.lib().wb_sdf_trace(None, C.byref(d), C.c_int32(3), C.byref(rays), None, C.c_int64(1), None, C.c_int32(8), C.c_float(1.0),
-                              C.c_float(1e-4), C.c_int32(0), C.byref(st), None, None, None, None, None, None, None)
+                              C.c_double(1e-4), C.c_int32(0), C.byref(st), None, None, None, None, None, None, None)
     assert rc == -1 and b"phase by phase" in A.lib().wb_last_error()
 
 
