@@ -20,6 +20,7 @@
 //                                                               constant-one slab behind every X_l tile gives the bias gradient;
 //                                                               fp32 accumulators in shared memory, one private copy per group)
 //     data grad     dX_l = dY_l . W_l                           (weight pack read MN-major: no transposed copy)
+//   as one commit group and one wait per layer (layers with inputs wider than 64: one round per chain, for the registers),
 //   and writes dL/dfeat as fp16 level-major planes [L][S][F], or scatters it into the hash table in its last epilogue.
 // Scatter  (wb_table_scatter_kernel, SIMT): lanes = consecutive samples; a thread builds its sample position once and walks all
 //   LODs; per LOD, runs of lanes that fall into the same cell are summed with a segmented warp scan and only the last lane of a
@@ -33,6 +34,7 @@
 #include "wb_shade_tc.cuh"
 #include "wb_tc.cuh"
 #include <math.h>
+#include <type_traits>
 
 #define TC_ML 16
 constexpr int TC_ROWS = 64;                 // samples per sub-tile (wgmma M)
@@ -353,30 +355,54 @@ struct TcCtx {
 __device__ __forceinline__ void tc_ctx_init(TcCtx& c, const WbTc& m, uint8_t* smem)
 {
     const int tig = threadIdx.x & (TC_GROUP - 1);
-    c.g = threadIdx.x / TC_GROUP;
+    // group and column half are broadcast from lane 0: ptxas then knows they are warp-uniform, and so is every branch and loop
+    // bound derived from them (the tile loop, the per-half warp-collective scatter).  Without that it treats the wgmmas as issued
+    // on a possibly divergent path and serializes every one of them (C7520).
+    c.g = __shfl_sync(0xffffffffu, threadIdx.x / TC_GROUP, 0);
     c.sub = smem + c.g * m.group_bytes; c.blob = smem + m.w_smem_off;
     c.scr = reinterpret_cast<float*>(c.sub + m.scr_off);
-    c.r = tig & (TC_ROWS - 1); c.h = tig / TC_ROWS; c.wl = tig;
+    c.r = tig & (TC_ROWS - 1); c.h = __shfl_sync(0xffffffffu, tig / TC_ROWS, 0); c.wl = tig;
 }
 __device__ __forceinline__ void tc_sync(const TcCtx& c) { tc_group_sync(c.g + 1, TC_GROUP); }
 // operand tiles written by the group's threads -> visible to the tensor cores of the whole group
 __device__ __forceinline__ void tc_publish(const TcCtx& c) { tc_fence_smem_async(); tc_sync(c); }
 
-// One MMA chain of the group: D[64 x N] = bias (fp16, bias pack: entry n at half index 8n) or 0, then += A . B over nk K-steps of
-// 16; wait; group barrier (every MMA of the group has read its operands: the epilogue may overwrite them); epi(d) on the fragments.
+// A round of the group: accumulators initialised (tc_acc_init), one fence, one or more chains issued (tc_issue), then
+// tc_round_wait: commit, wait, group barrier (every MMA of the group has read its operands: the epilogues may overwrite them).
+// Accumulator fragments D[64 x 2 NR] start from the bias (fp16, bias pack: entry n at half index 8n) or from +0.
+template <int NR>
+__device__ __forceinline__ void tc_acc_init(const TcCtx& c, float (&d)[NR], const __half* bias)
+{
+#pragma unroll
+    for (int i = 0; i < NR; ++i) {
+        if (bias) d[i] = __half2float(bias[tc_frag_col(c.wl, i) * 8]);
+        else d[i] = tc_opaque_zero();
+    }
+}
+// D += A . B over nk K-steps of 16, the descriptors advancing by aadv / badv (16-byte units) per step
+template <int TA, int TB, int NR>
+__device__ __forceinline__ void tc_issue(float (&d)[NR], uint64_t da, uint64_t db, int nk, uint32_t aadv, uint32_t badv)
+{
+    for (int kb = 0; kb < nk; ++kb) { WgMma<2 * NR, TA, TB>::run(d, da, db, 1u); da += aadv; db += badv; }
+}
+template <class... D>
+__device__ __forceinline__ void tc_round_wait(const TcCtx& c, D&... d)
+{
+    tc_wg_commit();
+    tc_wg_wait0();
+    (tc_wg_hold(d), ...);
+    tc_sync(c);
+}
+// One round of a single chain D[64 x N] = bias or 0, += A . B; then epi(d) on the fragments.
 template <int N, int TA, int TB, class Epi>
 __device__ __forceinline__ void tc_chain(const TcCtx& c, uint64_t da, uint64_t db, int nk, uint32_t aadv, uint32_t badv,
                                          const __half* bias, Epi&& epi)
 {
     float d[N / 2];
-#pragma unroll
-    for (int i = 0; i < N / 2; ++i) d[i] = bias ? __half2float(bias[tc_frag_col(c.wl, i) * 8]) : 0.0f;
+    tc_acc_init(c, d, bias);
     tc_wg_fence();
-    for (int kb = 0; kb < nk; ++kb) { WgMma<N, TA, TB>::run(d, da, db, 1u); da += aadv; db += badv; }
-    tc_wg_commit();
-    tc_wg_wait0();
-    tc_wg_hold(d);
-    tc_sync(c);
+    tc_issue<TA, TB>(d, da, db, nk, aadv, badv);
+    tc_round_wait(c, d);
     epi(d);
 }
 // the same with N chosen at run time (a multiple of 16, at most NMAX <= 128: the widest padded layer the kernel was built for; a
@@ -659,6 +685,55 @@ __device__ __forceinline__ void tc_scatter_level_f2(const WbGrid& g, int l, floa
     }
 }
 
+// One backward round of a layer, for the 64 output rows of the weight gradient whose dY^T slabs `dyw` addresses: the weight-grad
+// chain acc^T[64 x NK] += dY^T . X (wg), the bias-grad chain acc^T[64 x 8] += dY^T . [1 | 0] from the constant-one slab `xone`
+// (wg && bg) and the data-grad chain dX[64 x ND] = dY . W over nkd K-steps (dg) go out as one commit group, so their MMAs overlap;
+// then one wait, one group barrier and the epilogues in that order.  NK: the layer's padded input width; ND: NK, or 16 for the
+// first colour layer.
+template <int NK, int ND, class WEpi, class BEpi, class DEpi>
+__device__ __forceinline__ void tc_bwd_round(const TcCtx& c, bool wg, bool bg, bool dg, uint64_t dyw, uint64_t xw, uint64_t xone,
+                                             uint64_t dyd, uint64_t wd, int nkd, WEpi&& wepi, BEpi&& bepi, DEpi&& depi)
+{
+    float aw[NK / 2], ab[4], ad[ND / 2];
+    tc_acc_init(c, aw, nullptr); tc_acc_init(c, ab, nullptr); tc_acc_init(c, ad, nullptr);
+    tc_wg_fence();
+    if (wg) {
+        tc_issue<1, 1>(aw, dyw, xw, TC_ROWS / 16, 256 >> 4, 256 >> 4);           // K = the 64 samples, both operands MN-major
+        if (bg) tc_issue<1, 1>(ab, dyw, xone, TC_ROWS / 16, 256 >> 4, 256 >> 4);
+    }
+    if (dg) tc_issue<0, 1>(ad, dyd, wd, nkd, (2 * TC_SLAB) >> 4, 256 >> 4);       // weight pack read MN-major: no transposed copy
+    tc_round_wait(c, aw, ab, ad);
+    if (wg) { wepi(aw); if (bg) bepi(ab); }
+    if (dg) depi(ad);
+}
+// the same chains as one round each: inputs wider than 64, where the accumulators of a merged round (up to 132 per thread) no
+// longer fit the registers beside the rest of the kernel
+template <int NK, int ND, class WEpi, class BEpi, class DEpi>
+__device__ __forceinline__ void tc_bwd_rounds_seq(const TcCtx& c, bool wg, bool bg, bool dg, uint64_t dyw, uint64_t xw, uint64_t xone,
+                                                  uint64_t dyd, uint64_t wd, int nkd, WEpi&& wepi, BEpi&& bepi, DEpi&& depi)
+{
+    if (wg) {
+        tc_chain<NK, 1, 1>(c, dyw, xw, TC_ROWS / 16, 256 >> 4, 256 >> 4, nullptr, wepi);
+        if (bg) tc_chain<8, 1, 1>(c, dyw, xone, TC_ROWS / 16, 256 >> 4, 256 >> 4, nullptr, bepi);
+    }
+    if (dg) tc_chain<ND, 0, 1>(c, dyd, wd, nkd, (2 * TC_SLAB) >> 4, 256 >> 4, nullptr, depi);
+}
+// the round(s) with NK = Kp chosen at run time (a multiple of 16, at most 128); D16: the data grad is 16 wide
+template <bool D16, class... A>
+__device__ __forceinline__ void tc_bwd_round_n(int Kp, A&&... a)
+{
+    switch (Kp) {
+        case 16: tc_bwd_round<16, 16>(a...); break;
+        case 32: tc_bwd_round<32, D16 ? 16 : 32>(a...); break;
+        case 48: tc_bwd_round<48, D16 ? 16 : 48>(a...); break;
+        case 64: tc_bwd_round<64, D16 ? 16 : 64>(a...); break;
+        case 80: tc_bwd_rounds_seq<80, D16 ? 16 : 80>(a...); break;
+        case 96: tc_bwd_rounds_seq<96, D16 ? 16 : 96>(a...); break;
+        case 112: tc_bwd_rounds_seq<112, D16 ? 16 : 112>(a...); break;
+        default: tc_bwd_rounds_seq<128, D16 ? 16 : 128>(a...); break;
+    }
+}
+
 // wmask: layers whose weight gradients this launch accumulates; emit: this launch produces dL/dfeat (planes, or FUSE: the hash-table
 // scatter of an F == 2 'cat' grid in the last epilogue).  Wide decoders whose accumulators do not all fit run several launches.
 template <int NG, bool FUSE>
@@ -715,37 +790,43 @@ wb_mlp_bwd_tc_kernel(WbTc m, const uint8_t* __restrict__ blob, TcIn in, const fl
             tc_publish(c);
             const int I = m.I[l], O = m.O[l], Kp = m.Kp[l], Np = m.Np[l];
             const uint32_t xb = tc_smem_u32(c.sub + m.tile_off[l]);
-            if (m.acc_l[l] >= 0) {
-                // acc_l^T[out, in] += dY_l^T . X_l and, from the constant-one slab, acc_l^T[out, I] += dY_l^T . 1  (K = the 64 samples)
-                float* al = acc + m.acc_l[l];
-                for (int mb = 0; mb < Np; mb += 64) {
-                    const uint64_t da = tc_desc(dyb + (uint32_t)(mb / 8) * TC_SLAB, 128, TC_SLAB);
-                    tc_chain_n<1, 1>(c, Kp, da, tc_desc(xb, 128, TC_SLAB), TC_ROWS / 16, 256 >> 4, 256 >> 4, nullptr, [&](auto& d) {
-                        constexpr int NR = sizeof(d) / sizeof(float);
+            // weight grad acc_l^T[out, in] += dY_l^T . X_l and, from the constant-one slab, acc_l^T[out, I] += dY_l^T . 1, one round per
+            // block of 64 outputs; the data grad dX_l = dY_l . W_l joins the round of the last block
+            const bool wg = m.acc_l[l] >= 0, bg = m.src_b[l] >= 0, dg = l > 0 || emit;
+            float* al = acc + m.acc_l[l];
+            const uint64_t xw = tc_desc(xb, 128, TC_SLAB), xone = tc_desc(xb + (uint32_t)(Kp / 8) * TC_SLAB, 128, TC_SLAB);
+            const uint64_t dyd = tc_desc(dyb, TC_SLAB, 128), wd = tc_desc(wb + m.w_off[l], 128, Np * 16);
+            auto rounds = [&](auto d16, auto&& depi) {
+                const int nmb = wg ? (Np + 63) / 64 : 1;
+                for (int b = 0; b < nmb; ++b) {
+                    const int mb = 64 * b;
+                    tc_bwd_round_n<decltype(d16)::value>(Kp, c, wg, bg, dg && b == nmb - 1, tc_desc(dyb + (uint32_t)(mb / 8) * TC_SLAB, 128, TC_SLAB),
+                                                         xw, xone, dyd, wd, Np / 16,
+                        [&](auto& d) {
+                            constexpr int NR = sizeof(d) / sizeof(float);
 #pragma unroll
-                        for (int i = 0; i < NR; ++i) {
-                            const int o = mb + tc_frag_row(c.wl, i), k = tc_frag_col(c.wl, i);
-                            if (o < O && k < I) al[o * (I + 1) + k] += d[i];
-                        }
-                    });
-                    if (m.src_b[l] >= 0)
-                        tc_chain<8, 1, 1>(c, da, tc_desc(xb + (uint32_t)(Kp / 8) * TC_SLAB, 128, TC_SLAB), TC_ROWS / 16, 256 >> 4, 256 >> 4, nullptr, [&](auto& d) {
+                            for (int i = 0; i < NR; ++i) {
+                                const int o = mb + tc_frag_row(c.wl, i), k = tc_frag_col(c.wl, i);
+                                if (o < O && k < I) al[o * (I + 1) + k] += d[i];
+                            }
+                        },
+                        [&](auto& d) {
 #pragma unroll
                             for (int i = 0; i < 4; ++i) {
                                 const int o = mb + tc_frag_row(c.wl, i);
                                 if (o < O && tc_frag_col(c.wl, i) == 0) al[o * (I + 1) + I] += d[i];
                             }
-                        });
+                        },
+                        depi);
                 }
+            };
+            if (!dg) {
+                if (wg) rounds(std::false_type(), [](auto&) {});
+                break;
             }
-            if (l == 0 && !emit) break;
-            // dX_l = dY_l . W_l  (A: dY tile K-major over the Np outputs, B: weight pack read MN-major); the first colour layer only needs
-            // the gradient of its dout - 1 <= 15 density features
-            const int N = (l == m.nl_d) ? 16 : Kp;
-            const uint64_t da = tc_desc(dyb, TC_SLAB, 128), db = tc_desc(wb + m.w_off[l], 128, Np * 16);
             if (l == m.nl_d) {
-                // first colour layer: inputs [df[1:dout], embed(ray_d)]; only the first dout-1 carry gradient (nerf.py:259)
-                tc_chain_n<0, 1>(c, N, da, db, Np / 16, (2 * TC_SLAB) >> 4, 256 >> 4, nullptr, [&](auto& d) { TC_FRAG_TO_SCRATCH(c, d, 16); });
+                // first colour layer: inputs [df[1:dout], embed(ray_d)]; only the first dout-1 <= 15 carry gradient (nerf.py:259)
+                rounds(std::true_type(), [&](auto& d) { TC_FRAG_TO_SCRATCH(c, d, 16); });
                 tc_sync(c);
                 const float* v = c.scr + c.r * TC_SCR_LD;
                 const int dout = m.O[m.nl_d - 1];
@@ -758,7 +839,7 @@ wb_mlp_bwd_tc_kernel(WbTc m, const uint8_t* __restrict__ blob, TcIn in, const fl
             } else if (l == 0 && FUSE) {
                 // dL/d(grid features) -> hash table: column half h holds features [16h, 16h+16) = LODs 8h .. 8h+7; a warp = 32
                 // consecutive samples of one half
-                tc_chain_n<0, 1>(c, N, da, db, Np / 16, (2 * TC_SLAB) >> 4, 256 >> 4, nullptr, [&](auto& d) { TC_FRAG_TO_SCRATCH(c, d, 32); });
+                rounds(std::false_type(), [&](auto& d) { TC_FRAG_TO_SCRATCH(c, d, 32); });
                 tc_sync(c);
                 const float* v = c.scr + c.r * TC_SCR_LD + c.h * 16;
                 const float3 p = wb_ray_point(in.origins, in.dirs, ray, __ldg(in.rec_t + s));
@@ -771,7 +852,7 @@ wb_mlp_bwd_tc_kernel(WbTc m, const uint8_t* __restrict__ blob, TcIn in, const fl
                 // dL/d(grid features) -> fp16 planes [plane][S][width] (still loss-scaled), straight from the fragments
                 const int W = G.width, nfe = G.planes * W;
                 const int64_t srow0 = tile * TC_ROWS;
-                tc_chain_n<0, 1>(c, N, da, db, Np / 16, (2 * TC_SLAB) >> 4, 256 >> 4, nullptr, [&](auto& d) {
+                rounds(std::false_type(), [&](auto& d) {
                     constexpr int NR = sizeof(d) / sizeof(float);
 #pragma unroll
                     for (int i = 0; i < NR; i += 2) {
@@ -788,7 +869,7 @@ wb_mlp_bwd_tc_kernel(WbTc m, const uint8_t* __restrict__ blob, TcIn in, const fl
             } else {
                 // hidden layer input: apply relu' from the retained activation tile, write the next dY (Np[l-1] == Kp[l])
                 const uint8_t* xt = c.sub + m.tile_off[l];
-                tc_chain_n<0, 1>(c, N, da, db, Np / 16, (2 * TC_SLAB) >> 4, 256 >> 4, nullptr, [&](auto& d) {
+                rounds(std::false_type(), [&](auto& d) {
                     constexpr int NR = sizeof(d) / sizeof(float);
                     const __half2 z2 = __float2half2_rn(0.0f);
 #pragma unroll

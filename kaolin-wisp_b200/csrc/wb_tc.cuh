@@ -118,6 +118,14 @@ template <int TA, int TB> struct WgMma<128, TA, TB> {
 __device__ __forceinline__ void tc_wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void tc_wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void tc_wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// +0.0f as a value ptxas cannot fold: when the accumulators of a chain start from a known zero, ptxas puts an arrive and a full
+// wait around every wgmma of the kernel (C7519), serializing the chains
+__device__ __forceinline__ float tc_opaque_zero()
+{
+    float z;
+    asm volatile("mov.b32 %0, 0;" : "=f"(z));
+    return z;
+}
 // keep the accumulator registers live across the asynchronous MMAs (the compiler must not move reads above the wait)
 template <int NR> __device__ __forceinline__ void tc_wg_hold(float (&d)[NR])
 {
