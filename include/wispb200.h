@@ -114,12 +114,9 @@ typedef struct wb_octree {
 } wb_octree;                                /*   marcher skip whole 32-candidate words. NULL -> off  */
 
 /* ------------------------------------------------------------------------------------------------
- * SPC helpers  -- replace kaolin.ops.spc.{scan_octrees, generate_points, unbatched_query}
+ * SPC helpers  -- replace kaolin.ops.spc.unbatched_query; occupancy bitmasks for the marcher
  *   call sites: wisp/ops/spc/conversions.py:84-87, wisp/accelstructs/octree_as.py:146-163
  * ---------------------------------------------------------------------------------------------- */
-/* points: int16 [total,3] (generate_points); pyramid on the host. */
-int wb_octree_generate_points(const uint8_t* octree, const int32_t* prefix, int64_t nbytes,
-                              int16_t* points, int64_t total, wb_stream s);
 /* bits: zero-initialised uint32 [(8^level + 31)/32]; bit (x<<2L | y<<L | z) set iff the level-L cell is occupied. */
 int wb_octree_build_bits(const int16_t* level_points, int64_t num_points, int32_t level, uint32_t* bits, wb_stream s);
 /* coarse_bits: zero-initialised uint32 [(8^coarse_level + 31)/32]; a bit is set iff the coarse cell or one of its 26

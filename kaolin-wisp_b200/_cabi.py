@@ -82,7 +82,7 @@ class RMSpropSegment(C.Structure):
 
 EXPORTS = [
     "wb_last_error", "wb_version", "wb_device_check", "wb_launch_count",
-    "wb_octree_generate_points", "wb_octree_build_bits", "wb_octree_build_coarse", "wb_query",
+    "wb_octree_build_bits", "wb_octree_build_coarse", "wb_query",
     "wb_raymarch_ray_count", "wb_scan_workspace_bytes", "wb_scan_counts", "wb_raymarch_ray_fill",
     "wb_raytrace_count", "wb_raytrace_fill", "wb_raytrace_cache_bytes", "wb_raytrace_count_cached", "wb_raytrace_fill_cached", "wb_raymarch_voxel_fill", "wb_raymarch_uniform_count", "wb_raymarch_uniform_fill",
     "wb_hashgrid_fwd", "wb_hashgrid_bwd", "wb_triplane_fwd", "wb_triplane_bwd", "wb_triplane_relayout",

@@ -164,12 +164,16 @@ __device__ __forceinline__ uint32_t wb_hash_idx(int x, int y, int z, int res, ui
 // wb_hash_idx, evaluated with one multiply per axis.  The level kind is warp-uniform, so this is a branch, not a select: the
 // straightforward form made ptxas compute BOTH index kinds for all 8 corners with the products and the constant loads repeated
 // (~100 instructions per level in the gather and the scatter).
+// Dense levels: from res 258 on the clamp bound fl(res - 1 - 1e-5) is res - 1 itself, so a coordinate at +1 lands on cell res - 1
+// with weight 0 on its +1 corner, which would be row res on that axis -- outside the level's res^3 rows (past the table's end on the
+// last level).  That corner keeps the cell's own row instead: its coefficient is 0, so finite tables give the same features.
 __device__ __forceinline__ void wb_corner_indices(const WbGrid& g, int l, int px, int py, int pz, uint32_t idx[8]) {
     if (g.dense[l]) {
-        const uint32_t r1 = (uint32_t)g.res[l], r2 = r1 * r1;
+        const uint32_t r1 = (uint32_t)g.res[l], r2 = r1 * r1, top = r1 - 1u;
         const uint32_t b = (uint32_t)px + (uint32_t)py * r1 + (uint32_t)pz * r2;
+        const uint32_t sx = (uint32_t)px < top ? 1u : 0u, sy = (uint32_t)py < top ? r1 : 0u, sz = (uint32_t)pz < top ? r2 : 0u;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) idx[j] = b + ((j & 4) ? 1u : 0u) + ((j & 2) ? r1 : 0u) + ((j & 1) ? r2 : 0u);
+        for (int j = 0; j < 8; ++j) idx[j] = b + ((j & 4) ? sx : 0u) + ((j & 2) ? sy : 0u) + ((j & 1) ? sz : 0u);
     } else {
         const uint32_t m = g.Tmask;
         const uint32_t x0 = (uint32_t)px, x1 = x0 + 1u;

@@ -1,53 +1,7 @@
-// wb_spc.cu -- SPC (octree) helpers: point generation, dense occupancy bitmask, point-in-octree query.
-// Replaces kaolin.ops.spc.{generate_points, unbatched_query} at the call sites
+// wb_spc.cu -- SPC (octree) helpers: dense occupancy bitmasks, point-in-octree query.
+// Replaces kaolin.ops.spc.unbatched_query at the call sites
 // wisp/ops/spc/conversions.py:84-87 and wisp/accelstructs/octree_as.py:146-163.
 #include "wb_common.cuh"
-
-// generate_points [KAOLIN-EXT]: children of node i (in bit order) are points prefix[i]+1 ... ; child = 2*p + (c>>2&1, c>>1&1, c&1).
-// One thread per (node, child bit): each level only depends on the previous one, so the kernel is launched
-// once per level by the host wrapper below (levels are contiguous ranges of nodes).
-__global__ void wb_generate_points_kernel(const uint8_t* __restrict__ octree, const int32_t* __restrict__ prefix,
-                                          int64_t node_begin, int64_t node_end, int16_t* __restrict__ points, int64_t total)
-{
-    int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int64_t node = node_begin + (t >> 3);
-    int c = (int)(t & 7);
-    if (node >= node_end) return;
-    uint32_t b = octree[node];
-    if (!(b & (1u << c))) return;
-    int64_t child = (int64_t)prefix[node] + __popc(b & ((2u << c) - 1u));
-    if (child >= total) return;
-    points[child * 3 + 0] = (int16_t)(2 * points[node * 3 + 0] + ((c >> 2) & 1));
-    points[child * 3 + 1] = (int16_t)(2 * points[node * 3 + 1] + ((c >> 1) & 1));
-    points[child * 3 + 2] = (int16_t)(2 * points[node * 3 + 2] + (c & 1));
-}
-
-__global__ void wb_zero_root_kernel(int16_t* points) { points[0] = points[1] = points[2] = 0; }
-
-extern "C" int wb_octree_generate_points(const uint8_t* octree, const int32_t* prefix, int64_t nbytes,
-                                         int16_t* points, int64_t total, wb_stream s)
-{
-    WB_CHECK_ARG(octree && prefix && points, "null pointer");
-    WB_CHECK_ARG(total >= 1, "total must include the root");
-    cudaStream_t st = (cudaStream_t)s;
-    wb_zero_root_kernel<<<1, 1, 0, st>>>(points); WB_LAUNCH_CHECK();
-    // level boundaries are data dependent; walking them needs the per-level counts, which the host shim already
-    // has in `pyramid`.  To stay self-contained we derive them here from prefix[] with tiny D2H reads.
-    int64_t begin = 0, count = 1;
-    while (begin < nbytes) {
-        int64_t end = begin + count; if (end > nbytes) end = nbytes;
-        int64_t threads = (end - begin) * 8;
-        wb_generate_points_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(octree, prefix, begin, end, points, total);
-        WB_LAUNCH_CHECK();
-        int32_t pe = 0, pb = 0;   // children of this level = prefix[end] - prefix[begin]
-        WB_CUDA(cudaMemcpyAsync(&pe, prefix + end, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        WB_CUDA(cudaMemcpyAsync(&pb, prefix + begin, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        WB_CUDA(cudaStreamSynchronize(st));   // setup-time only (octree construction), never on the render path
-        begin = end; count = (int64_t)pe - pb;
-        if (count <= 0) break;
-    }
-    return WB_OK;
-}
 
 __global__ void wb_build_bits_kernel(const int16_t* __restrict__ pts, int64_t n, int level, uint32_t* __restrict__ bits)
 {
@@ -130,7 +84,8 @@ extern "C" int wb_query(const wb_octree* oct, const float* coords, int64_t N, in
 //     does not depend on it).  u: explicit [N,3] tensor (parity tests replay the reference's draw) or the counter-based stream
 //     keyed by (seed, cell, axis) -- the same seed on every rank gives the same probe points, so pruned octrees agree across
 //     GPUs without a broadcast.
-//   wb_prune_update: occupancy = max(density, occupancy * decay) (:186,:196), keep = occupancy > min_density (:198).
+//   wb_prune_update: occupancy = max(density, occupancy * decay) (:186,:196) with torch.max's NaN propagation, keep = occupancy >
+//     min_density (:198).
 // The probe itself is the fused shade kernel (wb_rf_shade_fwd with the probe points as zero-length rays).
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void wb_prune_samples_kernel(const int16_t* __restrict__ points, int64_t N, float res, const float* __restrict__ u, uint32_t seed,
@@ -166,7 +121,10 @@ __global__ void wb_prune_update_kernel(const float4* __restrict__ shaded, int64_
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N) return;
-    const float occ = fmaxf(__ldg(shaded + i).w, __fmul_rn(occupancy[i], decay));
+    // torch.stack([density, occupancy * decay], -1).max(-1) propagates a NaN from either side (fmaxf would drop it): a cell whose
+    // density or occupancy has diverged stores NaN and is not kept
+    const float d = __ldg(shaded + i).w, od = __fmul_rn(occupancy[i], decay);
+    const float occ = (isnan(d) || isnan(od)) ? __fadd_rn(d, od) : fmaxf(d, od);
     occupancy[i] = occ;
     keep[i] = occ > min_density ? 1 : 0;
 }

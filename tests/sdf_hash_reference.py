@@ -6,9 +6,7 @@ _scatter (the atomics of dL/dfeat).  This module adds a HashField and hooks thos
 the unchanged octree functions, so octree results stay bit-identical.  Importing the module installs the hook.
 
 Rounding points of a hash field (wb_sdf.cuh: sdf_hash_features, wb_sdf_train.cu: sdf_hash_scatter)
-  cells      wb_cell per axis: x = fmaf(c, res/2, res/2), clamped into [0, fl(res - 1 - 1e-5)], p = floor(x), w = x - p (exact),
-             1 - w rounded; coefficients ((i_x i_y) i_z ...) z fastest, each product rounded; corner rows x + y res + z res^2 on dense
-             levels (res^3 < 2^bitwidth), the xor-prime hash & (2^bitwidth - 1) on the others.  Bit-exact.
+  cells      tests/grid_index_reference.py: corners (wb_cell, wb_corner_setup, wb_corner_indices).  Bit-exact.
   features   per LOD fl(v_0 c_0), then fmaf over corners 1..7 (wb_hashgrid_fwd's order); 'sum' adds all LODs in LOD order whatever
              lod_idx, 'cat' is L * F wide with the LODs >= lod_idx zero.  Bit-exact, radius 0.
   scatter    fl(g c_j) per sample, LOD and corner, one atomic each (colliding corners of one sample count separately); the zeroed 'cat'
@@ -22,7 +20,9 @@ import numpy as np
 
 from oracle import sdf_reference as S
 
-P1, P2 = 2654435761, 805459861
+import grid_index_reference as GR
+
+P1, P2 = GR.P1, GR.P2
 
 
 @dataclass
@@ -41,33 +41,12 @@ def hash_field(table, begin, resolutions, bitwidth, multiscale, Ws, bs, pos_mode
                      pos_mode, pos_freq, False, [int(r) for r in resolutions], int(bitwidth))
 
 
-def _axis(c, res):
-    h = np.float32(0.5 * res)
-    x = S.fma32(c, h, h)
-    x = np.maximum(0.0, np.minimum(float(np.float32(res - 1 - 1e-5)), x))
-    p = np.floor(x)
-    w = x - p
-    return p.astype(np.int64), w, S.r32(1.0 - w)
-
-
 def _hash_cells(field: HashField, coords: np.ndarray) -> S.Cells:
-    c = np.asarray(coords, np.float32).astype(np.float64)
-    T = 2 ** field.bitwidth
+    c = np.asarray(coords, np.float32)
     oks, tks, cfs = [], [], []
     for res in field.resolutions:
-        (px, wx, ix), (py, wy, iy), (pz, wz, iz) = (_axis(c[:, a], res) for a in range(3))
-        xy = {0: S.r32(ix * iy), 1: S.r32(ix * wy), 2: S.r32(wx * iy), 3: S.r32(wx * wy)}
-        cf = np.zeros((c.shape[0], 8)); tk = np.zeros((c.shape[0], 8), np.int64)
-        dense = res < T and res ** 2 < T and res ** 3 < T
-        for j in range(8):
-            dx, dy, dz = (j >> 2) & 1, (j >> 1) & 1, j & 1
-            cf[:, j] = S.r32(xy[j >> 1] * (wz if dz else iz))
-            x, y, z = px + dx, py + dy, pz + dz
-            if dense:
-                tk[:, j] = x + y * res + z * res * res
-            else:
-                tk[:, j] = (x ^ ((y * P1) & 0xFFFFFFFF) ^ ((z * P2) & 0xFFFFFFFF)) & (T - 1)
-        oks.append(np.ones(c.shape[0], bool)); tks.append(tk); cfs.append(cf)
+        tk, cf = GR.corners(c, res, field.bitwidth)
+        oks.append(np.ones(c.shape[0], bool)); tks.append(tk); cfs.append(cf.astype(np.float64))
     return S.Cells(oks, tks, cfs)
 
 
