@@ -478,6 +478,41 @@ int wb_prune_update(const float* shaded, int64_t N, float decay, float min_densi
  * ---------------------------------------------------------------------------------------------- */
 int wb_tc_selftest(const void* a_img, int a_bytes, const void* b_img, int b_bytes, float* D, int N, int K, int mode, wb_stream s);
 
+/* ------------------------------------------------------------------------------------------------
+ * HashGrid.interpolate over [N, 2] coordinates (app/image): wb_hashgrid_fwd / _bwd's contract and layouts, with the reference's 2-D
+ * kernels (hashgrid_interpolate_2d_cuda_kernel and its backward, hashgrid_interpolate_cuda.cu:214-339, hash_index_2d in
+ * hash_utils.cuh:65-84; the reference picks them from coords.size(1), :374): 4 corners per LOD, dense rows x + y*res
+ * when res < T and res^2 < T, hashed rows (x ^ y*2654435761) & (T-1) otherwise.  Only the hash fields of `grid` are read.  Rows are
+ * level-local from begin_idxes, so tables of min(res^3, T) rows per level (coord_dim = 3, what image_hash.yaml builds) and of
+ * min(res^2, T) rows (coord_dim = 2) both work.  Deviation: on a dense level's last cell (res >= 258, coordinate +1) the weight-0 +1
+ * corner keeps the cell's own row instead of the reference's row past the level.  No gradient to the coordinates. */
+int wb_hashgrid2d_fwd(const float* coords, int64_t N, const wb_nef_desc* grid, float* feats, wb_stream s);
+int wb_hashgrid2d_bwd(const float* coords, int64_t N, const wb_nef_desc* grid, const float* grad_feats,
+                      float* grad_table, wb_stream s);
+
+/* ------------------------------------------------------------------------------------------------
+ * ImageNeuralField (wisp/models/nefs/image_nef.py:37-97) of app/image over a 2-D HashGrid, fp32 SIMT, one launch each:
+ *   wb_image_eval  replaces ImageNeuralField.rgb: sigmoid(decoder(cat([HashGrid.interpolate(coords, lod_idx), embed(coords)]))),
+ *                  embed = get_positional_embedder(3, include_input=True) on [N, 2]: [x, y, sin(x 2^k, y 2^k)_k, cos(...)_k], 14 wide.
+ *                  'cat': features of LODs >= lod_idx are zero (hash_grid.py:228); 'sum' adds all LODs.  rgb f32 [N, 3].
+ *   wb_image_train one ImageTrainer.step (wisp/trainers/image_trainer.py:51-80) without the optimiser: the forward of wb_image_eval,
+ *                  F.mse_loss over [N, 3] and the backward.  Accumulates (the caller zeroes): *loss_out += sum (y - gt)^2 * inv_count
+ *                  (inv_count = 1 / (3N): the mean), grad_table [rows, F] += dL/d codebook.feats (the zeroed 'cat' LODs get nothing),
+ *                  grad_params += dL/d params.
+ * grid: hash fields of a wb_nef_desc, feature_dim 2, 4 or 8, table 8-byte (F = 2) or 16-byte aligned, grad_table aligned alike.
+ * Decoder: BasicDecoder(in, 3, relu, bias=True, num_layers=1, hidden_dim) with in = (L*F 'cat' | F 'sum') + 14 and hidden_dim a
+ * multiple of 4 up to 128; params: HOST array of 4 device pointers W0 [H, in], b0 [H], Wout [3, H], bout [3] (nn.Linear layout);
+ * grad_params packed [W0, b0, Wout, bout] in that order.  N >= 1.
+ * Deviations: the table is read in fp32 (no enable_amp fp16 copy); embedder.bands is not trained (requires_grad=False in the
+ * reference too) and is taken as 2^0, 2^1, 2^2. */
+int wb_image_eval(const wb_nef_desc* grid, int32_t hidden_dim, const float* const* params, int32_t lod_idx, const float* coords,
+                  int64_t N, float* rgb, wb_stream s);
+int wb_image_train(const wb_nef_desc* grid, int32_t hidden_dim, const float* const* params, int32_t lod_idx, const float* coords,
+                   const float* rgb_gt, int64_t N, float inv_count, float* grad_table, float* grad_params, float* loss_out, wb_stream s);
+/* Dynamic shared memory (bytes) of a wb_image_eval (train = 0) or wb_image_train (train != 0) launch for this field, or < 0 when the
+ * kernel does not take it (the reason in wb_last_error()).  Host only: no device is touched. */
+int64_t wb_image_smem_bytes(const wb_nef_desc* grid, int32_t hidden_dim, int32_t train);
+
 #ifdef __cplusplus
 }
 #endif

@@ -47,7 +47,7 @@ class HashGrid(nn.Module):
     def __init__(self, blas: OctreeAS, feature_dim: int, resolutions: List[int], multiscale_type: str = 'sum',
                  feature_std: float = 0.0, feature_bias: float = 0.0, codebook_bitwidth: int = 8, coord_dim: int = 3):
         super().__init__()
-        assert coord_dim == 3, "the accelerated path covers the 3D hash grid"
+        assert coord_dim in (2, 3)                         # hash_grid.py:62
         self.blas = blas
         if blas is not None:
             lvl = blas.max_level

@@ -2,7 +2,7 @@
 (INTEGRATION.md section 3).  Nothing is patched unless `wisp` imports; WISP_B200=0 disables the hook.
 
 What is patched (reference file:line -> native replacement):
-  wisp.ops.grid.hashgrid                        (ops/grid.py:128-144)              ops.hashgrid
+  wisp.ops.grid.hashgrid                        (ops/grid.py:128-144)              ops.hashgrid ([N, 3] and, for app/image, [N, 2])
   OctreeAS.query / raytrace                     (octree_as.py:146-186)             wb_query / wb_raytrace_*
   OctreeAS._raymarch_ray / _voxel / _uniform    (octree_as.py:188-374)             wb_raymarch_*
   TriplanarGrid.interpolate                     (triplanar_grid.py:98-121)         wb_triplane_*
@@ -10,11 +10,13 @@ What is patched (reference file:line -> native replacement):
   PackedRFTracer.trace                          (packed_rf_tracer.py:84-181)       fused render path (ops.rf_trace)
   PackedSDFTracer.trace                         (packed_sdf_tracer.py:57-174)      wb_sdf_trace
   NeuralSDF.sdf (no-grad)                       (neural_sdf.py:120-155)            wb_sdf_eval
+  ImageNeuralField.rgb (no-grad)                (image_nef.py:77-97)               wb_image_eval
   NeuralRadianceField.prune                     (nerf.py:175-212)                  ops.prune_field
 Every replacement keeps the reference signature, falls back to the original method for configurations outside the native
 path (unknown embedders, activations, grids), and keeps the attributes other wisp code reads (`prev_num_samples`, `bg_color`).
 The grid and SDF-tracer replacements run the methods of this package's mirror classes (grids.py, tracers.py); the rest share
-their host logic with the mirrors through ops (octree_tensors, march, resolve_precision, sdf_channel).
+their host logic with the mirrors through ops (octree_tensors, march, resolve_precision, sdf_channel, image_rgb).
+ImageTrainer.step itself is not patched: wisp_b200.ImageStep is its native counterpart (INTEGRATION.md).
 """
 from __future__ import annotations
 
@@ -141,6 +143,20 @@ def install() -> bool:
         return ops.sdf_channel(self, coords, lod_idx) or orig_sdf(self, coords, lod_idx)
 
     _patch(NeuralSDF, "sdf", sdf)
+
+    # ---- image field (app/image; a wisp without it keeps every other patch) ---------------------------------------
+    try:
+        from wisp.models.nefs.image_nef import ImageNeuralField
+    except Exception:
+        ImageNeuralField = None
+    if ImageNeuralField is not None:
+        orig_rgb = ImageNeuralField.rgb
+
+        def image_rgb(self, coords, lod=None):
+            fused = ops.image_rgb(self, coords, lod)
+            return fused if fused is not None else orig_rgb(self, coords, lod)
+
+        _patch(ImageNeuralField, "rgb", image_rgb)
 
     # ---- pruning -------------------------------------------------------------------------------------------------
     orig_prune = NeuralRadianceField.prune

@@ -3,6 +3,7 @@
   wisp.models.nefs.BaseNeuralField       (wisp/models/nefs/base_nef.py:120-202, channel dispatch)
   wisp.models.decoders.BasicDecoder      (wisp/models/decoders/basic_decoders.py:16-101)
   wisp.models.embedders.PositionalEmbedder / get_positional_embedder (positional_embedder.py:15-100)
+  wisp.models.nefs.ImageNeuralField      (wisp/models/nefs/image_nef.py:37-97)
 Module / parameter names are the reference's (decoder_density.layers.N.weight, decoder_color.lout.bias,
 grid.codebook.feats ...).  `rgba()` is the unfused route (our hash-grid kernel + torch Linear); the tracer uses
 `fused_spec()` to hand the whole field to the fused native pipeline instead.
@@ -271,3 +272,39 @@ class NeuralSDF(BaseNeuralField):
 
     def decoder_input_dim(self):
         return self.effective_feature_dim() + self.pos_embed_dim
+
+
+class ImageNeuralField(BaseNeuralField):
+    """wisp.models.nefs.ImageNeuralField (image_nef.py:37-97): grid features (FIRST) + a 3-band positional embedding of the [N, 2]
+    pixel coordinates -> BasicDecoder(bias=True, 3 outputs) -> sigmoid.  Parameter names are the reference's (grid.codebook.feats,
+    decoder.layers.0.weight, decoder.lout.bias, embedder.bands)."""
+
+    def __init__(self, grid, activation_type='relu', layer_type='none', hidden_dim=128, num_layers=1):
+        super().__init__()
+        self.grid = grid
+        if activation_type != 'relu' or layer_type not in ('linear', 'none'):
+            raise NotImplementedError("wisp_b200 covers activation_type='relu', layer_type='linear'/'none'")
+        self.activation_type, self.layer_type, self.hidden_dim, self.num_layers = activation_type, layer_type, hidden_dim, num_layers
+        self.feature_dim = grid.feature_dim * len(grid.resolutions) if grid.multiscale_type == 'cat' else grid.feature_dim
+        self.embedder, self.embed_dim = get_positional_embedder(frequencies=3, include_input=True)
+        self.embed_dim = 14                       # image_nef.py:63: the embedder's out_dim says 21 (input_dim=3), 2-D input gives 14
+        self.input_dim = self.feature_dim + self.embed_dim
+        self.decoder = BasicDecoder(self.input_dim, 3, torch.relu, True, nn.Linear, num_layers, hidden_dim)
+
+    def register_forward_functions(self):
+        self._register_forward_function(self.rgb, ["rgb"])
+
+    def rgb(self, coords, lod=None):
+        """image_nef.py:77-97.  Without autograd or autocast (the trainer's validate() and render_final_view) the whole evaluation --
+        2-D hash-grid gather of every LOD, embedding, decoder, sigmoid -- is one native launch (wb_image_eval); otherwise the native
+        grid kernel + torch embedding and decoder."""
+        fused = ops.image_rgb(self, coords, lod)
+        if fused is not None:
+            return fused
+        if lod is None:
+            lod = len(self.grid.resolutions) - 1
+        batch, _ = coords.shape
+        feats = self.grid.interpolate(coords, lod).reshape(-1, self.feature_dim)
+        embedded_pos = self.embedder(coords).view(batch, self.embed_dim)
+        fpos = torch.cat([feats, embedded_pos], dim=-1)
+        return torch.sigmoid(self.decoder(fpos))

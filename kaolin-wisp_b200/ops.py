@@ -412,7 +412,8 @@ def _no_coords_grad(ctx, i: int) -> None:
 
 
 class HashGridInterpolate(torch.autograd.Function):
-    """wisp.ops.grid.HashGridInterpolate (ops/grid.py:77-126) over wb_hashgrid_fwd / wb_hashgrid_bwd.
+    """wisp.ops.grid.HashGridInterpolate (ops/grid.py:77-126) over wb_hashgrid_fwd / wb_hashgrid_bwd ([N, 3] coordinates) or
+    wb_hashgrid2d_fwd / wb_hashgrid2d_bwd ([N, 2], app/image), chosen from the coordinate width as the reference's kernel does.
     Differences by design: all LODs in one launch; the table is read as fp32 master (no per-call .half() copy,
     ops/grid.py:88-89) and gradients accumulate in fp32."""
 
@@ -421,7 +422,9 @@ class HashGridInterpolate(torch.autograd.Function):
         if codebook.shape[-1] % 2 == 1:
             raise Exception("The codebook feature dimension needs to be a multiple of 2.")   # ops/grid.py:83-84
         _no_coords_grad(ctx, 0)
-        assert coords.shape[-1] == 3, "only the 3D hash grid is on the accelerated path"
+        dim = coords.shape[-1]
+        if dim not in (2, 3):
+            raise ValueError(f"HashGrid.interpolate: coordinates must be 2-D or 3-D (the reference's coord_dim), got width {dim}")
         A.require_device(codebook)
         c = A.f32c(coords)
         res = [int(r) for r in torch.as_tensor(resolutions).reshape(-1).tolist()]
@@ -429,7 +432,8 @@ class HashGridInterpolate(torch.autograd.Function):
         table = A.f32c(codebook.detach())
         desc = A.make_grid_desc(table, res, begin, 2 ** codebook_bitwidth)
         feats = torch.empty((c.shape[0], len(res) * table.shape[1]), dtype=torch.float32, device=c.device)
-        A.check(A.lib().wb_hashgrid_fwd(A.ptr(c), C.c_int64(c.shape[0]), C.byref(desc), A.ptr(feats), A.stream()))
+        fwd = A.lib().wb_hashgrid_fwd if dim == 3 else A.lib().wb_hashgrid2d_fwd
+        A.check(fwd(A.ptr(c), C.c_int64(c.shape[0]), C.byref(desc), A.ptr(feats), A.stream()))
         ctx.save_for_backward(c, table)
         ctx.meta = (res, begin, codebook_bitwidth)
         return feats
@@ -441,7 +445,8 @@ class HashGridInterpolate(torch.autograd.Function):
         desc = A.make_grid_desc(table, res, begin, 2 ** bw)
         g = A.f32c(grad_output)
         gt = torch.zeros_like(table)                      # hashgrid_interpolate.cpp:85
-        A.check(A.lib().wb_hashgrid_bwd(A.ptr(c), C.c_int64(c.shape[0]), C.byref(desc), A.ptr(g), A.ptr(gt), A.stream()))
+        bwd = A.lib().wb_hashgrid_bwd if c.shape[-1] == 3 else A.lib().wb_hashgrid2d_bwd
+        A.check(bwd(A.ptr(c), C.c_int64(c.shape[0]), C.byref(desc), A.ptr(g), A.ptr(gt), A.stream()))
         return None, None, None, None, gt, None
 
 
@@ -452,6 +457,85 @@ def hashgrid(coords, codebook_bitwidth, lod_idx, codebook):
                                       codebook.feats, codebook.begin_idxes)
     feature_dim = codebook.feats.shape[1] * len(codebook.resolutions)
     return feats.reshape(batch, feature_dim)
+
+
+# --------------------------------------------------------------------------------------------------------------
+# ImageNeuralField (app/image): wb_image_eval / wb_image_train
+# --------------------------------------------------------------------------------------------------------------
+IMAGE_BANDS = (1.0, 2.0, 4.0)          # get_positional_embedder(frequencies=3): 2^linspace(0, 2, 3)
+
+
+def image_field(nef):
+    """(grid desc, hidden_dim, decoder pointers, keepalive) of an ImageNeuralField for wb_image_eval / wb_image_train, or None when the
+    kernels do not take the field: a grid other than a hash grid of 2, 4 or 8 features per LOD, a decoder other than one relu hidden
+    layer (a multiple of 4 up to 128 wide) with biases and 3 outputs, an embedder other than the reference's 3-band one with input, a
+    decoder input wider than the kernels' shared-memory image allows, or parameters that are not contiguous fp32 on the device.
+    The decoder pointers are a host array [W0, b0, Wout, bout] aimed at the parameters themselves: no copy, no launch."""
+    grid, dec, emb = getattr(nef, "grid", None), getattr(nef, "decoder", None), getattr(nef, "embedder", None)
+    cb = getattr(grid, "codebook", None)
+    if grid is None or dec is None or emb is None or not hasattr(cb, "feats") or not hasattr(cb, "begin_idxes"):
+        return None
+    if getattr(grid, "multiscale_type", None) not in ("cat", "sum") or getattr(dec, "activation", None) is not torch.relu:
+        return None
+    layers = list(getattr(dec, "layers", []))
+    if len(layers) != 1 or getattr(dec, "skip", []) or any(type(l) is not torch.nn.Linear or l.bias is None for l in layers + [dec.lout]):
+        return None
+    bands = getattr(emb, "bands", None)
+    if (not getattr(emb, "include_input", False) or not torch.is_tensor(bands) or bands.numel() != 3
+            or [float(b) for b in bands.detach().reshape(-1).tolist()] != list(IMAGE_BANDS)):
+        return None
+    F, L = int(cb.feats.shape[1]), len(grid.resolutions)
+    fw = F * L if grid.multiscale_type == "cat" else F
+    H = int(layers[0].out_features)
+    if layers[0].in_features != fw + 14 or dec.lout.out_features != 3:
+        return None
+    params = decoder_params(dec)
+    table = cb.feats
+    if any(not p.is_cuda or p.dtype != torch.float32 or not p.is_contiguous() for p in params + [table]):
+        return None
+    res = [int(r) for r in torch.as_tensor(grid.resolutions).reshape(-1).tolist()]
+    desc = A.make_grid_desc(table.data, res, [int(b) for b in cb.begin_idxes.tolist()], 2 ** int(grid.codebook_bitwidth), grid.multiscale_type)
+    if A.lib().wb_image_smem_bytes(C.byref(desc), C.c_int32(H), C.c_int32(1)) < 0:
+        return None
+    ptrs = (C.c_void_p * 4)(*[p.data_ptr() for p in params])
+    return desc, H, ptrs, [table] + params
+
+
+def image_eval(nef, coords: torch.Tensor, lod_idx: int) -> Optional[torch.Tensor]:
+    """ImageNeuralField.rgb in one launch (wb_image_eval): rgb [N, 3], or None when image_field declines the field."""
+    fd = image_field(nef)
+    if fd is None:
+        return None
+    desc, H, params, _ = fd
+    A.require_device(coords)
+    c = A.f32c(coords)
+    rgb = torch.empty((c.shape[0], 3), dtype=torch.float32, device=c.device)
+    A.check(A.lib().wb_image_eval(C.byref(desc), C.c_int32(H), params, C.c_int32(lod_idx), A.ptr(c), C.c_int64(c.shape[0]), A.ptr(rgb), A.stream()))
+    return rgb
+
+
+def image_rgb(nef, coords: torch.Tensor, lod=None) -> Optional[torch.Tensor]:
+    """ImageNeuralField.rgb's native route: rgb [N, 3] from image_eval for a non-empty [N, 2] CUDA batch outside autograd and
+    autocast (the trainer's validate() over 1 M-pixel chunks, render_final_view); None otherwise or when the kernel declines the field."""
+    if (coords.dim() != 2 or coords.shape[-1] != 2 or coords.shape[0] == 0 or not coords.is_cuda or torch.is_grad_enabled()
+            or torch.is_autocast_enabled()):
+        return None
+    return image_eval(nef, coords, len(nef.grid.resolutions) - 1 if lod is None else int(lod))
+
+
+def image_train(fd, coords: torch.Tensor, rgb_gt: torch.Tensor, lod_idx: int, grad_table: torch.Tensor, grad_params: torch.Tensor,
+                loss_out: torch.Tensor) -> None:
+    """Forward, F.mse_loss and backward of ImageTrainer.step in one launch (wb_image_train) for fd = image_field(nef); coords f32 [N, 2],
+    rgb_gt f32 [N, 3] on the device.  Accumulates loss_out[0] += mean (y - gt)^2, grad_table (codebook.feats) and grad_params
+    (packed [W0, b0, Wout, bout])."""
+    desc, H, params, _ = fd
+    A.require_device(coords)
+    N = int(coords.shape[0])
+    if N == 0:
+        raise A.WispB200Error("image_train: empty batch (the reference's mse_loss averages over it)")
+    c, g = A.f32c(coords), A.f32c(rgb_gt)
+    A.check(A.lib().wb_image_train(C.byref(desc), C.c_int32(H), params, C.c_int32(lod_idx), A.ptr(c), A.ptr(g), C.c_int64(N),
+                                   C.c_float(1.0 / (3.0 * N)), A.ptr(grad_table), A.ptr(grad_params), A.ptr(loss_out), A.stream()))
 
 
 # --------------------------------------------------------------------------------------------------------------

@@ -1,4 +1,6 @@
-"""MultiviewStep: the optimisation step of wisp.trainers.MultiviewTrainer (wisp/trainers/multiview_trainer.py:111-180) with the
+"""MultiviewStep (below), SDFStep and ImageStep (at the end): the trainers' steps as native sequences.
+
+MultiviewStep: the optimisation step of wisp.trainers.MultiviewTrainer (wisp/trainers/multiview_trainer.py:111-180) with the
 optimiser set-up of BaseTrainer.init_optimizer (wisp/trainers/base_trainer.py:205-235), as ONE native sequence without autograd:
 
     march (count / scan / fill; pre-marched on a side stream when the next batch is known)
@@ -457,3 +459,106 @@ class SDFStep:
             grads = [(p.grad if p.grad is not None else torch.zeros_like(p)).contiguous() for p in self.params]
             self.opt.step(grads, grad_scale=1.0, zero_grad=False)
         return loss.detach()
+
+
+class ImageStep:
+    """The optimisation step of wisp.trainers.ImageTrainer (wisp/trainers/image_trainer.py:51-80): loss = F.mse_loss(nef.rgb(coords),
+    rgb), the mean over N * 3, one optimiser step, then the MultiStepLR step of `scheduler: True`.  Parameter groups of
+    BaseTrainer.init_optimizer (base_trainer.py:205-246): 'decoder' -> lr and weight_decay, 'grid' -> lr * grid_lr_weight, the rest -> lr;
+    parameters with requires_grad=False (embedder.bands) are skipped.
+
+    An ImageNeuralField over a hash grid of 2, 4 or 8 features per LOD with one hidden layer (image_hash.yaml) trains natively in two
+    launches per step: wb_image_train (forward, loss and backward, no autograd) and the optimiser (wb_adamw_step by default: apex
+    FusedAdam's adam_w_mode), which also clears the gradients and applies the schedule's factor.  The decoder's parameters are flattened
+    in place into one buffer [W0, b0, Wout, bout], which the kernels read, whose gradient wb_image_train writes and which is one
+    optimiser segment; grid.codebook.feats is the other.  Every other field (deeper decoders, other grids or embedders, a decoder input
+    wider than the kernel's shared-memory image: ops.image_field is None) takes autograd plus the same native optimiser.
+
+    `precision`: 0 fp32 (the native route above); 1 the reference's enable_amp arithmetic, which runs the autograd route inside
+    torch.autocast("cuda", torch.float16) (no tensor-core image kernel) with the same native optimiser and no GradScaler.
+    `optimizer`: "adamw" (FusedAdam), "adam" or "rmsprop".
+    `scheduler_milestones` / `scheduler_gamma`: MultiStepLR stepped after every optimiser step, as MultiviewStep takes them: iteration
+    numbers; step t (1-based) runs at lr * gamma^k, k = the number of milestones <= t - 1.  The reference hands MultiStepLR
+    max_steps * (0.5, 0.75, 0.9), which fire only where that product is integer-valued.  `fused` tells which route was chosen."""
+
+    def __init__(self, pipeline, lr: float = 1e-3, eps: float = 1e-15, weight_decay: float = 0.0, grid_lr_weight: float = 1.0,
+                 betas=(0.9, 0.999), optimizer: str = "adamw", scheduler_milestones=(), scheduler_gamma: float = 0.333, precision: int = 0):
+        if precision not in (0, 1) or isinstance(precision, bool):
+            raise ValueError(f"ImageStep: precision must be 0 (fp32) or 1 (fp16 autocast arithmetic), got {precision!r}")
+        self.precision = int(precision)
+        self.pipeline, self.nef = pipeline, pipeline.nef
+        nef = self.nef
+        named = [(k, p) for k, p in nef.named_parameters() if p.requires_grad]
+        if not named:
+            raise A.WispB200Error("ImageStep: the field has no trainable parameters")
+        A.require_device(named[0][1])                                         # no CPU fallback
+        self.device = named[0][1].device
+        self.fd = self._fused_field(nef, [p for _, p in named]) if self.precision == 0 else None
+        self.fused = self.fd is not None
+        if self.fused:
+            table = nef.grid.codebook.feats
+            tensors = [(table.data, lr * grid_lr_weight, 0.0), (self.dec_flat, lr, weight_decay)]
+            self.g_table = torch.zeros_like(table.data)
+            self.g_dec = torch.zeros_like(self.dec_flat)
+        else:
+            tensors = [(p.data, lr if "decoder" in k or "grid" not in k else lr * grid_lr_weight, weight_decay if "decoder" in k else 0.0)
+                       for k, p in named]
+            self.params = [p for _, p in named]
+        self.opt = _make_optimizer(optimizer, tensors, betas, eps, 0.99, 0.0)
+        self.milestones, self.gamma = [int(m) for m in scheduler_milestones], float(scheduler_gamma)
+        if any(m != f for m, f in zip(self.milestones, scheduler_milestones)):
+            raise ValueError(f"scheduler_milestones are iteration numbers (ints), got {scheduler_milestones!r}")
+
+    def _fused_field(self, nef, params):
+        """ops.image_field of the field with the decoder flattened in place, or None when wb_image_train does not take the field or the
+        field has trainable parameters beyond codebook.feats and the decoder."""
+        if ops.image_field(nef) is None:
+            return None
+        dparams = ops.decoder_params(nef.decoder)
+        if {id(p) for p in params} != {id(p) for p in [nef.grid.codebook.feats] + dparams}:
+            return None
+        self.dec_flat = _flatten_in_place(dparams)
+        fd = ops.image_field(nef)
+        if fd is None or fd[2][0] != self.dec_flat.data_ptr():
+            return None
+        return fd
+
+    def step(self, coords: torch.Tensor, rgb: torch.Tensor, zero_grad: bool = True, update: bool = True) -> torch.Tensor:
+        """One optimisation step on (coords [N, 2], rgb [N, 3]); returns the loss as a device scalar (no host sync).  Host tensors are
+        copied to the device (image_trainer.py:53-54).  `update=False` stops after the backward: the gradients stay in g_table / g_dec
+        (autograd route: in the parameters' .grad), parameters, optimiser state and schedule untouched."""
+        pts, gts = coords.to(self.device), rgb.to(self.device)
+        if int(pts.shape[0]) == 0:
+            raise A.WispB200Error("ImageStep.step: empty batch (mse_loss averages over it)")
+        if not self.fused:
+            return self._step_autograd(pts, gts, update)
+        loss = torch.zeros(1, dtype=torch.float32, device=self.device)
+        ops.image_train(self.fd, A.f32c(pts).reshape(-1, 2), A.f32c(gts).reshape(-1, 3), len(self.nef.grid.resolutions) - 1,
+                        self.g_table, self.g_dec, loss)
+        if update:
+            self.opt.lr_scale = multistep_factor(self.milestones, self.gamma, self.opt.t + 1)
+            with ops._stage("adam"):
+                self.opt.step([self.g_table, self.g_dec], grad_scale=1.0, zero_grad=zero_grad)
+        return loss[0]
+
+    def zero_grads(self) -> None:
+        """Clear every gradient accumulator (after a step(update=False) whose gradients were only inspected)."""
+        if self.fused:
+            self.g_table.zero_()
+            self.g_dec.zero_()
+        else:
+            for p in self.params:
+                p.grad = None
+
+    def _step_autograd(self, pts, gts, update):
+        for p in self.params:
+            p.grad = None                                                     # self.optimizer.zero_grad() (:61)
+        amp = torch.autocast("cuda", torch.float16) if self.precision == 1 else contextlib.nullcontext()
+        with amp:                                                             # image_trainer.py:64 with enable_amp
+            loss = torch.nn.functional.mse_loss(self.nef.rgb(pts), gts)
+        loss.backward()
+        if update:
+            grads = [(p.grad if p.grad is not None else torch.zeros_like(p)).float().contiguous() for p in self.params]
+            self.opt.lr_scale = multistep_factor(self.milestones, self.gamma, self.opt.t + 1)
+            self.opt.step(grads, grad_scale=1.0, zero_grad=False)
+        return loss.detach().float()
