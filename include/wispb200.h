@@ -513,6 +513,17 @@ int wb_image_train(const wb_nef_desc* grid, int32_t hidden_dim, const float* con
  * kernel does not take it (the reason in wb_last_error()).  Host only: no device is touched. */
 int64_t wb_image_smem_bytes(const wb_nef_desc* grid, int32_t hidden_dim, int32_t train);
 
+/* ------------------------------------------------------------------------------------------------
+ * PackedSPCTracer.trace (wisp/tracers/packed_spc_tracer.py:50-90) over SPCField: the first nugget of every ray at `level`
+ * (the nugget of wb_raytrace_fill: the cell of `level` whose slab interval is first in front of the origin), in ONE launch.
+ * A hit writes depth[r] = its entry depth (the first depth[2 * offsets[r]] of wb_raytrace_fill), hit[r] = 1,
+ * rgb[3r..3r+2] = colors[(pidx - point_offset) * color_stride + 0..2] (pidx: the cell's point index) and alpha[r] = 1;
+ * a miss writes 0 to all four.  colors: f32, color_stride >= 3; the caller keeps pidx - point_offset inside the colour rows
+ * (SPCField: point_offset = pyramid[1, max_level] and level = max_level).  depth / alpha f32 [R], hit uint8 [R], rgb f32 [R, 3].
+ * level <= 15 and <= oct->max_level.  R = 0 launches nothing. */
+int wb_spc_trace(const wb_octree* oct, int32_t level, const wb_rays* rays, const float* colors, int64_t color_stride, int64_t point_offset,
+                 float* depth, uint8_t* hit, float* rgb, float* alpha, wb_stream s);
+
 #ifdef __cplusplus
 }
 #endif

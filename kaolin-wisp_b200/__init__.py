@@ -9,8 +9,8 @@ from ._cabi import WispB200Error                                                
 from .core import Rays, RenderBuffer                                            # noqa: F401
 from .accelstructs import OctreeAS, AxisAlignedBBoxAS, ASQueryResults, ASRaymarchResults, ASRaytraceResults   # noqa: F401
 from .grids import HashGrid, MultiTable, TriplanarGrid, TriplanarFeatureVolume, OctreeGrid, CodebookOctreeGrid                                         # noqa: F401
-from .nefs import NeuralRadianceField, NeuralSDF, ImageNeuralField, BasicDecoder, PositionalEmbedder, get_positional_embedder   # noqa: F401
-from .tracers import PackedRFTracer, PackedSDFTracer                                             # noqa: F401
+from .nefs import NeuralRadianceField, NeuralSDF, ImageNeuralField, SPCField, BasicDecoder, PositionalEmbedder, get_positional_embedder   # noqa: F401
+from .tracers import PackedRFTracer, PackedSDFTracer, PackedSPCTracer                                             # noqa: F401
 from .pipeline import Pipeline                                                  # noqa: F401
 from . import trainers                                                          # noqa: F401
 from .trainers import ImageStep, MultiviewStep, NativeAdam, NativeAdamW, NativeRMSprop, SDFStep   # noqa: F401

@@ -90,7 +90,12 @@ EXPORTS = [
     "wb_octree_interp_fwd", "wb_octree_interp_bwd", "wb_find_depth_bound", "wb_sdf_eval", "wb_sdf_train", "wb_sdf_train_smem_bytes", "wb_sdf_train_tc", "wb_sdf_train_tc_smem_bytes", "wb_sdf_trace", "wb_sdf_phase", "wb_composite_fwd", "wb_composite_bwd",
     "wb_rf_march_fill", "wb_rf_param_blob_floats", "wb_rf_precision_supported", "wb_rf_pack_params", "wb_rf_shade_fwd", "wb_rf_shade_bwd",
     "wb_rf_workspace_bytes", "wb_rf_feat_bytes", "wb_rf_decoder_bwd", "wb_rf_table_scatter", "wb_rf_loss_scale", "wb_rf_workspace_holds_ray_rows", "wb_prune_samples", "wb_prune_update", "wb_raygen_lookat", "wb_raygen_pinhole", "wb_codebook_rows_fwd", "wb_codebook_rows_bwd", "wb_composite_bwd_loss", "wb_adam_step", "wb_adamw_step", "wb_rmsprop_step", "wb_tc_selftest",
+    "wb_spc_trace",
 ]
+
+# wb_spc_trace(oct, level, rays, colors, color_stride, point_offset, depth, hit, rgb, alpha, stream) -> int
+SPC_TRACE_ARGTYPES = [C.POINTER(OctreeDesc), C.c_int32, C.POINTER(RaysDesc), C.c_void_p, C.c_int64, C.c_int64,
+                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
 
 _lib: Optional[C.CDLL] = None
 _checked_devices = set()
@@ -122,6 +127,7 @@ def lib() -> C.CDLL:
         L.wb_sdf_train_smem_bytes.restype = C.c_int64
         L.wb_sdf_train_tc_smem_bytes.restype = C.c_int64
         L.wb_image_smem_bytes.restype = C.c_int64
+        L.wb_spc_trace.restype, L.wb_spc_trace.argtypes = C.c_int, SPC_TRACE_ARGTYPES
         _lib = L
     return _lib
 

@@ -242,3 +242,61 @@ extern "C" int wb_raymarch_uniform_fill(const wb_rays* rays, const int32_t* nug_
     WB_LAUNCH_CHECK();
     return WB_OK;
 }
+
+// ---- PackedSPCTracer.trace: the first nugget of every ray (packed_spc_tracer.py:50-90) -----------------------------------
+// wb_raytrace_kernel's walk (same stack, same i ^ mask child order, same wb_slab nugget) stopped at the first cell of `level`:
+// the walk visits a ray's nuggets front to back, so that cell is the nugget the reference keeps after mark_pack_boundaries.
+// One launch replaces count + scan + fill + the first-hit selection, and no nugget list is written.
+__global__ void __launch_bounds__(128)
+wb_spc_trace_kernel(WbOct oc, const float* __restrict__ origins, const float* __restrict__ dirs, int64_t R,
+                    const float* __restrict__ colors, int64_t color_stride, int64_t point_offset,
+                    float* __restrict__ depth, uint8_t* __restrict__ hit, float* __restrict__ rgb, float* __restrict__ alpha)
+{
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= R) return;
+    const float o[3] = { origins[3 * r], origins[3 * r + 1], origins[3 * r + 2] };
+    const float d[3] = { dirs[3 * r], dirs[3 * r + 1], dirs[3 * r + 2] };
+    const int mask = (d[0] < 0.0f ? 4 : 0) | (d[1] < 0.0f ? 2 : 0) | (d[2] < 0.0f ? 1 : 0);
+    int32_t st_node[7 * 15 + 2]; uint64_t st_cell[7 * 15 + 2];
+    int sp = 1; st_node[0] = 0; st_cell[0] = 0;
+    while (sp > 0) {
+        --sp;
+        const int32_t node = st_node[sp]; const uint64_t cell = st_cell[sp];
+        const int l = (int)(cell >> 48), cx = (int)((cell >> 32) & 0xffff), cy = (int)((cell >> 16) & 0xffff), cz = (int)(cell & 0xffff);
+        float t0, t1;
+        if (!wb_slab(o, d, cx, cy, cz, l, t0, t1)) continue;
+        if (l == oc.level) {
+            const float* c = colors + ((int64_t)node - point_offset) * color_stride;
+            depth[r] = t0; hit[r] = 1; alpha[r] = 1.0f;
+            rgb[3 * r] = __ldg(c); rgb[3 * r + 1] = __ldg(c + 1); rgb[3 * r + 2] = __ldg(c + 2);
+            return;
+        }
+        const uint32_t bits = __ldg(oc.octree + node);
+        const int32_t base = __ldg(oc.prefix + node);
+        for (int i = 7; i >= 0; --i) {
+            const int c = i ^ mask;
+            if (!(bits & (1u << c))) continue;
+            st_node[sp] = base + __popc(bits & ((2u << c) - 1u));
+            st_cell[sp] = ((uint64_t)(l + 1) << 48) | ((uint64_t)(2 * cx + ((c >> 2) & 1)) << 32) | ((uint64_t)(2 * cy + ((c >> 1) & 1)) << 16) | (uint64_t)(2 * cz + (c & 1));
+            ++sp;
+        }
+    }
+    depth[r] = 0.0f; hit[r] = 0; alpha[r] = 0.0f;                 // miss: the reference's zero-initialised buffers (:76-83)
+    rgb[3 * r] = 0.0f; rgb[3 * r + 1] = 0.0f; rgb[3 * r + 2] = 0.0f;
+}
+
+extern "C" int wb_spc_trace(const wb_octree* oct, int32_t level, const wb_rays* rays, const float* colors, int64_t color_stride, int64_t point_offset,
+                            float* depth, uint8_t* hit, float* rgb, float* alpha, wb_stream s)
+{
+    WbOct o; int rc = wb_make_oct(oct, level, &o); if (rc) return rc;
+    WB_CHECK_ARG(rays != nullptr, "null rays");
+    const int64_t R = rays->num_rays;
+    WB_CHECK_ARG(R >= 0 && R < ((int64_t)1 << 31) * 128, "num_rays out of range");
+    if (R == 0) return WB_OK;
+    WB_CHECK_ARG(rays->origins && rays->dirs && colors && depth && hit && rgb && alpha, "null pointer");
+    WB_CHECK_ARG(color_stride >= 3 && point_offset >= 0, "color_stride must be >= 3 and point_offset >= 0");
+    wb_spc_trace_kernel<<<(unsigned)((R + 127) / 128), 128, 0, (cudaStream_t)s>>>(o, rays->origins, rays->dirs, R, colors, color_stride, point_offset,
+                                                                                 depth, hit, rgb, alpha);
+    WB_LAUNCH_CHECK();
+    return WB_OK;
+}

@@ -9,12 +9,14 @@ What is patched (reference file:line -> native replacement):
   OctreeGrid.interpolate                        (octree_grid.py:165-219)           wb_octree_interp_*
   PackedRFTracer.trace                          (packed_rf_tracer.py:84-181)       fused render path (ops.rf_trace)
   PackedSDFTracer.trace                         (packed_sdf_tracer.py:57-174)      wb_sdf_trace
+  PackedSPCTracer.trace                         (packed_spc_tracer.py:37-90)       wb_spc_trace (torch + OctreeAS.raytrace below max_level)
   NeuralSDF.sdf (no-grad)                       (neural_sdf.py:120-155)            wb_sdf_eval
   ImageNeuralField.rgb (no-grad)                (image_nef.py:77-97)               wb_image_eval
   NeuralRadianceField.prune                     (nerf.py:175-212)                  ops.prune_field
 Every replacement keeps the reference signature, falls back to the original method for configurations outside the native
 path (unknown embedders, activations, grids), and keeps the attributes other wisp code reads (`prev_num_samples`, `bg_color`).
-The grid and SDF-tracer replacements run the methods of this package's mirror classes (grids.py, tracers.py); the rest share
+SPCField itself is not patched: its Kaolin calls build the octree (like OctreeAS's constructor) and its rgba() is plain torch.
+The grid, SDF- and SPC-tracer replacements run the methods of this package's mirror classes (grids.py, tracers.py); the rest share
 their host logic with the mirrors through ops (octree_tensors, march, resolve_precision, sdf_channel, image_rgb).
 ImageTrainer.step itself is not patched: wisp_b200.ImageStep is its native counterpart (INTEGRATION.md).
 """
@@ -59,7 +61,7 @@ def install() -> bool:
         from wisp.core import RenderBuffer
         from wisp.models.grids import HashGrid, OctreeGrid, TriplanarGrid
         from wisp.models.nefs import NeuralRadianceField, NeuralSDF
-        from wisp.tracers import PackedRFTracer, PackedSDFTracer
+        from wisp.tracers import PackedRFTracer, PackedSDFTracer, PackedSPCTracer
     except Exception:          # wisp (or one of its dependencies) is not importable here
         return False
 
@@ -143,6 +145,13 @@ def install() -> bool:
         return ops.sdf_channel(self, coords, lod_idx) or orig_sdf(self, coords, lod_idx)
 
     _patch(NeuralSDF, "sdf", sdf)
+
+    # ---- SPC tracer (no Kaolin: mark_pack_boundaries is torch in the mirror's body) ------------------------------------------
+    def spc_trace(self, nef, rays, channels, extra_channels, lod_idx=None):
+        rb = tracers.PackedSPCTracer.trace(self, nef, rays, channels, extra_channels, lod_idx)
+        return RenderBuffer(depth=rb.depth, hit=rb.hit, rgb=rb.rgb, alpha=rb.alpha)
+
+    _patch(PackedSPCTracer, "trace", spc_trace)
 
     # ---- image field (app/image; a wisp without it keeps every other patch) ---------------------------------------
     try:

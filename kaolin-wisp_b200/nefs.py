@@ -4,6 +4,7 @@
   wisp.models.decoders.BasicDecoder      (wisp/models/decoders/basic_decoders.py:16-101)
   wisp.models.embedders.PositionalEmbedder / get_positional_embedder (positional_embedder.py:15-100)
   wisp.models.nefs.ImageNeuralField      (wisp/models/nefs/image_nef.py:37-97)
+  wisp.models.nefs.SPCField              (wisp/models/nefs/spc_field.py:19-157)
 Module / parameter names are the reference's (decoder_density.layers.N.weight, decoder_color.lout.bias,
 grid.codebook.feats ...).  `rgba()` is the unfused route (our hash-grid kernel + torch Linear); the tracer uses
 `fused_spec()` to hand the whole field to the fused native pipeline instead.
@@ -17,7 +18,9 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import ops, spc
+from .accelstructs import OctreeAS
+from .grids import OctreeGrid
 
 
 class PositionalEmbedder(nn.Module):
@@ -308,3 +311,48 @@ class ImageNeuralField(BaseNeuralField):
         embedded_pos = self.embedder(coords).view(batch, self.embed_dim)
         fpos = torch.cat([feats, embedded_pos], dim=-1)
         return torch.sigmoid(self.decoder(fpos))
+
+
+class SPCField(BaseNeuralField):
+    """wisp.models.nefs.SPCField (spc_field.py:19-157): an SPC rendered with its own per-point colours, no embedder or decoder.
+    PackedSPCTracer renders it in one launch (ops.spc_trace) from the f32 [M, 3] rows of ops.spc_colors."""
+
+    def __init__(self, spc_octree: torch.Tensor, features_dict=None, device='cuda'):
+        super().__init__()
+        self.spc_octree = spc_octree
+        self.features_dict = features_dict if features_dict is not None else dict()
+        self.spc_device = device
+        self.grid = None
+        self.colors = None
+        self.normals = None
+        self.init_grid(spc_octree)
+
+    def init_grid(self, spc_octree: torch.Tensor):
+        """spc_field.py:69-114: RGBA colours / 255, else 0.5 * (normals + 1), else the finest level's point coordinates / 2^level
+        (each with the reference's dtype promotion)."""
+        if "colors" in self.features_dict:
+            self.colors = self.features_dict["colors"].reshape(-1, 4) / 255.0
+        if "normals" in self.features_dict:
+            self.normals = self.features_dict["normals"].reshape(-1, 3)
+        if self.colors is None:
+            if self.normals is not None:
+                colors = 0.5 * (self.normals + 1.0)
+            else:
+                level, pyramid, _ = spc.scan_octree(spc_octree)
+                colors = spc.generate_points(spc_octree, pyramid)[int(pyramid[1, level]):]
+                colors = colors / np.power(2, level)
+            self.colors = colors
+        self.grid = OctreeGrid(OctreeAS(spc_octree), feature_dim=3, num_lods=0)
+
+    @property
+    def device(self):
+        return self.spc_device
+
+    def register_forward_functions(self):
+        self._register_forward_function(self.rgba, ["rgb"])
+
+    def rgba(self, ridx_hit=None):
+        """spc_field.py:130-147: colours of point-hierarchy indices, made relative to the finest level -> rgb [batch, 1, 3]."""
+        level = self.grid.blas.max_level
+        offset = self.grid.blas.pyramid[1, level]
+        return dict(rgb=self.colors[ridx_hit - offset, :3].unsqueeze(1))

@@ -11,6 +11,7 @@ from typing import List, Optional, Sequence
 import torch
 
 from . import _cabi as A
+from .core import RenderBuffer
 
 # Optional per-stage device timing (bench.py): when PROFILE is a list, every native stage appends
 # (name, start_event, end_event) recorded on the launching (current torch) stream.
@@ -345,6 +346,45 @@ def raytrace(oct: OctreeTensors, origins, dirs, level: int):
             else:
                 A.check(L.wb_raytrace_fill(C.byref(od), C.c_int32(level), C.byref(rays), A.ptr(offsets), A.ptr(ridx), A.ptr(pidx), A.ptr(depth), A.stream()))
     return ridx, pidx, depth, offsets
+
+
+def spc_trace(oct: OctreeTensors, origins, dirs, level: int, colors: torch.Tensor, point_offset: int):
+    """PackedSPCTracer.trace (packed_spc_tracer.py:50-90) in one launch (wb_spc_trace): the first nugget of every ray at `level`
+    -> RenderBuffer(depth f32 [R, 1], hit bool [R], rgb f32 [R, 3], alpha f32 [R, 1]), rgb = colors[pidx - point_offset, :3].
+    colors: f32 [M, >= 3] with unit column stride on the rays' device, holding a row for every point of `level`."""
+    A.require_device(origins)
+    first, cnt = int(oct.pyramid[1, level]), int(oct.pyramid[0, level])
+    if (colors.dtype != torch.float32 or colors.dim() != 2 or colors.shape[1] < 3 or colors.stride(1) != 1 or colors.device != origins.device
+            or not 0 <= point_offset <= first or first + cnt - point_offset > colors.shape[0]):
+        raise A.WispB200Error(f"spc_trace: colors must be f32 [M >= {first + cnt - point_offset}, >= 3] with unit column stride on "
+                              f"{origins.device} and 0 <= point_offset <= {first}; got {tuple(colors.shape)} {colors.dtype} on {colors.device}, "
+                              f"point_offset {point_offset}")
+    rays, keep = A.make_rays(origins, dirs, 0.0, 0.0)
+    R, dev = rays.num_rays, origins.device
+    depth = torch.empty((R, 1), dtype=torch.float32, device=dev)
+    hit = torch.empty(R, dtype=torch.bool, device=dev)
+    rgb = torch.empty((R, 3), dtype=torch.float32, device=dev)
+    alpha = torch.empty((R, 1), dtype=torch.float32, device=dev)
+    od = oct.desc()
+    with _stage("spc_trace"):
+        A.check(A.lib().wb_spc_trace(C.byref(od), level, C.byref(rays), A.ptr(colors), colors.stride(0), point_offset,
+                                     A.ptr(depth), A.ptr(hit), A.ptr(rgb), A.ptr(alpha), A.stream()))
+    return RenderBuffer(depth=depth, hit=hit, rgb=rgb, alpha=alpha)
+
+
+def spc_colors(nef) -> Optional[torch.Tensor]:
+    """The f32 [M, 3] rows SPCField.rgba gathers (spc_field.py:130-147: colors[:, :3]) as a view of the field's colours, made once per
+    colour tensor and kept on the field; None unless the colours are an f32 [M, >= 3] CUDA tensor (the reference's tracer writes
+    them into an f32 buffer with an index put, which refuses any other dtype: packed_spc_tracer.py:87)."""
+    src = getattr(nef, "colors", None)
+    if not torch.is_tensor(src) or not src.is_cuda or src.dtype != torch.float32 or src.dim() != 2 or src.shape[1] < 3:
+        return None
+    cached = getattr(nef, "_wb_spc_colors", None)
+    if cached is None or cached[0] is not src or cached[1] != src._version:
+        view = src.detach()[:, :3]
+        cached = (src, src._version, view if view.stride(1) == 1 else view.contiguous())
+        nef._wb_spc_colors = cached
+    return cached[2]
 
 
 def uniform_scale(num_samples: int) -> int:

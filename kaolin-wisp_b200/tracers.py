@@ -1,8 +1,8 @@
-"""PackedRFTracer / PackedSDFTracer: host-side mirrors of wisp.tracers.PackedRFTracer (wisp/tracers/packed_rf_tracer.py:20-181),
-wisp.tracers.PackedSDFTracer (wisp/tracers/packed_sdf_tracer.py:20-174) and wisp.tracers.BaseTracer.forward
+"""PackedRFTracer / PackedSDFTracer / PackedSPCTracer: host-side mirrors of wisp.tracers.PackedRFTracer (wisp/tracers/packed_rf_tracer.py:20-181),
+wisp.tracers.PackedSDFTracer (wisp/tracers/packed_sdf_tracer.py:20-174), wisp.tracers.PackedSPCTracer (packed_spc_tracer.py:7-90) and wisp.tracers.BaseTracer.forward
 (wisp/tracers/base_tracer.py:99-162).  PackedRFTracer.trace() runs the fused native pipeline when the neural field is a
 NeuralRadianceField(HashGrid) with the 'ray' sampler, and otherwise the unfused route (native raymarch + nef forward + native
-compositing)."""
+compositing).  PackedSPCTracer.trace renders an SPCField in one first-hit launch."""
 from __future__ import annotations
 
 import inspect
@@ -201,3 +201,48 @@ class PackedSDFTracer(BaseTracer):
             buf[hit] = feats.to(buf.dtype)
             extra_outputs[channel] = buf
         return RenderBuffer(xyz=out["xyz"], depth=out["depth"], hit=hit, normal=out["normal"], rgb=out["rgb"], alpha=out["alpha"], **extra_outputs)
+
+
+class PackedSPCTracer(BaseTracer):
+    """wisp.tracers.PackedSPCTracer (packed_spc_tracer.py:7-90): every ray takes the colour of the first SPC cell it crosses.
+    At the finest level with the field's colours on the device this is ONE launch (ops.spc_trace -> wb_spc_trace); otherwise the
+    reference body runs over OctreeAS.raytrace with torch in place of Kaolin's mark_pack_boundaries."""
+
+    def __init__(self):
+        super().__init__()
+        self.bg_color = (0.0, 0.0, 0.0)
+
+    def get_supported_channels(self):
+        return {"depth", "hit", "rgb", "alpha"}
+
+    def get_required_nef_channels(self):
+        return {"rgb"}
+
+    def trace(self, nef, rays, channels, extra_channels, lod_idx=None):
+        """packed_spc_tracer.py:37-90; lod_idx is an octree level (None: the finest).  install() runs this body on the reference's
+        PackedSPCTracer too."""
+        blas = nef.grid.blas
+        colors = ops.spc_colors(nef) if lod_idx is None or lod_idx == blas.max_level else None
+        if colors is not None:
+            return ops.spc_trace(ops.octree_tensors(blas), rays.origins, rays.dirs, blas.max_level, colors, int(blas.pyramid[1, blas.max_level]))
+        N = rays.origins.shape[0]
+        if lod_idx is None:
+            lod_idx = blas.max_level
+        rt = blas.raytrace(rays, lod_idx, with_exit=False)
+        ridx, pidx, depths = rt.ridx, rt.pidx, rt.depth
+        first = torch.ones_like(ridx, dtype=torch.bool)                    # mark_pack_boundaries
+        first[1:] = ridx[1:] != ridx[:-1]
+        first_hits_point, first_hits_ray, first_hits_depth = pidx[first], ridx[first], depths[first]
+        color = nef(ridx_hit=first_hits_point.long(), channels="rgb")
+        ray_colors = color.squeeze(1)
+        depth = torch.zeros(N, 1, device=first_hits_depth.device)
+        depth[first_hits_ray.long(), :] = first_hits_depth
+        alpha = torch.ones([color.shape[0], 1], device=color.device)
+        hit = torch.zeros(N, device=color.device).bool()
+        rgb = torch.zeros(N, 3, device=color.device)
+        out_alpha = torch.zeros(N, 1, device=color.device)
+        color = alpha * ray_colors
+        hit[first_hits_ray.long()] = alpha[..., 0] > 0.0
+        rgb[first_hits_ray.long(), :3] = color
+        out_alpha[first_hits_ray.long()] = alpha
+        return RenderBuffer(depth=depth, hit=hit, rgb=rgb, alpha=out_alpha)
