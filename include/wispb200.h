@@ -524,6 +524,22 @@ int64_t wb_image_smem_bytes(const wb_nef_desc* grid, int32_t hidden_dim, int32_t
 int wb_spc_trace(const wb_octree* oct, int32_t level, const wb_rays* rays, const float* colors, int64_t color_stride, int64_t point_offset,
                  float* depth, uint8_t* hit, float* rgb, float* alpha, wb_stream s);
 
+/* ------------------------------------------------------------------------------------------------
+ * wisp.ops.mesh.compute_sdf (wisp/ops/mesh/compute_sdf.py; kernel wisp/csrc/external/mesh2sdf_kernel.cu:334-584, 844-903):
+ * out[i] = the signed distance from points[i] to the triangle soup tris, with the reference's arithmetic and sign rule:
+ * fp64 per pair except its fp32 roundings (idot2 = __frcp_rn, copysignf, the fminf-clamped edge parameter, the fminf minima),
+ * sqrtf of the fp32 minimum, negated when all 13 stab directions have a hit with t >= 0 and one with t < 0 (|det| < 1e-8 skipped);
+ * +inf when no triangle has a nonzero normal, and for a point with a NaN coordinate.
+ * A bounding-volume hierarchy (LBVH over centroid Morton codes) is built per call in `workspace` and culls, conservatively,
+ * the pairs that cannot set the fp32 minimum or a stab flag; the result is the reference's, not an approximation of it.
+ * tris: f64 [T, 9] (V[F] row-major), points: f64 [N, 3], out: f64 [N].  T < 2^31; T = 0 gives +inf.  N = 0 launches nothing.
+ * Launches (wb_launch_count): 6 for T >= 2 (the CUB radix sort counted as one), 5 for T = 1, 1 for T = 0. */
+/* Workspace bytes of a wb_mesh_sdf call over num_triangles triangles (any number of points); < 0 on a bad count or, for T >= 1, when
+ * the radix sort's size query of the current device fails (reason in wb_last_error()).  Launches nothing. */
+int64_t wb_mesh_sdf_workspace_bytes(int64_t num_triangles);
+int wb_mesh_sdf(const double* tris, int64_t num_triangles, const double* points, int64_t num_points, void* workspace,
+                int64_t workspace_bytes, double* out, wb_stream s);
+
 #ifdef __cplusplus
 }
 #endif

@@ -91,11 +91,14 @@ EXPORTS = [
     "wb_rf_march_fill", "wb_rf_param_blob_floats", "wb_rf_precision_supported", "wb_rf_pack_params", "wb_rf_shade_fwd", "wb_rf_shade_bwd",
     "wb_rf_workspace_bytes", "wb_rf_feat_bytes", "wb_rf_decoder_bwd", "wb_rf_table_scatter", "wb_rf_loss_scale", "wb_rf_workspace_holds_ray_rows", "wb_prune_samples", "wb_prune_update", "wb_raygen_lookat", "wb_raygen_pinhole", "wb_codebook_rows_fwd", "wb_codebook_rows_bwd", "wb_composite_bwd_loss", "wb_adam_step", "wb_adamw_step", "wb_rmsprop_step", "wb_tc_selftest",
     "wb_spc_trace",
+    "wb_mesh_sdf_workspace_bytes", "wb_mesh_sdf",
 ]
 
 # wb_spc_trace(oct, level, rays, colors, color_stride, point_offset, depth, hit, rgb, alpha, stream) -> int
 SPC_TRACE_ARGTYPES = [C.POINTER(OctreeDesc), C.c_int32, C.POINTER(RaysDesc), C.c_void_p, C.c_int64, C.c_int64,
                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+# wb_mesh_sdf(tris, num_triangles, points, num_points, workspace, workspace_bytes, out, stream) -> int
+MESH_SDF_ARGTYPES = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
 
 _lib: Optional[C.CDLL] = None
 _checked_devices = set()
@@ -128,6 +131,8 @@ def lib() -> C.CDLL:
         L.wb_sdf_train_tc_smem_bytes.restype = C.c_int64
         L.wb_image_smem_bytes.restype = C.c_int64
         L.wb_spc_trace.restype, L.wb_spc_trace.argtypes = C.c_int, SPC_TRACE_ARGTYPES
+        L.wb_mesh_sdf_workspace_bytes.restype, L.wb_mesh_sdf_workspace_bytes.argtypes = C.c_int64, [C.c_int64]
+        L.wb_mesh_sdf.restype, L.wb_mesh_sdf.argtypes = C.c_int, MESH_SDF_ARGTYPES
         _lib = L
     return _lib
 

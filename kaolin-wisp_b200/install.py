@@ -13,6 +13,7 @@ What is patched (reference file:line -> native replacement):
   NeuralSDF.sdf (no-grad)                       (neural_sdf.py:120-155)            wb_sdf_eval
   ImageNeuralField.rgb (no-grad)                (image_nef.py:77-97)               wb_image_eval
   NeuralRadianceField.prune                     (nerf.py:175-212)                  ops.prune_field
+  wisp.ops.mesh.compute_sdf                     (ops/mesh/compute_sdf.py:18-45)    wb_mesh_sdf (ops.compute_sdf)
 Every replacement keeps the reference signature, falls back to the original method for configurations outside the native
 path (unknown embedders, activations, grids), and keeps the attributes other wisp code reads (`prev_num_samples`, `bg_color`).
 SPCField itself is not patched: its Kaolin calls build the octree (like OctreeAS's constructor) and its rgba() is plain torch.
@@ -166,6 +167,14 @@ def install() -> bool:
             return fused if fused is not None else orig_rgb(self, coords, lod)
 
         _patch(ImageNeuralField, "rgb", image_rgb)
+
+    # ---- mesh SDF labels of the SDF datasets (a wisp whose wisp.ops.mesh does not import keeps every other patch) -----
+    try:
+        import wisp.ops.mesh as mesh_ops
+    except Exception:
+        mesh_ops = None
+    if mesh_ops is not None:
+        _patch(mesh_ops, "compute_sdf", lambda V, F, points, split_size=10 ** 6: ops.compute_sdf(V, F, points, split_size))
 
     # ---- pruning -------------------------------------------------------------------------------------------------
     orig_prune = NeuralRadianceField.prune

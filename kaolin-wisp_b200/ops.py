@@ -1437,3 +1437,38 @@ def prune_field(nef, jitter: Optional[torch.Tensor] = None, seed: Optional[int] 
         raise Exception(f"The BLAS {cls.__name__} does not support initialization from_quantized_points, which is required for pruning.")
     g.blas = cls.from_quantized_points(kept, level)
     return True
+
+
+# --------------------------------------------------------------------------------------------------------------
+# mesh SDF labels (wisp/ops/mesh/compute_sdf.py): the dataset side of app/nglod
+# --------------------------------------------------------------------------------------------------------------
+def compute_sdf(V: torch.Tensor, F: torch.Tensor, points: torch.Tensor, split_size: int = 10 ** 6) -> torch.Tensor:
+    """wisp.ops.mesh.compute_sdf (compute_sdf.py:18-45): the signed distance from each point to the mesh (V, F) -> f64 [N, 1] on the
+    current CUDA device, the value the reference's kernel (mesh2sdf_gpu_fast_nopre) returns for the same inputs in float64, in one
+    wb_mesh_sdf call that culls pairs through a bounding-volume hierarchy built per call.
+    V: [#V, 3] and points: [N, 3], float32 or float64 on any device (float32 widens to float64 exactly, so a float32 call returns the
+    reference's answer for the .double() inputs; the reference itself refuses float32).  F: [#F, 3] integer indices into V.
+    split_size: accepted for the reference's signature; the result does not depend on it (the reference splits the points only to
+    bound its per-point scratch, which this route does not have).  Without a CUDA device it raises WispB200Error."""
+    if not torch.cuda.is_available():
+        raise A.WispB200Error("compute_sdf needs a CUDA device (H100, sm_90a); there is no CPU fallback")
+    for name, t in (("V", V), ("points", points)):
+        if t.dtype not in (torch.float32, torch.float64) or t.dim() != 2 or t.shape[1] != 3:
+            raise A.WispB200Error(f"compute_sdf: {name} must be float32 or float64 [n, 3], got {t.dtype} {tuple(t.shape)}")
+    if F.dtype.is_floating_point or F.dtype == torch.bool or F.dim() != 2 or F.shape[1] != 3:
+        raise A.WispB200Error(f"compute_sdf: F must be integer [#F, 3], got {F.dtype} {tuple(F.shape)}")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    pts = points.to(dev, torch.float64).contiguous()
+    A.require_device(pts)
+    out = torch.empty((pts.shape[0], 1), dtype=torch.float64, device=dev)
+    if pts.shape[0] == 0:
+        return out
+    tris = V.to(dev, torch.float64)[F.to(dev, torch.int64)].reshape(-1, 9).contiguous()
+    L = A.lib()
+    nbytes = int(L.wb_mesh_sdf_workspace_bytes(tris.shape[0]))
+    if nbytes < 0:
+        raise A.WispB200Error(f"compute_sdf: {L.wb_last_error().decode()}")
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    with _stage("mesh_sdf"):
+        A.check(L.wb_mesh_sdf(A.ptr(tris), tris.shape[0], A.ptr(pts), pts.shape[0], A.ptr(ws), nbytes, A.ptr(out), A.stream()))
+    return out
