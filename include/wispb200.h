@@ -33,7 +33,7 @@ enum wb_status {
 
 const char* wb_last_error(void);
 int wb_version(void);
-/* Device check used by the host shim at import: WB_OK only on compute capability 10.x. */
+/* Device check used by the host shim at import: WB_OK only on compute capability 9.0. */
 int wb_device_check(int device);
 /* Number of kernels this library launched since load (bench.py's gpu_launches). */
 int64_t wb_launch_count(void);

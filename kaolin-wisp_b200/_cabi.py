@@ -80,32 +80,108 @@ class RMSpropSegment(C.Structure):
                 ("lr", C.c_float), ("weight_decay", C.c_float)]
 
 
-EXPORTS = [
-    "wb_last_error", "wb_version", "wb_device_check", "wb_launch_count",
-    "wb_octree_build_bits", "wb_octree_build_coarse", "wb_query",
-    "wb_raymarch_ray_count", "wb_scan_workspace_bytes", "wb_scan_counts", "wb_raymarch_ray_fill",
-    "wb_raytrace_count", "wb_raytrace_fill", "wb_raytrace_cache_bytes", "wb_raytrace_count_cached", "wb_raytrace_fill_cached", "wb_raymarch_voxel_fill", "wb_raymarch_uniform_count", "wb_raymarch_uniform_fill",
-    "wb_hashgrid_fwd", "wb_hashgrid_bwd", "wb_hashgrid2d_fwd", "wb_hashgrid2d_bwd", "wb_image_eval", "wb_image_train", "wb_image_smem_bytes",
-    "wb_triplane_fwd", "wb_triplane_bwd", "wb_triplane_relayout",
-    "wb_octree_interp_fwd", "wb_octree_interp_bwd", "wb_find_depth_bound", "wb_sdf_eval", "wb_sdf_train", "wb_sdf_train_smem_bytes", "wb_sdf_train_tc", "wb_sdf_train_tc_smem_bytes", "wb_sdf_trace", "wb_sdf_phase", "wb_composite_fwd", "wb_composite_bwd",
-    "wb_rf_march_fill", "wb_rf_param_blob_floats", "wb_rf_precision_supported", "wb_rf_pack_params", "wb_rf_shade_fwd", "wb_rf_shade_bwd",
-    "wb_rf_workspace_bytes", "wb_rf_feat_bytes", "wb_rf_decoder_bwd", "wb_rf_table_scatter", "wb_rf_loss_scale", "wb_rf_workspace_holds_ray_rows", "wb_prune_samples", "wb_prune_update", "wb_raygen_lookat", "wb_raygen_pinhole", "wb_codebook_rows_fwd", "wb_codebook_rows_bwd", "wb_composite_bwd_loss", "wb_adam_step", "wb_adamw_step", "wb_rmsprop_step", "wb_tc_selftest",
-    "wb_spc_trace",
-    "wb_mesh_sdf_workspace_bytes", "wb_mesh_sdf",
-]
-
-# wb_spc_trace(oct, level, rays, colors, color_stride, point_offset, depth, hit, rgb, alpha, stream) -> int
-SPC_TRACE_ARGTYPES = [C.POINTER(OctreeDesc), C.c_int32, C.POINTER(RaysDesc), C.c_void_p, C.c_int64, C.c_int64,
-                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-# wb_mesh_sdf(tris, num_triangles, points, num_points, workspace, workspace_bytes, out, stream) -> int
-MESH_SDF_ARGTYPES = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+# The C ABI's prototypes, in header order: name -> (restype, argtypes).  Data pointers (device or host) are c_void_p, host arrays of
+# device pointers POINTER(c_void_p), descriptors a POINTER to their mirror above (ctypes then refuses a descriptor of another kind
+# and takes the struct itself by reference).
+_i32, _int, _i64, _u32, _f32, _f64 = C.c_int32, C.c_int, C.c_int64, C.c_uint32, C.c_float, C.c_double
+_p, _pp = C.c_void_p, C.POINTER(C.c_void_p)
+_nef, _rays, _oct, _sdf, _state, _adam, _rms = (C.POINTER(s) for s in (NefDesc, RaysDesc, OctreeDesc, SdfDesc, SdfState, AdamSegment, RMSpropSegment))
+PROTOTYPES = {
+    "wb_last_error": (C.c_char_p, []),
+    "wb_version": (_int, []),
+    "wb_device_check": (_int, [_int]),
+    "wb_launch_count": (_i64, []),
+    "wb_octree_build_bits": (_int, [_p, _i64, _i32, _p, _p]),
+    "wb_octree_build_coarse": (_int, [_p, _i64, _i32, _i32, _p, _p]),
+    "wb_query": (_int, [_oct, _p, _i64, _i32, _i32, _p, _p]),
+    "wb_raymarch_ray_count": (_int, [_oct, _i32, _rays, _i32, _p, _u32, _p, _p, _p]),
+    "wb_scan_workspace_bytes": (_i64, [_i64]),
+    "wb_scan_counts": (_int, [_p, _i64, _p, _p, _i64, _p]),
+    "wb_raymarch_ray_fill": (_int, [_rays, _i32, _p, _u32, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "wb_raytrace_count": (_int, [_oct, _i32, _rays, _p, _p]),
+    "wb_raytrace_fill": (_int, [_oct, _i32, _rays, _p, _p, _p, _p, _p]),
+    "wb_raytrace_cache_bytes": (_i64, [_i64, _i32]),
+    "wb_raytrace_count_cached": (_int, [_oct, _i32, _rays, _p, _p, _i32, _p]),
+    "wb_raytrace_fill_cached": (_int, [_oct, _i32, _rays, _p, _p, _i32, _p, _p, _p, _p]),
+    "wb_raymarch_voxel_fill": (_int, [_rays, _p, _p, _i64, _i32, _p, _u32, _p, _p, _p, _p, _p, _p, _p]),
+    "wb_raymarch_uniform_count": (_int, [_p, _i64, _i32, _p, _p]),
+    "wb_raymarch_uniform_fill": (_int, [_rays, _p, _p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "wb_hashgrid_fwd": (_int, [_p, _i64, _nef, _p, _p]),
+    "wb_hashgrid_bwd": (_int, [_p, _i64, _nef, _p, _p, _p]),
+    "wb_triplane_fwd": (_int, [_p, _i64, _i32, _i32, _p, _pp, _p, _p]),
+    "wb_triplane_bwd": (_int, [_p, _i64, _i32, _i32, _p, _pp, _p, _pp, _p]),
+    "wb_triplane_relayout": (_int, [_pp, _pp, _p, _i32, _i32, _i32, _p]),
+    "wb_octree_interp_fwd": (_int, [_oct, _p, _p, _p, _i64, _i32, _i32, _i32, _i32, _i32, _pp, _p, _p]),
+    "wb_octree_interp_bwd": (_int, [_oct, _p, _p, _p, _i64, _i32, _i32, _i32, _i32, _pp, _p, _pp, _p]),
+    "wb_find_depth_bound": (_int, [_p, _p, _p, _i64, _i64, _p, _p]),
+    "wb_sdf_eval": (_int, [_oct, _sdf, _i32, _p, _i64, _p, _p]),
+    "wb_sdf_train": (_int, [_oct, _sdf, _i32, _p, _p, _i64, _f32, _pp, _p, _p, _p]),
+    "wb_sdf_train_smem_bytes": (_i64, [_sdf]),
+    "wb_sdf_train_tc": (_int, [_oct, _sdf, _i32, _p, _p, _i64, _f32, _pp, _p, _p, _p]),
+    "wb_sdf_train_tc_smem_bytes": (_i64, [_sdf]),
+    "wb_sdf_trace": (_int, [_oct, _sdf, _i32, _rays, _p, _i64, _p, _i32, _f32, _f64, _i32, _state, _p, _p, _p, _p, _p, _p, _p]),
+    "wb_sdf_phase": (_int, [_i32, _rays, _p, _i64, _p, _i32, _i32, _f64, _state, _p, _p, _p, _p, _p]),
+    "wb_composite_fwd": (_int, [_p, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _p]),
+    "wb_composite_bwd": (_int, [_p, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _p, _p]),
+    "wb_rf_march_fill": (_int, [_rays, _i32, _p, _u32, _p, _p, _p, _p, _p, _p]),
+    "wb_rf_param_blob_floats": (_i64, [_nef, _i32]),
+    "wb_rf_precision_supported": (_int, [_nef, _i32, _i32]),
+    "wb_rf_pack_params": (_int, [_nef, _i32, _p, _p]),
+    "wb_rf_workspace_bytes": (_i64, [_nef, _i32, _i64, _i64, _i32]),
+    "wb_rf_feat_bytes": (_i64, [_nef, _i32, _i64]),
+    "wb_rf_shade_fwd": (_int, [_nef, _p, _i32, _rays, _p, _p, _i64, _p, _p, _p, _p]),
+    "wb_rf_shade_bwd": (_int, [_nef, _p, _i32, _rays, _p, _p, _i64, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "wb_rf_workspace_holds_ray_rows": (_int, [_i32]),
+    "wb_rf_loss_scale": (_int, [_p, _p, _p]),
+    "wb_rf_decoder_bwd": (_int, [_nef, _p, _rays, _p, _p, _i64, _p, _p, _p, _p, _p, _p, _p]),
+    "wb_rf_table_scatter": (_int, [_nef, _rays, _p, _p, _i64, _p, _p, _p, _p]),
+    "wb_codebook_rows_fwd": (_int, [_p, _p, _i64, _i32, _i32, _i32, _p, _p, _p]),
+    "wb_codebook_rows_bwd": (_int, [_p, _p, _p, _i64, _i32, _i32, _p, _p, _p]),
+    "wb_composite_bwd_loss": (_int, [_p, _p, _p, _p, _i64, _p, _p, _p, _i32, _f32, _p, _p, _p, _p]),
+    "wb_adam_step": (_int, [_adam, _i32, _f32, _f32, _f32, _i32, _f32, _i32, _p]),
+    "wb_adamw_step": (_int, [_adam, _i32, _f32, _f32, _f32, _i32, _f32, _i32, _p]),
+    "wb_rmsprop_step": (_int, [_rms, _i32, _f32, _f32, _f32, _f32, _i32, _p]),
+    "wb_raygen_lookat": (_int, [_p, _p, _p, _p, _f32, _i32, _i32, _i32, _p, _p, _p]),
+    "wb_raygen_pinhole": (_int, [_p, _p, _f32, _f32, _f32, _f32, _i32, _i32, _i32, _i32, _p, _p, _p]),
+    "wb_prune_samples": (_int, [_p, _i64, _i32, _p, _u32, _p, _p, _p, _p, _p]),
+    "wb_prune_update": (_int, [_p, _i64, _f32, _f32, _p, _p, _p]),
+    "wb_tc_selftest": (_int, [_p, _int, _p, _int, _p, _int, _int, _int, _p]),
+    "wb_hashgrid2d_fwd": (_int, [_p, _i64, _nef, _p, _p]),
+    "wb_hashgrid2d_bwd": (_int, [_p, _i64, _nef, _p, _p, _p]),
+    "wb_image_eval": (_int, [_nef, _i32, _pp, _i32, _p, _i64, _p, _p]),
+    "wb_image_train": (_int, [_nef, _i32, _pp, _i32, _p, _p, _i64, _f32, _p, _p, _p, _p]),
+    "wb_image_smem_bytes": (_i64, [_nef, _i32, _i32]),
+    "wb_spc_trace": (_int, [_oct, _i32, _rays, _p, _i64, _i64, _p, _p, _p, _p, _p]),
+    "wb_mesh_sdf_workspace_bytes": (_i64, [_i64]),
+    "wb_mesh_sdf": (_int, [_p, _i64, _p, _i64, _p, _i64, _p, _p]),
+}
+EXPORTS = list(PROTOTYPES)
+# int results that are answers, not a wb_status; every other int result raises WispB200Error when nonzero
+NOT_STATUS = ("wb_version", "wb_rf_precision_supported")
 
 _lib: Optional[C.CDLL] = None
 _checked_devices = set()
 
 
 class WispB200Error(RuntimeError):
-    pass
+    """status: the wb_status a library call returned, or None for an error raised on the host side."""
+
+    def __init__(self, message: str, status: Optional[int] = None):
+        super().__init__(message)
+        self.status = status
+
+
+def check(rc: int) -> None:
+    """Raise WispB200Error for a nonzero wb_status.  The status entry points already raise through their errcheck, so a successful
+    call's result passes through: callers written as check(lib().wb_...(...)) keep working."""
+    if rc != 0:
+        raise WispB200Error(f"libwispb200 error {rc}: {lib().wb_last_error().decode()}", status=rc)
+
+
+def _raise_on_status(rc: int, func, args) -> int:
+    """errcheck of the wb_status entry points: wb_last_error() is read on the calling thread, right after the failed call."""
+    check(rc)
+    return rc
 
 
 def lib() -> C.CDLL:
@@ -119,27 +195,13 @@ def lib() -> C.CDLL:
                 f"{LIB_PATH} not found: build it with `python kaolin-wisp_b200/build.py` (or __graft_entry__.build()). "
                 "wisp_b200 has no CPU/eager fallback.")
         L = C.CDLL(LIB_PATH)
-        L.wb_last_error.restype = C.c_char_p
-        L.wb_launch_count.restype = C.c_int64
-        L.wb_scan_workspace_bytes.restype = C.c_int64
-        L.wb_scan_workspace_bytes.argtypes = [C.c_int64]
-        L.wb_rf_param_blob_floats.restype = C.c_int64
-        L.wb_rf_workspace_bytes.restype = C.c_int64
-        L.wb_rf_feat_bytes.restype = C.c_int64
-        L.wb_raytrace_cache_bytes.restype = C.c_int64
-        L.wb_sdf_train_smem_bytes.restype = C.c_int64
-        L.wb_sdf_train_tc_smem_bytes.restype = C.c_int64
-        L.wb_image_smem_bytes.restype = C.c_int64
-        L.wb_spc_trace.restype, L.wb_spc_trace.argtypes = C.c_int, SPC_TRACE_ARGTYPES
-        L.wb_mesh_sdf_workspace_bytes.restype, L.wb_mesh_sdf_workspace_bytes.argtypes = C.c_int64, [C.c_int64]
-        L.wb_mesh_sdf.restype, L.wb_mesh_sdf.argtypes = C.c_int, MESH_SDF_ARGTYPES
+        for name, (restype, argtypes) in PROTOTYPES.items():
+            fn = getattr(L, name)
+            fn.restype, fn.argtypes = restype, argtypes
+            if restype is _int and name not in NOT_STATUS:
+                fn.errcheck = _raise_on_status
         _lib = L
     return _lib
-
-
-def check(rc: int) -> None:
-    if rc != 0:
-        raise WispB200Error(f"libwispb200 error {rc}: {lib().wb_last_error().decode()}")
 
 
 def require_device(t: torch.Tensor) -> None:
@@ -151,7 +213,7 @@ def require_device(t: torch.Tensor) -> None:
         raise WispB200Error(f"tensor on cuda:{idx} but the current device is cuda:{torch.cuda.current_device()}: call under torch.cuda.device({idx}) "
                             "(the library launches on the current device; one process per GPU is the supported layout)")
     if idx not in _checked_devices:
-        check(lib().wb_device_check(C.c_int(idx)))
+        lib().wb_device_check(idx)
         _checked_devices.add(idx)
 
 

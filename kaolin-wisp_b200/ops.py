@@ -77,13 +77,13 @@ class OctreeTensors:
         bits = torch.zeros(words, dtype=torch.int32, device=self.octree.device)
         start, cnt = int(self.pyramid[1, level]), int(self.pyramid[0, level])
         lvl = self.points[start:start + cnt].contiguous()
-        A.check(A.lib().wb_octree_build_bits(A.ptr(lvl), C.c_int64(cnt), C.c_int32(level), A.ptr(bits), A.stream()))
+        A.lib().wb_octree_build_bits(A.ptr(lvl), cnt, level, A.ptr(bits), A.stream())
         self.bits, self.bits_level = bits, level
         self.coarse, self.coarse_level = None, 0
         cl = min(level - 1, COARSE_LEVEL)
         if cl >= 2 and cnt > 0:
             coarse = torch.zeros((8 ** cl + 31) // 32, dtype=torch.int32, device=self.octree.device)
-            A.check(A.lib().wb_octree_build_coarse(A.ptr(lvl), C.c_int64(cnt), C.c_int32(level), C.c_int32(cl), A.ptr(coarse), A.stream()))
+            A.lib().wb_octree_build_coarse(A.ptr(lvl), cnt, level, cl, A.ptr(coarse), A.stream())
             self.coarse, self.coarse_level = coarse, cl
         if cnt > 0:     # one-off (per octree) host read of the occupied extent; exact dyadic cell faces
             mn, mx = lvl.min(0).values.cpu().tolist(), lvl.max(0).values.cpu().tolist()
@@ -108,7 +108,7 @@ def query(oct: OctreeTensors, coords: torch.Tensor, level: int, with_parents: bo
     N = c.shape[0]
     out = torch.empty((N, level + 1) if with_parents else (N,), dtype=torch.int32, device=c.device)
     d = oct.desc()
-    A.check(A.lib().wb_query(C.byref(d), A.ptr(c), C.c_int64(N), C.c_int32(level), C.c_int32(int(with_parents)), A.ptr(out), A.stream()))
+    A.lib().wb_query(d, A.ptr(c), N, level, int(with_parents), A.ptr(out), A.stream())
     return out
 
 
@@ -148,12 +148,12 @@ def march_count(oct: OctreeTensors, origins, dirs, dist_min, dist_max, num_sampl
     od = oct.desc()
     L = A.lib()
     with _stage("march_count"):
-        A.check(L.wb_raymarch_ray_count(C.byref(od), C.c_int32(level), C.byref(rays), C.c_int32(num_samples), A.ptr(jit),
-                                        C.c_uint32(seed & 0xFFFFFFFF), A.ptr(hitmask), A.ptr(counts), A.stream()))
-    wsb = int(L.wb_scan_workspace_bytes(C.c_int64(R)))
+        L.wb_raymarch_ray_count(od, level, rays, num_samples, A.ptr(jit),
+                                seed & 0xFFFFFFFF, A.ptr(hitmask), A.ptr(counts), A.stream())
+    wsb = int(L.wb_scan_workspace_bytes(R))
     ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
     with _stage("scan"):
-        A.check(L.wb_scan_counts(A.ptr(counts), C.c_int64(R), A.ptr(offsets), A.ptr(ws), C.c_int64(wsb), A.stream()))
+        L.wb_scan_counts(A.ptr(counts), R, A.ptr(offsets), A.ptr(ws), wsb, A.stream())
     ms = MarchState(rays, keep + [jit], num_samples, jit, seed & 0xFFFFFFFF, hitmask, counts, offsets, -1)
     if defer_total:                        # pre-march on a side stream: the total travels to pinned memory, no host sync here
         host = _pinned_slot()
@@ -207,8 +207,8 @@ def march_fill_reference_layout(ms: MarchState, device):
     deltas = torch.empty((S, 1), dtype=torch.float32, device=device)
     boundary = torch.empty(S, dtype=torch.bool, device=device)
     if S > 0:
-        A.check(A.lib().wb_raymarch_ray_fill(C.byref(ms.rays), C.c_int32(ms.n), A.ptr(ms.jitter), C.c_uint32(ms.seed), A.ptr(ms.hitmask),
-                                             A.ptr(ms.offsets), A.ptr(ridx), A.ptr(samples), A.ptr(depth), A.ptr(deltas), A.ptr(boundary), A.stream()))
+        A.lib().wb_raymarch_ray_fill(ms.rays, ms.n, A.ptr(ms.jitter), ms.seed, A.ptr(ms.hitmask),
+                                     A.ptr(ms.offsets), A.ptr(ridx), A.ptr(samples), A.ptr(depth), A.ptr(deltas), A.ptr(boundary), A.stream())
     return ridx, samples, depth, deltas, boundary
 
 
@@ -281,8 +281,8 @@ def march_fill_records(ms: MarchState, device):
     rec_ray = _empty_s(S, (), torch.int32, device)
     if S > 0:
         with _stage("march_fill"):
-            A.check(A.lib().wb_rf_march_fill(C.byref(ms.rays), C.c_int32(ms.n), A.ptr(ms.jitter), C.c_uint32(ms.seed), A.ptr(ms.hitmask),
-                                             A.ptr(ms.offsets), A.ptr(rec_t), A.ptr(rec_delta), A.ptr(rec_ray), A.stream()))
+            A.lib().wb_rf_march_fill(ms.rays, ms.n, A.ptr(ms.jitter), ms.seed, A.ptr(ms.hitmask),
+                                     A.ptr(ms.offsets), A.ptr(rec_t), A.ptr(rec_delta), A.ptr(rec_ray), A.stream())
     return rec_t, rec_delta, rec_ray
 
 
@@ -293,9 +293,9 @@ def _scan(counts: torch.Tensor) -> torch.Tensor:
     n = counts.shape[0]
     offsets = torch.empty(n + 1, dtype=torch.int64, device=counts.device)
     L = A.lib()
-    wsb = int(L.wb_scan_workspace_bytes(C.c_int64(n)))
+    wsb = int(L.wb_scan_workspace_bytes(n))
     ws = torch.empty(wsb, dtype=torch.uint8, device=counts.device)
-    A.check(L.wb_scan_counts(A.ptr(counts), C.c_int64(n), A.ptr(offsets), A.ptr(ws), C.c_int64(wsb), A.stream()))
+    L.wb_scan_counts(A.ptr(counts), n, A.ptr(offsets), A.ptr(ws), wsb, A.stream())
     return offsets
 
 
@@ -328,12 +328,12 @@ def raytrace(oct: OctreeTensors, origins, dirs, level: int):
     # one traversal: the count pass caches the first RAYTRACE_CACHE_K nuggets of every ray, the fill copies them (rays with more are
     # traversed again); the cache is scratch (12 B x K per ray) and is skipped for ray counts where it would be unreasonably large
     K = RAYTRACE_CACHE_K if (RAYTRACE_CACHE_K > 0 and R * RAYTRACE_CACHE_K * 12 <= (2 << 30)) else 0
-    cache = _raytrace_scratch(int(L.wb_raytrace_cache_bytes(C.c_int64(R), C.c_int32(K))), dev) if K > 0 else None
+    cache = _raytrace_scratch(int(L.wb_raytrace_cache_bytes(R, K)), dev) if K > 0 else None
     with _stage("raytrace_count"):
         if K > 0:
-            A.check(L.wb_raytrace_count_cached(C.byref(od), C.c_int32(level), C.byref(rays), A.ptr(counts), A.ptr(cache), C.c_int32(K), A.stream()))
+            L.wb_raytrace_count_cached(od, level, rays, A.ptr(counts), A.ptr(cache), K, A.stream())
         else:
-            A.check(L.wb_raytrace_count(C.byref(od), C.c_int32(level), C.byref(rays), A.ptr(counts), A.stream()))
+            L.wb_raytrace_count(od, level, rays, A.ptr(counts), A.stream())
     offsets = _scan(counts)
     Ng = int(offsets[-1].item())
     ridx = _empty_n(Ng, (), torch.int32, dev); pidx = _empty_n(Ng, (), torch.int32, dev)
@@ -341,10 +341,10 @@ def raytrace(oct: OctreeTensors, origins, dirs, level: int):
     if Ng > 0:
         with _stage("raytrace_fill"):
             if K > 0:
-                A.check(L.wb_raytrace_fill_cached(C.byref(od), C.c_int32(level), C.byref(rays), A.ptr(offsets), A.ptr(cache), C.c_int32(K),
-                                                  A.ptr(ridx), A.ptr(pidx), A.ptr(depth), A.stream()))
+                L.wb_raytrace_fill_cached(od, level, rays, A.ptr(offsets), A.ptr(cache), K,
+                                          A.ptr(ridx), A.ptr(pidx), A.ptr(depth), A.stream())
             else:
-                A.check(L.wb_raytrace_fill(C.byref(od), C.c_int32(level), C.byref(rays), A.ptr(offsets), A.ptr(ridx), A.ptr(pidx), A.ptr(depth), A.stream()))
+                L.wb_raytrace_fill(od, level, rays, A.ptr(offsets), A.ptr(ridx), A.ptr(pidx), A.ptr(depth), A.stream())
     return ridx, pidx, depth, offsets
 
 
@@ -367,8 +367,8 @@ def spc_trace(oct: OctreeTensors, origins, dirs, level: int, colors: torch.Tenso
     alpha = torch.empty((R, 1), dtype=torch.float32, device=dev)
     od = oct.desc()
     with _stage("spc_trace"):
-        A.check(A.lib().wb_spc_trace(C.byref(od), level, C.byref(rays), A.ptr(colors), colors.stride(0), point_offset,
-                                     A.ptr(depth), A.ptr(hit), A.ptr(rgb), A.ptr(alpha), A.stream()))
+        A.lib().wb_spc_trace(od, level, rays, A.ptr(colors), colors.stride(0), point_offset,
+                             A.ptr(depth), A.ptr(hit), A.ptr(rgb), A.ptr(alpha), A.stream())
     return RenderBuffer(depth=depth, hit=hit, rgb=rgb, alpha=alpha)
 
 
@@ -406,7 +406,7 @@ def march_nuggets(oct: OctreeTensors, origins, dirs, level: int, num_samples: in
     else:
         scale = uniform_scale(num_samples)
         cnt = torch.empty(Ng, dtype=torch.int32, device=dev)
-        A.check(L.wb_raymarch_uniform_count(A.ptr(depth_n), C.c_int64(Ng), C.c_int32(scale), A.ptr(cnt), A.stream()))
+        L.wb_raymarch_uniform_count(A.ptr(depth_n), Ng, scale, A.ptr(cnt), A.stream())
         sample_off = _scan(cnt)
         S = int(sample_off[-1].item())
     t = torch.empty(S, dtype=torch.float32, device=dev); dl = torch.empty(S, dtype=torch.float32, device=dev)
@@ -419,12 +419,12 @@ def march_nuggets(oct: OctreeTensors, origins, dirs, level: int, num_samples: in
     jit = None if jitter is None else A.f32c(jitter)
     with _stage("march_" + kind):
         if kind == 'voxel':
-            A.check(L.wb_raymarch_voxel_fill(C.byref(rays), A.ptr(ridx_n), A.ptr(depth_n), C.c_int64(Ng), C.c_int32(num_samples), A.ptr(jit),
-                                             C.c_uint32(seed & 0xFFFFFFFF), A.ptr(ridx), A.ptr(samples), A.ptr(t), A.ptr(dl), A.ptr(boundary), A.ptr(rr), A.stream()))
+            L.wb_raymarch_voxel_fill(rays, A.ptr(ridx_n), A.ptr(depth_n), Ng, num_samples, A.ptr(jit),
+                                     seed & 0xFFFFFFFF, A.ptr(ridx), A.ptr(samples), A.ptr(t), A.ptr(dl), A.ptr(boundary), A.ptr(rr), A.stream())
             offsets = ray_off * num_samples
         else:
-            A.check(L.wb_raymarch_uniform_fill(C.byref(rays), A.ptr(ridx_n), A.ptr(depth_n), C.c_int64(Ng), C.c_int32(scale), A.ptr(sample_off), A.ptr(ray_off),
-                                               A.ptr(ridx), A.ptr(samples), A.ptr(t), A.ptr(dl), A.ptr(boundary), A.ptr(rr), A.stream()))
+            L.wb_raymarch_uniform_fill(rays, A.ptr(ridx_n), A.ptr(depth_n), Ng, scale, A.ptr(sample_off), A.ptr(ray_off),
+                                       A.ptr(ridx), A.ptr(samples), A.ptr(t), A.ptr(dl), A.ptr(boundary), A.ptr(rr), A.stream())
             offsets = sample_off[ray_off]
     ms = MarchState(rays, keep, num_samples, None, seed & 0xFFFFFFFF, None, None, offsets.contiguous(), S, records=(t, dl, rr))
     if reference_layout:
@@ -473,7 +473,7 @@ class HashGridInterpolate(torch.autograd.Function):
         desc = A.make_grid_desc(table, res, begin, 2 ** codebook_bitwidth)
         feats = torch.empty((c.shape[0], len(res) * table.shape[1]), dtype=torch.float32, device=c.device)
         fwd = A.lib().wb_hashgrid_fwd if dim == 3 else A.lib().wb_hashgrid2d_fwd
-        A.check(fwd(A.ptr(c), C.c_int64(c.shape[0]), C.byref(desc), A.ptr(feats), A.stream()))
+        fwd(A.ptr(c), c.shape[0], desc, A.ptr(feats), A.stream())
         ctx.save_for_backward(c, table)
         ctx.meta = (res, begin, codebook_bitwidth)
         return feats
@@ -486,7 +486,7 @@ class HashGridInterpolate(torch.autograd.Function):
         g = A.f32c(grad_output)
         gt = torch.zeros_like(table)                      # hashgrid_interpolate.cpp:85
         bwd = A.lib().wb_hashgrid_bwd if c.shape[-1] == 3 else A.lib().wb_hashgrid2d_bwd
-        A.check(bwd(A.ptr(c), C.c_int64(c.shape[0]), C.byref(desc), A.ptr(g), A.ptr(gt), A.stream()))
+        bwd(A.ptr(c), c.shape[0], desc, A.ptr(g), A.ptr(gt), A.stream())
         return None, None, None, None, gt, None
 
 
@@ -535,7 +535,7 @@ def image_field(nef):
         return None
     res = [int(r) for r in torch.as_tensor(grid.resolutions).reshape(-1).tolist()]
     desc = A.make_grid_desc(table.data, res, [int(b) for b in cb.begin_idxes.tolist()], 2 ** int(grid.codebook_bitwidth), grid.multiscale_type)
-    if A.lib().wb_image_smem_bytes(C.byref(desc), C.c_int32(H), C.c_int32(1)) < 0:
+    if A.lib().wb_image_smem_bytes(desc, H, 1) < 0:
         return None
     ptrs = (C.c_void_p * 4)(*[p.data_ptr() for p in params])
     return desc, H, ptrs, [table] + params
@@ -550,7 +550,7 @@ def image_eval(nef, coords: torch.Tensor, lod_idx: int) -> Optional[torch.Tensor
     A.require_device(coords)
     c = A.f32c(coords)
     rgb = torch.empty((c.shape[0], 3), dtype=torch.float32, device=c.device)
-    A.check(A.lib().wb_image_eval(C.byref(desc), C.c_int32(H), params, C.c_int32(lod_idx), A.ptr(c), C.c_int64(c.shape[0]), A.ptr(rgb), A.stream()))
+    A.lib().wb_image_eval(desc, H, params, lod_idx, A.ptr(c), c.shape[0], A.ptr(rgb), A.stream())
     return rgb
 
 
@@ -574,8 +574,8 @@ def image_train(fd, coords: torch.Tensor, rgb_gt: torch.Tensor, lod_idx: int, gr
     if N == 0:
         raise A.WispB200Error("image_train: empty batch (the reference's mse_loss averages over it)")
     c, g = A.f32c(coords), A.f32c(rgb_gt)
-    A.check(A.lib().wb_image_train(C.byref(desc), C.c_int32(H), params, C.c_int32(lod_idx), A.ptr(c), A.ptr(g), C.c_int64(N),
-                                   C.c_float(1.0 / (3.0 * N)), A.ptr(grad_table), A.ptr(grad_params), A.ptr(loss_out), A.stream()))
+    A.lib().wb_image_train(desc, H, params, lod_idx, A.ptr(c), A.ptr(g), N,
+                           1.0 / (3.0 * N), A.ptr(grad_table), A.ptr(grad_params), A.ptr(loss_out), A.stream())
 
 
 # --------------------------------------------------------------------------------------------------------------
@@ -595,7 +595,7 @@ class TriplaneInterpolate(torch.autograd.Function):
         res = (C.c_int32 * num_lods)(*[pl[3 * l].shape[-1] - 1 for l in range(num_lods)])
         ptrs = (C.c_void_p * (3 * num_lods))(*[p.data_ptr() for p in pl])
         feats = torch.empty((N, num_lods * 3 * fdim), dtype=torch.float32, device=c.device)
-        A.check(A.lib().wb_triplane_fwd(A.ptr(c), C.c_int64(N), C.c_int32(num_lods), C.c_int32(fdim), res, ptrs, A.ptr(feats), A.stream()))
+        A.lib().wb_triplane_fwd(A.ptr(c), N, num_lods, fdim, res, ptrs, A.ptr(feats), A.stream())
         ctx.save_for_backward(c, *pl)
         ctx.num_lods, ctx.nplanes = num_lods, len(planes)
         return feats
@@ -609,7 +609,7 @@ class TriplaneInterpolate(torch.autograd.Function):
         res = (C.c_int32 * num_lods)(*[pl[3 * l].shape[-1] - 1 for l in range(num_lods)])
         ptrs = (C.c_void_p * (3 * num_lods))(*[p.data_ptr() for p in pl])
         gptrs = (C.c_void_p * (3 * num_lods))(*[p.data_ptr() for p in gp])
-        A.check(A.lib().wb_triplane_bwd(A.ptr(c), C.c_int64(c.shape[0]), C.c_int32(num_lods), C.c_int32(fdim), res, ptrs, A.ptr(g), gptrs, A.stream()))
+        A.lib().wb_triplane_bwd(A.ptr(c), c.shape[0], num_lods, fdim, res, ptrs, A.ptr(g), gptrs, A.stream())
         return (None, None, *gp, *([None] * (ctx.nplanes - len(gp))))
 
 
@@ -629,8 +629,8 @@ class OctreeInterpolate(torch.autograd.Function):
         ptrs = (C.c_void_p * nl)(*[f.data_ptr() for f in fl])
         out = torch.empty((N, F if multiscale == 'sum' else nl * F), dtype=torch.float32, device=c.device)
         od = oct.desc()
-        A.check(A.lib().wb_octree_interp_fwd(C.byref(od), A.ptr(oct.points), A.ptr(trinkets), A.ptr(c), C.c_int64(N), C.c_int32(F), C.c_int32(base_lod),
-                                             C.c_int32(nl), C.c_int32(1 if multiscale == 'sum' else 0), C.c_int32(int(half_round)), ptrs, A.ptr(out), A.stream()))
+        A.lib().wb_octree_interp_fwd(od, A.ptr(oct.points), A.ptr(trinkets), A.ptr(c), N, F, base_lod,
+                                     nl, 1 if multiscale == 'sum' else 0, int(half_round), ptrs, A.ptr(out), A.stream())
         ctx.save_for_backward(c, trinkets, *fl)
         ctx.meta = (oct, base_lod, multiscale)
         return out
@@ -643,8 +643,8 @@ class OctreeInterpolate(torch.autograd.Function):
         gf = [torch.zeros_like(f) for f in fl]
         ptrs = (C.c_void_p * nl)(*[f.data_ptr() for f in fl]); gptrs = (C.c_void_p * nl)(*[f.data_ptr() for f in gf])
         od = oct.desc()
-        A.check(A.lib().wb_octree_interp_bwd(C.byref(od), A.ptr(oct.points), A.ptr(trinkets), A.ptr(c), C.c_int64(c.shape[0]), C.c_int32(F), C.c_int32(base_lod),
-                                             C.c_int32(nl), C.c_int32(1 if multiscale == 'sum' else 0), ptrs, A.ptr(A.f32c(g)), gptrs, A.stream()))
+        A.lib().wb_octree_interp_bwd(od, A.ptr(oct.points), A.ptr(trinkets), A.ptr(c), c.shape[0], F, base_lod,
+                                     nl, 1 if multiscale == 'sum' else 0, ptrs, A.ptr(A.f32c(g)), gptrs, A.stream())
         return (None, None, None, None, None, None, *gf)
 
 
@@ -658,7 +658,7 @@ class CodebookRows(torch.autograd.Function):
         lg, dc = A.f32c(logits.detach()), A.f32c(dictionary.detach())
         rows, K, F = lg.shape[0], lg.shape[1], dc.shape[1]
         E = torch.empty((rows, F), dtype=torch.float32, device=lg.device)
-        A.check(A.lib().wb_codebook_rows_fwd(A.ptr(lg), A.ptr(dc), C.c_int64(rows), C.c_int32(K), C.c_int32(F), C.c_int32(int(training)), A.ptr(E), None, A.stream()))
+        A.lib().wb_codebook_rows_fwd(A.ptr(lg), A.ptr(dc), rows, K, F, int(training), A.ptr(E), None, A.stream())
         ctx.save_for_backward(lg, dc)
         ctx.training = bool(training)
         return E
@@ -672,8 +672,8 @@ class CodebookRows(torch.autograd.Function):
             return None, gd, None
         g_lg, g_dc = torch.zeros_like(lg), torch.zeros_like(dc)
         de = A.f32c(dE)
-        A.check(A.lib().wb_codebook_rows_bwd(A.ptr(lg), A.ptr(dc), A.ptr(de), C.c_int64(lg.shape[0]), C.c_int32(lg.shape[1]), C.c_int32(dc.shape[1]),
-                                             A.ptr(g_lg), A.ptr(g_dc), A.stream()))
+        A.lib().wb_codebook_rows_bwd(A.ptr(lg), A.ptr(dc), A.ptr(de), lg.shape[0], lg.shape[1], dc.shape[1],
+                                     A.ptr(g_lg), A.ptr(g_dc), A.stream())
         return g_lg, g_dc, None
 
 
@@ -684,7 +684,7 @@ def find_depth_bound(query: torch.Tensor, nug_depth: torch.Tensor, info=None, cu
     A.require_device(query)
     q, ci, dp = A.f32c(query).reshape(-1), curr_idxes.int().contiguous(), A.f32c(nug_depth)
     out = torch.empty(q.shape[0], dtype=torch.int32, device=q.device)
-    A.check(A.lib().wb_find_depth_bound(A.ptr(q), A.ptr(ci), A.ptr(dp), C.c_int64(q.shape[0]), C.c_int64(dp.shape[0]), A.ptr(out), A.stream()))
+    A.lib().wb_find_depth_bound(A.ptr(q), A.ptr(ci), A.ptr(dp), q.shape[0], dp.shape[0], A.ptr(out), A.stream())
     return out
 
 
@@ -775,7 +775,7 @@ def sdf_eval(nef, coords: torch.Tensor, lod_idx: Optional[int] = None) -> Option
     out = torch.empty((c.shape[0], 1), dtype=torch.float32, device=c.device)
     od = _sdf_octree(oct)
     with _stage("sdf_eval"):
-        A.check(A.lib().wb_sdf_eval(od, C.byref(d), C.c_int32(lod_idx), A.ptr(c), C.c_int64(c.shape[0]), A.ptr(out), A.stream()))
+        A.lib().wb_sdf_eval(od, d, lod_idx, A.ptr(c), c.shape[0], A.ptr(out), A.stream())
     return out
 
 
@@ -790,19 +790,19 @@ def sdf_channel(nef, coords: torch.Tensor, lod_idx: Optional[int] = None) -> Opt
 
 def _sdf_octree(oct):
     """The wb_octree argument of wb_sdf_eval / wb_sdf_train: the octree grid's occupancy, NULL for a hash field."""
-    return None if oct is None else C.byref(oct.desc())
+    return None if oct is None else oct.desc()
 
 
 def sdf_train_smem_bytes(fd) -> int:
     """Shared memory of a wb_sdf_train launch for the field fd = sdf_field(nef), or < 0 when the fused step cannot train it
     (its weights, weight-gradient accumulators and smallest sample tile exceed an SM's shared memory)."""
-    return int(A.lib().wb_sdf_train_smem_bytes(C.byref(fd[0])))
+    return int(A.lib().wb_sdf_train_smem_bytes(fd[0]))
 
 
 def sdf_train_tc_smem_bytes(fd) -> int:
     """Shared memory of a wb_sdf_train_tc launch (precision 1: fp16 weight packs, fp32 weight-gradient accumulators and one
     64-sample tile) for the field fd = sdf_field(nef), or < 0 when the tensor-core step cannot train it."""
-    return int(A.lib().wb_sdf_train_tc_smem_bytes(C.byref(fd[0])))
+    return int(A.lib().wb_sdf_train_tc_smem_bytes(fd[0]))
 
 
 def sdf_train(fd, coords: torch.Tensor, sdf_gt: torch.Tensor, lod_idx: int, inv_count: float, grad_feats: Sequence[torch.Tensor],
@@ -826,8 +826,7 @@ def sdf_train(fd, coords: torch.Tensor, sdf_gt: torch.Tensor, lod_idx: int, inv_
     od = _sdf_octree(oct)
     fn = A.lib().wb_sdf_train_tc if precision == 1 else A.lib().wb_sdf_train
     with _stage("sdf_train"):
-        A.check(fn(od, C.byref(d), C.c_int32(lod_idx), A.ptr(coords), A.ptr(sdf_gt), C.c_int64(coords.shape[0]),
-                                     C.c_float(inv_count), gptrs, A.ptr(grad_params), A.ptr(loss_out), A.stream()))
+        fn(od, d, lod_idx, A.ptr(coords), A.ptr(sdf_gt), coords.shape[0], inv_count, gptrs, A.ptr(grad_params), A.ptr(loss_out), A.stream())
 
 
 class _SdfState:
@@ -839,7 +838,7 @@ class _SdfState:
         f32 = lambda n: torch.empty(max(n, 1), dtype=torch.float32, device=dev)
         self.flags, self.pack_ray, self.cursor0, self.cursor1 = i32(R), i32(R), i32(R), i32(R)
         self.pack_off = torch.empty(R + 1, dtype=torch.int64, device=dev)
-        self.scan_ws = torch.empty(max(int(L.wb_scan_workspace_bytes(C.c_int64(R))), 1), dtype=torch.uint8, device=dev)
+        self.scan_ws = torch.empty(max(int(L.wb_scan_workspace_bytes(R)), 1), dtype=torch.uint8, device=dev)
         self.t, self.dist, self.dist_prev, self.x = f32(R), f32(R), f32(R), f32(3 * R)
         self.state = torch.empty(max(R, 1), dtype=torch.uint8, device=dev)
         self.iterflags = i32(2 * num_steps + 4)
@@ -882,16 +881,16 @@ def sdf_trace(nef, oct: OctreeTensors, origins, dirs, dist_max, level: int, lod_
     if fd is not None and not fd[0].hash and not (fd[0].multiscale == 0 and lod_idx != fd[0].num_lods - 1):
         d, _, keep2 = fd
         with _stage("sdf_trace"):
-            A.check(L.wb_sdf_trace(C.byref(od), C.byref(d), C.c_int32(lod_idx), C.byref(rays), A.ptr(nug_depth), C.c_int64(Ng), A.ptr(ray_off),
-                                   C.c_int32(num_steps), C.c_float(step_size), C.c_double(min_dis), C.c_int32(int(want_normals)), C.byref(st.c),
-                                   A.ptr(out["xyz"]), A.ptr(out["depth"]), A.ptr(out["hit"]), A.ptr(out["normal"]), A.ptr(out["rgb"]), A.ptr(out["alpha"]), A.stream()))
+            L.wb_sdf_trace(od, d, lod_idx, rays, A.ptr(nug_depth), Ng, A.ptr(ray_off),
+                           num_steps, step_size, min_dis, int(want_normals), st.c,
+                           A.ptr(out["xyz"]), A.ptr(out["depth"]), A.ptr(out["hit"]), A.ptr(out["normal"]), A.ptr(out["rgb"]), A.ptr(out["alpha"]), A.stream())
         out["_evals"] = st.iterflags[2 * num_steps + 2: 2 * num_steps + 3]      # device counter: field evaluations of this launch
         return out, None
 
     # ---- generic field: the state machine runs natively, the field through its own forward() between the phases ----
     def phase(ph, it=0):
-        A.check(L.wb_sdf_phase(C.c_int32(ph), C.byref(rays), A.ptr(nug_depth), C.c_int64(Ng), A.ptr(ray_off), C.c_int32(num_steps), C.c_int32(it),
-                               C.c_double(min_dis), C.byref(st.c), A.ptr(out["xyz"]), A.ptr(out["depth"]), A.ptr(out["hit"]), A.ptr(out["alpha"]), A.stream()))
+        L.wb_sdf_phase(ph, rays, A.ptr(nug_depth), Ng, A.ptr(ray_off), num_steps, it,
+                       min_dis, st.c, A.ptr(out["xyz"]), A.ptr(out["depth"]), A.ptr(out["hit"]), A.ptr(out["alpha"]), A.stream())
 
     def field(x):
         return nef(coords=x, lod_idx=lod_idx, channels="sdf").reshape(-1).float() * 1.0 * step_size
@@ -939,8 +938,8 @@ class CompositeFn(torch.autograd.Function):
         alpha = torch.empty((R, 1), dtype=torch.float32, device=dev)
         hit = torch.empty(R, dtype=torch.bool, device=dev)
         bgv = _bg3(bg)
-        A.check(A.lib().wb_composite_fwd(A.ptr(sh), A.ptr(dp), A.ptr(dl), A.ptr(offsets), C.c_int64(R), bgv,
-                                         A.ptr(rgb), A.ptr(dout), A.ptr(alpha), A.ptr(hit), A.stream()))
+        A.lib().wb_composite_fwd(A.ptr(sh), A.ptr(dp), A.ptr(dl), A.ptr(offsets), R, bgv,
+                                 A.ptr(rgb), A.ptr(dout), A.ptr(alpha), A.ptr(hit), A.stream())
         ctx.save_for_backward(sh, dp, dl, offsets)
         ctx.bg = bgv
         ctx.mark_non_differentiable(hit)
@@ -951,9 +950,9 @@ class CompositeFn(torch.autograd.Function):
         sh, dp, dl, offsets = ctx.saved_tensors
         R = offsets.shape[0] - 1
         g_sh = torch.zeros_like(sh)
-        A.check(A.lib().wb_composite_bwd(A.ptr(sh), A.ptr(dp), A.ptr(dl), A.ptr(offsets), C.c_int64(R), ctx.bg,
-                                         A.ptr(A.f32c(g_rgb)), A.ptr(A.f32c(g_depth).reshape(-1)) if g_depth is not None else None,
-                                         A.ptr(A.f32c(g_alpha).reshape(-1)) if g_alpha is not None else None, A.ptr(g_sh), None, A.stream()))
+        A.lib().wb_composite_bwd(A.ptr(sh), A.ptr(dp), A.ptr(dl), A.ptr(offsets), R, ctx.bg,
+                                 A.ptr(A.f32c(g_rgb)), A.ptr(A.f32c(g_depth).reshape(-1)) if g_depth is not None else None,
+                                 A.ptr(A.f32c(g_alpha).reshape(-1)) if g_alpha is not None else None, A.ptr(g_sh), None, A.stream())
         return g_sh, None, None, None, None
 
 
@@ -1050,7 +1049,7 @@ def triplane_relayout(src: Sequence[torch.Tensor], to_channel_last: bool, out: O
     n = len(src)
     sp = (C.c_void_p * n)(*[t.data_ptr() for t in src]); dp = (C.c_void_p * n)(*[t.data_ptr() for t in dst])
     sz = (C.c_int32 * n)(*sizes)
-    A.check(A.lib().wb_triplane_relayout(sp, dp, sz, C.c_int32(n), C.c_int32(Cc), C.c_int32(1 if to_channel_last else 0), A.stream()))
+    A.lib().wb_triplane_relayout(sp, dp, sz, n, Cc, 1 if to_channel_last else 0, A.stream())
     return dst
 
 
@@ -1225,11 +1224,11 @@ class RFTraceFn(torch.autograd.Function):
         dens_flat, col_flat = _flatten(params[:n_dens]), _flatten(params[n_dens:])
         oct, trinkets = octctx if octctx is not None else (None, None)
         desc, keep = spec.desc(gt, dens_flat, col_flat, oct, trinkets, layout=layout)
-        nblob = int(L.wb_rf_param_blob_floats(C.byref(desc), C.c_int32(precision)))
+        nblob = int(L.wb_rf_param_blob_floats(desc, precision))
         if nblob < 0:
             raise A.WispB200Error(L.wb_last_error().decode())
         blob = torch.empty(nblob, dtype=torch.float32, device=dev)
-        A.check(L.wb_rf_pack_params(C.byref(desc), C.c_int32(precision), A.ptr(blob), A.stream()))
+        L.wb_rf_pack_params(desc, precision, A.ptr(blob), A.stream())
         rec_t, rec_delta, rec_ray = march_fill_records(ms, dev)
         S, R = ms.total, ms.rays.num_rays
         shaded = _empty_s(S, (4,), torch.float32, dev)
@@ -1237,23 +1236,23 @@ class RFTraceFn(torch.autograd.Function):
         # tells us whether a backward pass can follow, so that inference neither saves features nor needs the backward tiles
         need_grad = bool(want_grad) and any(ctx.needs_input_grad[8:])
         Scap = _bucket(S)                                  # byte sizes for the bucketed capacity (layouts still use S)
-        wsb = int(L.wb_rf_workspace_bytes(C.byref(desc), C.c_int32(precision), C.c_int64(R), C.c_int64(Scap), C.c_int32(0)))
+        wsb = int(L.wb_rf_workspace_bytes(desc, precision, R, Scap, 0))
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev) if wsb > 0 else None
-        fb = int(L.wb_rf_feat_bytes(C.byref(desc), C.c_int32(precision), C.c_int64(Scap))) if need_grad else 0
+        fb = int(L.wb_rf_feat_bytes(desc, precision, Scap)) if need_grad else 0
         if fb < 0 or wsb < 0:        # e.g. the tensor-core backward of this decoder does not fit: fail at the forward, not mid-backward
             raise A.WispB200Error(L.wb_last_error().decode())
         feat = torch.empty(fb, dtype=torch.uint8, device=dev) if fb > 0 else None
         with _stage("shade_fwd"):
-            A.check(L.wb_rf_shade_fwd(C.byref(desc), A.ptr(blob), C.c_int32(precision), C.byref(ms.rays), A.ptr(rec_t), A.ptr(rec_ray),
-                                      C.c_int64(S), A.ptr(shaded), A.ptr(feat), A.ptr(ws), A.stream()))
+            L.wb_rf_shade_fwd(desc, A.ptr(blob), precision, ms.rays, A.ptr(rec_t), A.ptr(rec_ray),
+                              S, A.ptr(shaded), A.ptr(feat), A.ptr(ws), A.stream())
         rgb = torch.empty((R, 3), dtype=torch.float32, device=dev)
         depth = torch.empty((R, 1), dtype=torch.float32, device=dev)
         alpha = torch.empty((R, 1), dtype=torch.float32, device=dev)
         hit = torch.empty(R, dtype=torch.bool, device=dev)
         bgv = _bg3(bg)
         with _stage("composite_fwd"):
-            A.check(L.wb_composite_fwd(A.ptr(shaded), A.ptr(rec_t), A.ptr(rec_delta), A.ptr(ms.offsets), C.c_int64(R), bgv,
-                                       A.ptr(rgb), A.ptr(depth), A.ptr(alpha), A.ptr(hit), A.stream()))
+            L.wb_composite_fwd(A.ptr(shaded), A.ptr(rec_t), A.ptr(rec_delta), A.ptr(ms.offsets), R, bgv,
+                               A.ptr(rgb), A.ptr(depth), A.ptr(alpha), A.ptr(hit), A.stream())
         ctx.ms, ctx.spec, ctx.n_grid, ctx.n_dens, ctx.bg, ctx.precision, ctx.octctx = ms, spec, n_grid, n_dens, bgv, precision, octctx
         ctx.layout = layout
         ctx.param_shapes = [p.shape for p in params]
@@ -1278,28 +1277,28 @@ class RFTraceFn(torch.autograd.Function):
         grgb = A.f32c(g_rgb)
         absmax = torch.zeros(1, dtype=torch.float32, device=shaded.device) if ctx.precision == 1 else None
         with _stage("composite_bwd"):
-            A.check(L.wb_composite_bwd(A.ptr(shaded), A.ptr(rec_t), A.ptr(rec_delta), A.ptr(ms.offsets), C.c_int64(R), ctx.bg,
-                                       A.ptr(grgb), A.ptr(gd), A.ptr(ga), A.ptr(g_sh), A.ptr(absmax), A.stream()))
+            L.wb_composite_bwd(A.ptr(shaded), A.ptr(rec_t), A.ptr(rec_delta), A.ptr(ms.offsets), R, ctx.bg,
+                               A.ptr(grgb), A.ptr(gd), A.ptr(ga), A.ptr(g_sh), A.ptr(absmax), A.stream())
         g_dens = torch.zeros_like(dens_flat)
         g_col = torch.zeros_like(col_flat)
         scale = None
         if ctx.precision == 1 and S > 0:
             # power-of-two loss scale computed on the device (no host sync): largest |gradient| -> ~64 in fp16
             scale = torch.empty(1, dtype=torch.float32, device=shaded.device)
-            A.check(L.wb_rf_loss_scale(A.ptr(absmax), A.ptr(scale), A.stream()))
-        wsb = int(L.wb_rf_workspace_bytes(C.byref(desc), C.c_int32(ctx.precision), C.c_int64(R), C.c_int64(_bucket(S)), C.c_int32(1)))
+            L.wb_rf_loss_scale(A.ptr(absmax), A.ptr(scale), A.stream())
+        wsb = int(L.wb_rf_workspace_bytes(desc, ctx.precision, R, _bucket(S), 1))
         ws = torch.empty(wsb, dtype=torch.uint8, device=shaded.device) if wsb > 0 else None
         if ctx.precision == 1 and S > 0 and SPLIT_BWD:        # the two stages as separate launches (profiling; WB_SPLIT_BWD=1)
             with _stage("decoder_bwd"):
-                A.check(L.wb_rf_decoder_bwd(C.byref(desc), A.ptr(blob), C.byref(ms.rays), A.ptr(rec_t), A.ptr(rec_ray), C.c_int64(S), A.ptr(g_sh),
-                                            A.ptr(scale), A.ptr(ctx.feat), A.ptr(ws), A.ptr(g_dens), A.ptr(g_col), A.stream()))
+                L.wb_rf_decoder_bwd(desc, A.ptr(blob), ms.rays, A.ptr(rec_t), A.ptr(rec_ray), S, A.ptr(g_sh),
+                                    A.ptr(scale), A.ptr(ctx.feat), A.ptr(ws), A.ptr(g_dens), A.ptr(g_col), A.stream())
             with _stage("table_scatter"):
-                A.check(L.wb_rf_table_scatter(C.byref(desc), C.byref(ms.rays), A.ptr(rec_t), A.ptr(rec_ray), C.c_int64(S), A.ptr(scale), A.ptr(ws),
-                                              A.ptr(g_table), A.stream()))
+                L.wb_rf_table_scatter(desc, ms.rays, A.ptr(rec_t), A.ptr(rec_ray), S, A.ptr(scale), A.ptr(ws),
+                                      A.ptr(g_table), A.stream())
         else:   # precision 1: decoder backward with the hash-table scatter fused into its last epilogue (one kernel) where the shape allows
             with _stage("shade_bwd"):
-                A.check(L.wb_rf_shade_bwd(C.byref(desc), A.ptr(blob), C.c_int32(ctx.precision), C.byref(ms.rays), A.ptr(rec_t), A.ptr(rec_ray),
-                                          C.c_int64(S), A.ptr(g_sh), A.ptr(scale), A.ptr(ctx.feat), A.ptr(ws), A.ptr(g_table), A.ptr(g_dens), A.ptr(g_col), A.stream()))
+                L.wb_rf_shade_bwd(desc, A.ptr(blob), ctx.precision, ms.rays, A.ptr(rec_t), A.ptr(rec_ray),
+                                  S, A.ptr(g_sh), A.ptr(scale), A.ptr(ctx.feat), A.ptr(ws), A.ptr(g_table), A.ptr(g_dens), A.ptr(g_col), A.stream())
         grads = []
         for flat, shapes in ((g_dens, ctx.param_shapes[:ctx.n_dens]), (g_col, ctx.param_shapes[ctx.n_dens:])):
             o = 0
@@ -1332,7 +1331,7 @@ def precision_supported(spec: NefSpec, nef, precision: int, backward: bool) -> b
         d.lod_idx = spec.lod_idx if spec.kind == "hash" else d.num_lods
         if not spec.fill_decoders(d, dummy.data_ptr(), dummy.data_ptr()):
             return False
-        ans = bool(A.lib().wb_rf_precision_supported(C.byref(d), C.c_int32(precision), C.c_int32(1 if backward else 0)))
+        ans = bool(A.lib().wb_rf_precision_supported(d, precision, 1 if backward else 0))
         _SUPPORT_CACHE[key] = ans
     return ans
 
@@ -1407,23 +1406,23 @@ def prune_field(nef, jitter: Optional[torch.Tensor] = None, seed: Optional[int] 
     samples = torch.empty((N, 3), dtype=torch.float32, device=dev); dirs = torch.empty_like(samples)
     rec_t = torch.empty(N, dtype=torch.float32, device=dev); rec_ray = torch.empty(N, dtype=torch.int32, device=dev)
     with _stage("prune_samples"):
-        A.check(L.wb_prune_samples(A.ptr(points), C.c_int64(N), C.c_int32(level), A.ptr(u), C.c_uint32(seed & 0xFFFFFFFF), A.ptr(samples), A.ptr(dirs),
-                                   A.ptr(rec_t), A.ptr(rec_ray), A.stream()))
+        L.wb_prune_samples(A.ptr(points), N, level, A.ptr(u), seed & 0xFFFFFFFF, A.ptr(samples), A.ptr(dirs),
+                           A.ptr(rec_t), A.ptr(rec_ray), A.stream())
     gt = [A.f32c(t.detach()) for t in grid]
     dens_flat, col_flat = _flatten(decoder_params(nef.decoder_density)), _flatten(decoder_params(nef.decoder_color))
     oct, trinkets = _grid_context(nef, spec)
     desc, keep_alive = spec.desc(gt, dens_flat, col_flat, oct, trinkets)
-    blob = torch.empty(int(L.wb_rf_param_blob_floats(C.byref(desc), C.c_int32(0))), dtype=torch.float32, device=dev)
-    A.check(L.wb_rf_pack_params(C.byref(desc), C.c_int32(0), A.ptr(blob), A.stream()))
+    blob = torch.empty(int(L.wb_rf_param_blob_floats(desc, 0)), dtype=torch.float32, device=dev)
+    L.wb_rf_pack_params(desc, 0, A.ptr(blob), A.stream())
     rays, keep_rays = A.make_rays(samples, dirs, 0.0, 0.0)
     shaded = torch.empty((N, 4), dtype=torch.float32, device=dev)
     with _stage("prune_density"):             # fp32 decoders: the reference probes under torch.no_grad() outside autocast
-        A.check(L.wb_rf_shade_fwd(C.byref(desc), A.ptr(blob), C.c_int32(0), C.byref(rays), A.ptr(rec_t), A.ptr(rec_ray), C.c_int64(N), A.ptr(shaded),
-                                  None, None, A.stream()))
+        L.wb_rf_shade_fwd(desc, A.ptr(blob), 0, rays, A.ptr(rec_t), A.ptr(rec_ray), N, A.ptr(shaded),
+                          None, None, A.stream())
     keep = torch.empty(N, dtype=torch.bool, device=dev)
     with _stage("prune_update"):
-        A.check(L.wb_prune_update(A.ptr(shaded), C.c_int64(N), C.c_float(float(nef.prune_density_decay)), C.c_float(float(nef.prune_min_density)),
-                                  A.ptr(occ), A.ptr(keep), A.stream()))
+        L.wb_prune_update(A.ptr(shaded), N, float(nef.prune_density_decay), float(nef.prune_min_density),
+                          A.ptr(occ), A.ptr(keep), A.stream())
     import torch.distributed as dist
     if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
         dist.broadcast(occ, src=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
@@ -1470,5 +1469,5 @@ def compute_sdf(V: torch.Tensor, F: torch.Tensor, points: torch.Tensor, split_si
         raise A.WispB200Error(f"compute_sdf: {L.wb_last_error().decode()}")
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     with _stage("mesh_sdf"):
-        A.check(L.wb_mesh_sdf(A.ptr(tris), tris.shape[0], A.ptr(pts), pts.shape[0], A.ptr(ws), nbytes, A.ptr(out), A.stream()))
+        L.wb_mesh_sdf(A.ptr(tris), tris.shape[0], A.ptr(pts), pts.shape[0], A.ptr(ws), nbytes, A.ptr(out), A.stream())
     return out

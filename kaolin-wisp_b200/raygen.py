@@ -33,8 +33,8 @@ def look_at_rays(f, t, height: int, width: int, mode: str = 'persp', fov: float 
     A.require_device(origins)
     v3 = lambda a: (C.c_float * 3)(*[float(x) for x in a])
     with torch.cuda.device(dev):
-        A.check(A.lib().wb_raygen_lookat(v3(fo), v3(view), v3(right), v3(up), C.c_float(float(np.float32(np.tan(np.radians(fov / 2))))),
-                                         C.c_int32(height), C.c_int32(width), C.c_int32(1 if mode == 'ortho' else 0), A.ptr(origins), A.ptr(dirs), A.stream()))
+        A.lib().wb_raygen_lookat(v3(fo), v3(view), v3(right), v3(up), float(np.float32(np.tan(np.radians(fov / 2)))),
+                                 height, width, 1 if mode == 'ortho' else 0, A.ptr(origins), A.ptr(dirs), A.stream())
     return Rays(origins, dirs, dist_min=dist_min, dist_max=dist_max)
 
 
@@ -51,7 +51,6 @@ def pinhole_rays(cam_pos, cam_to_world_rot, fov_h_deg: float, img_height: int, i
     A.require_device(origins)
     Rm = np.asarray(cam_to_world_rot, np.float32).reshape(9)
     with torch.cuda.device(dev):
-        A.check(A.lib().wb_raygen_pinhole((C.c_float * 3)(*[float(x) for x in cam_pos]), (C.c_float * 9)(*[float(x) for x in Rm]), C.c_float(x0), C.c_float(y0),
-                                          C.c_float(tanh), C.c_float(tanv), C.c_int32(img_height), C.c_int32(img_width), C.c_int32(res_y), C.c_int32(res_x),
-                                          A.ptr(origins), A.ptr(dirs), A.stream()))
+        A.lib().wb_raygen_pinhole((C.c_float * 3)(*[float(x) for x in cam_pos]), (C.c_float * 9)(*[float(x) for x in Rm]), x0, y0,
+                                  tanh, tanv, img_height, img_width, res_y, res_x, A.ptr(origins), A.ptr(dirs), A.stream())
     return Rays(origins, dirs, dist_min=near, dist_max=far)

@@ -19,7 +19,6 @@ Fields outside the fused path (ops.nef_spec is None) fall back to autograd + the
 from __future__ import annotations
 
 import contextlib
-import ctypes as C
 from typing import Optional
 
 import torch
@@ -61,8 +60,7 @@ class NativeAdam:
         segs = (A.AdamSegment * n)()
         _fill_segments(segs, self.entries, grads, self.lr_scale, exp_avg=self.exp_avg, exp_avg_sq=self.exp_avg_sq)
         self.t += 1
-        A.check(getattr(A.lib(), self._entry)(segs, C.c_int32(n), C.c_float(self.betas[0]), C.c_float(self.betas[1]), C.c_float(self.eps), C.c_int32(self.t),
-                                              C.c_float(grad_scale), C.c_int32(int(zero_grad)), A.stream()))
+        getattr(A.lib(), self._entry)(segs, n, self.betas[0], self.betas[1], self.eps, self.t, grad_scale, int(zero_grad), A.stream())
 
 
 class NativeAdamW(NativeAdam):
@@ -88,8 +86,7 @@ class NativeRMSprop:
         segs = (A.RMSpropSegment * n)()
         _fill_segments(segs, self.entries, grads, self.lr_scale, square_avg=self.square_avg, momentum_buffer=self.momentum_buffer)
         self.t += 1
-        A.check(A.lib().wb_rmsprop_step(segs, C.c_int32(n), C.c_float(self.alpha), C.c_float(self.eps), C.c_float(self.momentum),
-                                        C.c_float(grad_scale), C.c_int32(int(zero_grad)), A.stream()))
+        A.lib().wb_rmsprop_step(segs, n, self.alpha, self.eps, self.momentum, grad_scale, int(zero_grad), A.stream())
 
 
 OPTIMIZERS = ("adam", "adamw", "rmsprop")
@@ -218,14 +215,14 @@ class MultiviewStep:
             g_used = self._cl[1]
         oct, trinkets = ops._grid_context(nef, spec)
         desc, keep = spec.desc(gt, self.dens_flat, self.col_flat, oct, trinkets, grads=g_used, layout=layout)
-        blob = torch.empty(int(L.wb_rf_param_blob_floats(C.byref(desc), C.c_int32(precision))), dtype=torch.float32, device=dev)
-        A.check(L.wb_rf_pack_params(C.byref(desc), C.c_int32(precision), A.ptr(blob), A.stream()))
+        blob = torch.empty(int(L.wb_rf_param_blob_floats(desc, precision)), dtype=torch.float32, device=dev)
+        L.wb_rf_pack_params(desc, precision, A.ptr(blob), A.stream())
         rec_t, rec_delta, rec_ray = ops.march_fill_records(ms, dev)
         Scap = ops._bucket(S)
         shaded = ops._empty_s(S, (4,), torch.float32, dev)
         g_sh = ops._empty_s(S, (4,), torch.float32, dev)
-        wsb = int(L.wb_rf_workspace_bytes(C.byref(desc), C.c_int32(precision), C.c_int64(R), C.c_int64(Scap), C.c_int32(1)))
-        fb = int(L.wb_rf_feat_bytes(C.byref(desc), C.c_int32(precision), C.c_int64(Scap)))
+        wsb = int(L.wb_rf_workspace_bytes(desc, precision, R, Scap, 1))
+        fb = int(L.wb_rf_feat_bytes(desc, precision, Scap))
         if wsb < 0 or fb < 0:
             raise A.WispB200Error(L.wb_last_error().decode())
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev) if wsb > 0 else None
@@ -237,25 +234,25 @@ class MultiviewStep:
         bgv = ops._bg3(tr.bg_color)
         tgt = A.f32c(img_gts)
         with ops._stage("shade_fwd"):
-            A.check(L.wb_rf_shade_fwd(C.byref(desc), A.ptr(blob), C.c_int32(precision), C.byref(ms.rays), A.ptr(rec_t), A.ptr(rec_ray), C.c_int64(S),
-                                      A.ptr(shaded), A.ptr(feat), A.ptr(ws), A.stream()))
+            L.wb_rf_shade_fwd(desc, A.ptr(blob), precision, ms.rays, A.ptr(rec_t), A.ptr(rec_ray), S,
+                              A.ptr(shaded), A.ptr(feat), A.ptr(ws), A.stream())
         with ops._stage("composite_fwd"):
-            A.check(L.wb_composite_fwd(A.ptr(shaded), A.ptr(rec_t), A.ptr(rec_delta), A.ptr(ms.offsets), C.c_int64(R), bgv, A.ptr(rgb), None, A.ptr(alpha),
-                                       A.ptr(hit), A.stream()))
+            L.wb_composite_fwd(A.ptr(shaded), A.ptr(rec_t), A.ptr(rec_delta), A.ptr(ms.offsets), R, bgv, A.ptr(rgb), None, A.ptr(alpha),
+                               A.ptr(hit), A.stream())
         self._scalars.zero_()
         # rgb_loss.mean() over the GLOBAL batch (SURVEY 8(e)): every rank contributes sum / (3 * R * world); 'samples' divides by the local count
         inv = 1.0 / (3.0 * R * world) if self.loss_denom == "rays" else 1.0 / (max(S, 1) * world)
         with ops._stage("composite_bwd"):
-            A.check(L.wb_composite_bwd_loss(A.ptr(shaded), A.ptr(rec_t), A.ptr(rec_delta), A.ptr(ms.offsets), C.c_int64(R), bgv, A.ptr(rgb), A.ptr(tgt),
-                                            C.c_int32(LOSS_TYPES[self.loss_type]), C.c_float(inv), A.ptr(g_sh), A.ptr(self.absmax), A.ptr(self.loss_buf), A.stream()))
+            L.wb_composite_bwd_loss(A.ptr(shaded), A.ptr(rec_t), A.ptr(rec_delta), A.ptr(ms.offsets), R, bgv, A.ptr(rgb), A.ptr(tgt),
+                                    LOSS_TYPES[self.loss_type], inv, A.ptr(g_sh), A.ptr(self.absmax), A.ptr(self.loss_buf), A.stream())
         g_table = g_used[0] if spec.kind == "hash" else None
         if S > 0:
             if precision == 1:
-                A.check(L.wb_rf_loss_scale(A.ptr(self.absmax), A.ptr(self.scale), A.stream()))
-                L.wb_rf_workspace_holds_ray_rows(C.c_int32(1))      # same workspace, same rays as the forward above
+                L.wb_rf_loss_scale(A.ptr(self.absmax), A.ptr(self.scale), A.stream())
+                L.wb_rf_workspace_holds_ray_rows(1)      # same workspace, same rays as the forward above
             with ops._stage("shade_bwd"):      # precision 1: decoder backward + table scatter in one kernel where the shape allows
-                A.check(L.wb_rf_shade_bwd(C.byref(desc), A.ptr(blob), C.c_int32(precision), C.byref(ms.rays), A.ptr(rec_t), A.ptr(rec_ray), C.c_int64(S), A.ptr(g_sh),
-                                          A.ptr(self.scale) if precision == 1 else None, A.ptr(feat), A.ptr(ws), A.ptr(g_table), A.ptr(self.g_dens), A.ptr(self.g_col), A.stream()))
+                L.wb_rf_shade_bwd(desc, A.ptr(blob), precision, ms.rays, A.ptr(rec_t), A.ptr(rec_ray), S, A.ptr(g_sh),
+                                  A.ptr(self.scale) if precision == 1 else None, A.ptr(feat), A.ptr(ws), A.ptr(g_table), A.ptr(self.g_dens), A.ptr(self.g_col), A.stream())
         if layout:          # -> self.g_grid (reference layout, overwritten with the accumulated channel-last gradients)
             ops.triplane_relayout(g_used, False, out=self.g_grid)
         self.last_rgb, self.last_alpha, self.last_hit = rgb, alpha, hit

@@ -68,8 +68,8 @@ def _fwd(W, b, bg, with_depth=True):
     dout = torch.full((b.R,), SENTINEL, device="cuda") if with_depth else None
     alpha = torch.full((b.R,), SENTINEL, device="cuda")
     hit = torch.full((b.R,), 3, dtype=torch.uint8, device="cuda")
-    A.check(A.lib().wb_composite_fwd(A.ptr(b.sh), A.ptr(b.dp), A.ptr(b.dl), A.ptr(b.off), C.c_int64(b.R), _bg3(bg), A.ptr(rgb), A.ptr(dout),
-                                     A.ptr(alpha), A.ptr(hit), A.stream()))
+    A.lib().wb_composite_fwd(A.ptr(b.sh), A.ptr(b.dp), A.ptr(b.dl), A.ptr(b.off), b.R, _bg3(bg), A.ptr(rgb), A.ptr(dout),
+                             A.ptr(alpha), A.ptr(hit), A.stream())
     return rgb, dout, alpha, hit
 
 
@@ -85,8 +85,8 @@ def _bwd(W, b, bg, g_rgb, g_depth, g_alpha):
     A = W._cabi
     g = _gsh(b)
     absmax = torch.zeros(1, device="cuda")
-    A.check(A.lib().wb_composite_bwd(A.ptr(b.sh), A.ptr(b.dp), A.ptr(b.dl), A.ptr(b.off), C.c_int64(b.R), _bg3(bg), A.ptr(g_rgb),
-                                     A.ptr(g_depth), A.ptr(g_alpha), A.ptr(g), A.ptr(absmax), A.stream()))
+    A.lib().wb_composite_bwd(A.ptr(b.sh), A.ptr(b.dp), A.ptr(b.dl), A.ptr(b.off), b.R, _bg3(bg), A.ptr(g_rgb),
+                             A.ptr(g_depth), A.ptr(g_alpha), A.ptr(g), A.ptr(absmax), A.stream())
     _tail_ok(g, b)
     return g[:b.S], absmax
 
@@ -95,8 +95,8 @@ def _bwd_loss(W, b, bg, rgb_pred, target, loss_type, inv):
     A = W._cabi
     g = _gsh(b)
     absmax, loss = torch.zeros(1, device="cuda"), torch.zeros(1, device="cuda")
-    A.check(A.lib().wb_composite_bwd_loss(A.ptr(b.sh), A.ptr(b.dp), A.ptr(b.dl), A.ptr(b.off), C.c_int64(b.R), _bg3(bg), A.ptr(rgb_pred),
-                                          A.ptr(target), C.c_int32(loss_type), C.c_float(inv), A.ptr(g), A.ptr(absmax), A.ptr(loss), A.stream()))
+    A.lib().wb_composite_bwd_loss(A.ptr(b.sh), A.ptr(b.dp), A.ptr(b.dl), A.ptr(b.off), b.R, _bg3(bg), A.ptr(rgb_pred),
+                                  A.ptr(target), loss_type, inv, A.ptr(g), A.ptr(absmax), A.ptr(loss), A.stream())
     _tail_ok(g, b)
     return g[:b.S], absmax, loss
 
@@ -203,8 +203,7 @@ def test_composite_bwd_loss(W, loss, denom, shape):
 
 # ---- Adam ---------------------------------------------------------------------------------------------------------------------
 def _adam_call(W, segs, n, b1, b2, eps, step, gs, zero_grad):
-    return W._cabi.lib().wb_adam_step(segs, C.c_int32(n), C.c_float(b1), C.c_float(b2), C.c_float(eps), C.c_int32(step), C.c_float(gs),
-                                      C.c_int32(zero_grad), W._cabi.stream())
+    return W._cabi.lib().wb_adam_step(segs, n, b1, b2, eps, step, gs, zero_grad, W._cabi.stream())
 
 
 def _addr(t):
@@ -247,7 +246,7 @@ def test_adam_segments(W, step, zero_grad):
             t[key] = buf[off:off + n]
         segs[i] = _seg(A, t["p"], t["g"], t["m"], t["v"], lr, wd)
         keep.append(t); host.append(h)
-    A.check(_adam_call(W, segs, len(plan), b1, b2, eps, step, gs, zero_grad))
+    _adam_call(W, segs, len(plan), b1, b2, eps, step, gs, zero_grad)
     torch.cuda.synchronize()
     for (n, mis, lr, wd, scale), t, h in zip(plan, keep, host):
         pk, mk, vk, gk = (t[x].cpu().numpy() for x in "pmvg")
@@ -263,8 +262,8 @@ def test_adam_segments(W, step, zero_grad):
         assert np.array_equal(gk, np.zeros_like(gk) if zero_grad else h["g"]), name
 
 
-def test_adam_segment_count_and_refusals(W):
-    """64 segments in one launch; 65 segments, nseg 0 and step 0 return WB_ERR_INVALID and launch nothing."""
+def test_adam_segment_count_and_raised_refusals(W):
+    """64 segments in one launch; 65 segments, nseg 0 and step 0 raise WispB200Error with WB_ERR_INVALID and launch nothing."""
     A = W._cabi
     segs = (A.AdamSegment * 65)()
     ts = []
@@ -274,11 +273,12 @@ def test_adam_segment_count_and_refusals(W):
         segs[i] = _seg(A, *t, 1e-3, 0.0)
         ts.append(t)
     before = A.launch_count()
-    assert _adam_call(W, segs, 65, 0.9, 0.999, 1e-8, 1, 1.0, 1) == -1
-    assert _adam_call(W, segs, 0, 0.9, 0.999, 1e-8, 1, 1.0, 1) == -1
-    assert _adam_call(W, segs, 64, 0.9, 0.999, 1e-8, 0, 1.0, 1) == -1
+    for n, step in ((65, 1), (0, 1), (64, 0)):
+        with pytest.raises(A.WispB200Error) as e:
+            _adam_call(W, segs, n, 0.9, 0.999, 1e-8, step, 1.0, 1)
+        assert e.value.status == -1
     assert A.launch_count() == before
-    A.check(_adam_call(W, segs, 64, 0.9, 0.999, 1e-8, 1, 1.0, 1))
+    _adam_call(W, segs, 64, 0.9, 0.999, 1e-8, 1, 1.0, 1)
     torch.cuda.synchronize()
     for i, (p, g, m, v) in enumerate(ts):
         pk = p.cpu().numpy()

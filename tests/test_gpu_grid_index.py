@@ -7,7 +7,6 @@ autograd functions, against tests/grid_index_reference.py:
   - wb_octree_build_bits / _coarse word for word against the exact masks, and the ensure_bits bounding box;
   - wb_prune_samples bit for bit (explicit u and the counter-based stream) and wb_prune_update with torch.max's NaN rule.
 Each hash case prints one GRIDINDEX line: max |k - c| / r over the entries with r > 0 and the median radius."""
-import ctypes as C
 import zlib
 
 import numpy as np
@@ -66,7 +65,7 @@ def _fwd(W, coords, table, res, bw, begin):
     c = dev(coords)
     feats = torch.full((c.shape[0], L * F), float("nan"), device="cuda")
     d = _desc(W, table, res, bw, begin)
-    A.check(A.lib().wb_hashgrid_fwd(A.ptr(c), C.c_int64(c.shape[0]), C.byref(d), A.ptr(feats), A.stream()))
+    A.lib().wb_hashgrid_fwd(A.ptr(c), c.shape[0], d, A.ptr(feats), A.stream())
     torch.cuda.synchronize()
     return feats.cpu().numpy()
 
@@ -75,7 +74,7 @@ def _bwd(W, coords, go, table, gt0, res, bw, begin):
     A = W._cabi
     c, g, gt = dev(coords), dev(go), dev(gt0)
     d = _desc(W, table, res, bw, begin)
-    A.check(A.lib().wb_hashgrid_bwd(A.ptr(c), C.c_int64(c.shape[0]), C.byref(d), A.ptr(g), A.ptr(gt), A.stream()))
+    A.lib().wb_hashgrid_bwd(A.ptr(c), c.shape[0], d, A.ptr(g), A.ptr(gt), A.stream())
     torch.cuda.synchronize()
     return gt.cpu().numpy()
 
@@ -217,7 +216,7 @@ def _build_bits(W, pts, level, n=None):
     bits = torch.zeros((8 ** level + 31) // 32, dtype=torch.int32, device="cuda")
     p = dev(pts.astype(np.int16))
     n = pts.shape[0] if n is None else n
-    A.check(A.lib().wb_octree_build_bits(A.ptr(p), C.c_int64(n), C.c_int32(level), A.ptr(bits), A.stream()))
+    A.lib().wb_octree_build_bits(A.ptr(p), n, level, A.ptr(bits), A.stream())
     return bits.cpu().numpy().view(np.uint32)
 
 
@@ -226,7 +225,7 @@ def _build_coarse(W, pts, level, cl, n=None):
     cb = torch.zeros((8 ** cl + 31) // 32, dtype=torch.int32, device="cuda")
     p = dev(pts.astype(np.int16))
     n = pts.shape[0] if n is None else n
-    A.check(A.lib().wb_octree_build_coarse(A.ptr(p), C.c_int64(n), C.c_int32(level), C.c_int32(cl), A.ptr(cb), A.stream()))
+    A.lib().wb_octree_build_coarse(A.ptr(p), n, level, cl, A.ptr(cb), A.stream())
     return cb.cpu().numpy().view(np.uint32)
 
 
@@ -272,8 +271,8 @@ def _prune_samples(W, pts, level, u, seed):
     uu = None if u is None else dev(u)
     samples = torch.empty((N, 3), device="cuda"); dirs = torch.empty((N, 3), device="cuda")
     rec_t = torch.full((N,), float("nan"), device="cuda"); rec_ray = torch.full((N,), -1, dtype=torch.int32, device="cuda")
-    A.check(A.lib().wb_prune_samples(A.ptr(p), C.c_int64(N), C.c_int32(level), A.ptr(uu), C.c_uint32(seed), A.ptr(samples), A.ptr(dirs),
-                                     A.ptr(rec_t), A.ptr(rec_ray), A.stream()))
+    A.lib().wb_prune_samples(A.ptr(p), N, level, A.ptr(uu), seed, A.ptr(samples), A.ptr(dirs),
+                             A.ptr(rec_t), A.ptr(rec_ray), A.stream())
     torch.cuda.synchronize()
     return samples.cpu().numpy(), dirs.cpu().numpy(), rec_t.cpu().numpy(), rec_ray.cpu().numpy()
 
@@ -304,7 +303,7 @@ def _prune_update(W, dens, occ0, decay, md):
     shaded = np.zeros((N, 4), f32); shaded[:, 3] = dens
     sh, occ = dev(shaded), dev(occ0.copy())
     keep = torch.full((N,), 7, dtype=torch.uint8, device="cuda")
-    A.check(A.lib().wb_prune_update(A.ptr(sh), C.c_int64(N), C.c_float(decay), C.c_float(md), A.ptr(occ), A.ptr(keep), A.stream()))
+    A.lib().wb_prune_update(A.ptr(sh), N, decay, md, A.ptr(occ), A.ptr(keep), A.stream())
     torch.cuda.synchronize()
     return occ.cpu().numpy(), keep.cpu().numpy()
 

@@ -9,7 +9,6 @@
   - ImageStep: two native launches per step, a 5-step trajectory against autograd + torch.optim.AdamW with init_optimizer's groups and
     MultiStepLR, precision=1 against autograd under autocast, the fall-back of a two-hidden-layer field, and one fit of a procedural
     512^2 image (native and autograd on the same batches; prints an IMAGEFIT line with both PSNRs)."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -68,7 +67,7 @@ def test_hashgrid2d_fwd_bwd(W, F, res, bw, cd, nr):
     desc = grid_desc(W, tt, res, begin, bw)
     L = len(res)
     out = torch.empty((coords.shape[0], L * F), dtype=torch.float32, device="cuda")
-    W._cabi.check(W._cabi.lib().wb_hashgrid2d_fwd(W._cabi.ptr(ct), C.c_int64(coords.shape[0]), C.byref(desc), W._cabi.ptr(out), W._cabi.stream()))
+    W._cabi.lib().wb_hashgrid2d_fwd(W._cabi.ptr(ct), coords.shape[0], desc, W._cabi.ptr(out), W._cabi.stream())
     emu, cen, rad = IR.hashgrid2d_fwd(coords, table, res, bw, begin)
     got = out.cpu().numpy()
     assert np.array_equal(got.view(np.uint32), emu.view(np.uint32)), np.argwhere(got != emu)[:5]
@@ -77,8 +76,8 @@ def test_hashgrid2d_fwd_bwd(W, F, res, bw, cd, nr):
     gf[::7] = 0.0
     g0 = (rng.standard_normal(table.shape) * 0.1).astype(f32)
     gt, gft = dev(g0), dev(gf)
-    W._cabi.check(W._cabi.lib().wb_hashgrid2d_bwd(W._cabi.ptr(ct), C.c_int64(coords.shape[0]), C.byref(desc), W._cabi.ptr(gft),
-                                                  W._cabi.ptr(gt), W._cabi.stream()))
+    W._cabi.lib().wb_hashgrid2d_bwd(W._cabi.ptr(ct), coords.shape[0], desc, W._cabi.ptr(gft),
+                                    W._cabi.ptr(gt), W._cabi.stream())
     c, r, k = IR.hashgrid2d_bwd(coords, gf, g0, res, bw, begin)
     k_ = gt.cpu().numpy().astype(np.float64)
     assert np.all(np.abs(k_ - c) <= r), float((np.abs(k_ - c) - r).max())
@@ -96,7 +95,7 @@ def test_hashgrid2d_large_and_single(W):
         coords = rng.uniform(-1.05, 1.05, (N, 2)).astype(f32)
         ct = dev(coords)
         out = torch.empty((N, len(res) * F), dtype=torch.float32, device="cuda")
-        W._cabi.check(W._cabi.lib().wb_hashgrid2d_fwd(W._cabi.ptr(ct), C.c_int64(N), C.byref(desc), W._cabi.ptr(out), W._cabi.stream()))
+        W._cabi.lib().wb_hashgrid2d_fwd(W._cabi.ptr(ct), N, desc, W._cabi.ptr(out), W._cabi.stream())
         emu, _, _ = IR.hashgrid2d_fwd(coords, table, res, bw, begin)
         assert np.array_equal(out.cpu().numpy(), emu)
 
@@ -123,13 +122,13 @@ def test_hashgrid2d_rows_stay_inside_their_level(W, cd):
     tt, ct = dev(table), dev(coords)
     desc = grid_desc(W, tt, res, begin, bw)
     out = torch.empty((coords.shape[0], len(res) * F), dtype=torch.float32, device="cuda")
-    W._cabi.check(W._cabi.lib().wb_hashgrid2d_fwd(W._cabi.ptr(ct), C.c_int64(coords.shape[0]), C.byref(desc), W._cabi.ptr(out), W._cabi.stream()))
+    W._cabi.lib().wb_hashgrid2d_fwd(W._cabi.ptr(ct), coords.shape[0], desc, W._cabi.ptr(out), W._cabi.stream())
     assert torch.isfinite(out).all()
     g0 = np.zeros(table.shape, f32)
     g0[guard] = -0.0
     gt, gft = dev(g0), dev(np.ones((coords.shape[0], len(res) * F), f32))
-    W._cabi.check(W._cabi.lib().wb_hashgrid2d_bwd(W._cabi.ptr(ct), C.c_int64(coords.shape[0]), C.byref(desc), W._cabi.ptr(gft),
-                                                  W._cabi.ptr(gt), W._cabi.stream()))
+    W._cabi.lib().wb_hashgrid2d_bwd(W._cabi.ptr(ct), coords.shape[0], desc, W._cabi.ptr(gft),
+                                    W._cabi.ptr(gt), W._cabi.stream())
     k = gt.cpu().numpy()
     assert np.all(np.signbit(k[guard])) and np.all(k[guard] == 0)
 
@@ -280,8 +279,8 @@ def test_image_train_three_tiles_per_cta_and_empty_batch(W):
                           torch.zeros_like(nef.grid.codebook.feats), torch.zeros(10, device="cuda"), torch.zeros(1, device="cuda"))
     with pytest.raises(W.WispB200Error):
         ct, out = dev(coords), torch.empty(3, device="cuda")
-        W._cabi.check(W._cabi.lib().wb_image_eval(C.byref(fd[0]), C.c_int32(64), fd[2], C.c_int32(15), W._cabi.ptr(ct), C.c_int64(0),
-                                                  W._cabi.ptr(out), W._cabi.stream()))
+        W._cabi.lib().wb_image_eval(fd[0], 64, fd[2], 15, W._cabi.ptr(ct), 0,
+                                    W._cabi.ptr(out), W._cabi.stream())
 
 
 # ---- ImageStep --------------------------------------------------------------------------------------------------------------

@@ -10,7 +10,6 @@ Every output is bit-exact against the C oracle, and the oracle-independent state
     changes a hit mask;
   - raytrace nuggets == the exact nuggets up to ambiguous cells, with entry / exit within the rounding radius.
 Each case prints one TRAVREPORT line: counts, ambiguous cells and max |k - exact| / radius (<= 1)."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -258,9 +257,9 @@ def test_scan_counts(W, R):
     L = W._cabi.lib()
     counts = dev(c) if R else torch.zeros(1, dtype=torch.int32, device="cuda")
     offsets = torch.full((R + 1,), -7, dtype=torch.int64, device="cuda")
-    wsb = int(L.wb_scan_workspace_bytes(C.c_int64(R)))
+    wsb = int(L.wb_scan_workspace_bytes(R))
     ws = torch.empty(wsb, dtype=torch.uint8, device="cuda")
-    W._cabi.check(L.wb_scan_counts(W._cabi.ptr(counts), C.c_int64(R), W._cabi.ptr(offsets), W._cabi.ptr(ws), C.c_int64(wsb), W._cabi.stream()))
+    L.wb_scan_counts(W._cabi.ptr(counts), R, W._cabi.ptr(offsets), W._cabi.ptr(ws), wsb, W._cabi.stream())
     exp = np.concatenate([[0], np.cumsum(c.astype(np.int64))])
     assert np.array_equal(offsets.cpu().numpy(), exp)
     print(f"TRAVREPORT scan R={R} total={int(exp[-1])} ambiguous=0 max|k-exact|/radius=0 (exact)")

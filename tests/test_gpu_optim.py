@@ -9,7 +9,6 @@ arguments of MultiviewStep and SDFStep, on the GPU:
     autograd route stepped by the torch optimiser and MultiStepLR, with the library launch count of the "adam" step;
   - SDFStep(optimizer="rmsprop") against the reference trainer's own eight steps (tests/golden/optim_groups.npz);
   - the defaults take the steps optimizer="adam" takes, bit for bit."""
-import ctypes as C
 import os
 
 import numpy as np
@@ -53,11 +52,19 @@ def _array(A, rule, n):
 
 
 def _call(W, rule, segs, n, eps, step, gs, zero_grad, momentum=None):
-    L, f = W._cabi.lib(), C.c_float
+    L = W._cabi.lib()
     if rule == "adamw":
-        return L.wb_adamw_step(segs, C.c_int32(n), f(B1), f(B2), f(eps), C.c_int32(step), f(gs), C.c_int32(zero_grad), W._cabi.stream())
+        return L.wb_adamw_step(segs, n, B1, B2, eps, step, gs, zero_grad, W._cabi.stream())
     mom = (MOM if rule == "rmsprop_m" else 0.0) if momentum is None else momentum
-    return L.wb_rmsprop_step(segs, C.c_int32(n), f(ALPHA), f(eps), f(mom), f(gs), C.c_int32(zero_grad), W._cabi.stream())
+    return L.wb_rmsprop_step(segs, n, ALPHA, eps, mom, gs, zero_grad, W._cabi.stream())
+
+
+def _refused(W, *args, **kw) -> str:
+    """_call(*args) fails with WB_ERR_INVALID: -> its message."""
+    with pytest.raises(W._cabi.WispB200Error) as e:
+        _call(W, *args, **kw)
+    assert e.value.status == -1
+    return str(e.value)
 
 
 def _emulate(rule, h, lr, wd, eps, step, gs):
@@ -99,7 +106,7 @@ def test_segments_bit_exact(W, rule, step, zero_grad):
         segs[i] = _seg(A, rule, t["p"], t["g"], t["a"], t["b"] if has_b else None, lr, wd)
         keep.append(t); host.append(h)
     before = A.launch_count()
-    A.check(_call(W, rule, segs, len(plan), eps, step, gs, zero_grad))
+    _call(W, rule, segs, len(plan), eps, step, gs, zero_grad)
     assert A.launch_count() == before + 1
     torch.cuda.synchronize()
     for (n, mis, lr, wd, scale), t, h in zip(plan, keep, host):
@@ -116,9 +123,9 @@ def test_segments_bit_exact(W, rule, step, zero_grad):
 
 
 @pytest.mark.parametrize("rule", RULES)
-def test_segment_count_and_refusals(W, rule):
-    """64 segments in one launch; 65 segments, nseg 0, a null pointer, AdamW's step 0 and momentum > 0 without a buffer return
-    WB_ERR_INVALID and launch nothing."""
+def test_segment_count_and_raised_refusals(W, rule):
+    """64 segments in one launch; 65 segments, nseg 0, a null pointer, AdamW's step 0 and momentum > 0 without a buffer raise
+    WispB200Error with WB_ERR_INVALID and launch nothing."""
     A = W._cabi
     segs = _array(A, rule, 65)
     ts = []
@@ -128,20 +135,19 @@ def test_segment_count_and_refusals(W, rule):
         segs[i] = _seg(A, rule, *t, 1e-3, 0.0)
         ts.append(t)
     before = A.launch_count()
-    assert _call(W, rule, segs, 65, 1e-8, 1, 1.0, 1) == -1
-    assert _call(W, rule, segs, 0, 1e-8, 1, 1.0, 1) == -1
-    assert _call(W, rule, None, 1, 1e-8, 1, 1.0, 1) == -1
+    _refused(W, rule, segs, 65, 1e-8, 1, 1.0, 1)
+    _refused(W, rule, segs, 0, 1e-8, 1, 1.0, 1)
+    _refused(W, rule, None, 1, 1e-8, 1, 1.0, 1)
     if rule == "adamw":
-        assert _call(W, rule, segs, 64, 1e-8, 0, 1.0, 1) == -1
+        _refused(W, rule, segs, 64, 1e-8, 0, 1.0, 1)
     if rule == "rmsprop":
-        assert _call(W, rule, segs, 64, 1e-8, 1, 1.0, 1, momentum=0.9) == -1
-        assert b"momentum" in A.lib().wb_last_error()
+        assert "momentum" in _refused(W, rule, segs, 64, 1e-8, 1, 1.0, 1, momentum=0.9)
     bad = _array(A, rule, 1)
     bad[0] = _seg(A, rule, *ts[3], 1e-3, 0.0)
     bad[0].grad = None
-    assert _call(W, rule, bad, 1, 1e-8, 1, 1.0, 1) == -1
+    _refused(W, rule, bad, 1, 1e-8, 1, 1.0, 1)
     assert A.launch_count() == before
-    A.check(_call(W, rule, segs, 64, 1e-8, 1, 1.0, 1))
+    _call(W, rule, segs, 64, 1e-8, 1, 1.0, 1)
     torch.cuda.synchronize()
     for i, (p, g, a, b) in enumerate(ts):
         pk = p.cpu().numpy()

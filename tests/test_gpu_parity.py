@@ -528,12 +528,11 @@ def weight_image(Wm):
 
 
 def _selftest(W, mode, rows, N, K, a, b):
-    import ctypes as C
     D = torch.zeros((128 if mode == 2 else rows, N), dtype=torch.float32, device="cuda")
     ta, tb = dev(a), dev(b)
     A = W._cabi
     m = mode | (4 if rows == 64 else 0)
-    A.check(A.lib().wb_tc_selftest(A.ptr(ta), C.c_int(a.size), A.ptr(tb), C.c_int(b.size), A.ptr(D), C.c_int(N), C.c_int(K), C.c_int(m), A.stream()))
+    A.lib().wb_tc_selftest(A.ptr(ta), a.size, A.ptr(tb), b.size, A.ptr(D), N, K, m, A.stream())
     torch.cuda.synchronize()
     return D.cpu().numpy()
 

@@ -243,10 +243,10 @@ class Setup:
 
     # ---- calls ----------------------------------------------------------------------------------------------------------------
     def blob(self, precision):
-        n = int(self.L.wb_rf_param_blob_floats(C.byref(self.desc), C.c_int32(precision)))
+        n = int(self.L.wb_rf_param_blob_floats(self.desc, precision))
         assert n > 0, self.L.wb_last_error()
         b = torch.empty(n, dtype=torch.float32, device="cuda")
-        self.A.check(self.L.wb_rf_pack_params(C.byref(self.desc), C.c_int32(precision), self.A.ptr(b), self.A.stream()))
+        self.L.wb_rf_pack_params(self.desc, precision, self.A.ptr(b), self.A.stream())
         return b
 
     def zero(self):
@@ -260,8 +260,8 @@ class Setup:
     def fwd(self, precision, blob, feat=None, ws=None):
         shaded = torch.full((max(self.S, 1), 4), 7.0, dtype=torch.float32, device="cuda")
         p = self.A.ptr
-        self.A.check(self.L.wb_rf_shade_fwd(C.byref(self.desc), p(blob), C.c_int32(precision), C.byref(self.rays), p(self.t_rec_t), p(self.t_rec_ray),
-                                            C.c_int64(self.S), p(shaded), p(feat), p(ws), self.A.stream()))
+        self.L.wb_rf_shade_fwd(self.desc, p(blob), precision, self.rays, p(self.t_rec_t), p(self.t_rec_ray),
+                               self.S, p(shaded), p(feat), p(ws), self.A.stream())
         torch.cuda.synchronize()
         return shaded.cpu().numpy().astype(np.float64)[:self.S]
 
@@ -270,8 +270,8 @@ class Setup:
         tg = dev(np.asarray(g, np.float32))
         p = self.A.ptr
         gt = self.grads[0] if self.c.kind == "hash" else None      # triplanar / octree: the gradients named in the description
-        self.A.check(self.L.wb_rf_shade_bwd(C.byref(self.desc), p(blob), C.c_int32(precision), C.byref(self.rays), p(self.t_rec_t), p(self.t_rec_ray),
-                                            C.c_int64(self.S), p(tg), p(scale), p(feat), p(ws), p(gt), p(gd), p(gc), self.A.stream()))
+        self.L.wb_rf_shade_bwd(self.desc, p(blob), precision, self.rays, p(self.t_rec_t), p(self.t_rec_ray),
+                               self.S, p(tg), p(scale), p(feat), p(ws), p(gt), p(gd), p(gc), self.A.stream())
         torch.cuda.synchronize()
         return gd.cpu().numpy().astype(np.float64), gc.cpu().numpy().astype(np.float64), self.grid_grads()
 
@@ -317,16 +317,16 @@ def run_precision0(s: Setup, report, rng, in_order=True):
 
 def run_precision1(s: Setup, report, rng):
     c, A, L, p = s.c, s.A, s.L, s.A.ptr
-    bwd = int(L.wb_rf_precision_supported(C.byref(s.desc), C.c_int32(1), C.c_int32(1)))
-    if not int(L.wb_rf_precision_supported(C.byref(s.desc), C.c_int32(1), C.c_int32(0))):
+    bwd = int(L.wb_rf_precision_supported(s.desc, 1, 1))
+    if not int(L.wb_rf_precision_supported(s.desc, 1, 0)):
         report.append("p1 refused")
         return
     blob = s.blob(1)
     I0 = s.dens_dims[0]
     Kp0, Kc = -(-I0 // 16) * 16, -(-s.col_dims[0] // 16) * 16
-    wsb = int(L.wb_rf_workspace_bytes(C.byref(s.desc), C.c_int32(1), C.c_int64(c.R), C.c_int64(s.S), C.c_int32(bwd)))
+    wsb = int(L.wb_rf_workspace_bytes(s.desc, 1, c.R, s.S, bwd))
     ws = torch.zeros(wsb, dtype=torch.uint8, device="cuda")
-    fb = int(L.wb_rf_feat_bytes(C.byref(s.desc), C.c_int32(1), C.c_int64(s.S))) if bwd else Kp0 * 2 * s.S + 256
+    fb = int(L.wb_rf_feat_bytes(s.desc, 1, s.S)) if bwd else Kp0 * 2 * s.S + 256
     feat = torch.full((fb,), 0xFF, dtype=torch.uint8, device="cuda")
     shaded = s.fwd(1, blob, feat, ws)
     X = feat[:2 * Kp0 * s.S].view(torch.float16).reshape(Kp0 // 8, s.S, 8).permute(1, 0, 2).reshape(s.S, Kp0).float().cpu().numpy().astype(np.float64)
@@ -344,7 +344,7 @@ def run_precision1(s: Setup, report, rng):
     g = _g_shaded(s, rng)
     absmax = torch.tensor([float(np.abs(g).max())], dtype=torch.float32, device="cuda")
     scale_t = torch.empty(1, dtype=torch.float32, device="cuda")
-    A.check(L.wb_rf_loss_scale(p(absmax), p(scale_t), A.stream()))
+    L.wb_rf_loss_scale(p(absmax), p(scale_t), A.stream())
     scale = float(scale_t.item())
     tg = dev(g)
     sms = torch.cuda.get_device_properties(0).multi_processor_count
@@ -360,10 +360,10 @@ def run_precision1(s: Setup, report, rng):
         return s.grid_reference(gx, np.zeros_like(gx), RF.SCAN_LEVELS)
     # two stages
     gd, gc = s.zero()
-    A.check(L.wb_rf_decoder_bwd(C.byref(s.desc), p(blob), C.byref(s.rays), p(s.t_rec_t), p(s.t_rec_ray), C.c_int64(s.S), p(tg), p(scale_t),
-                                p(feat), p(ws), p(gd), p(gc), A.stream()))
-    A.check(L.wb_rf_table_scatter(C.byref(s.desc), C.byref(s.rays), p(s.t_rec_t), p(s.t_rec_ray), C.c_int64(s.S), p(scale_t), p(ws), None,
-                                  A.stream()))
+    L.wb_rf_decoder_bwd(s.desc, p(blob), s.rays, p(s.t_rec_t), p(s.t_rec_ray), s.S, p(tg), p(scale_t),
+                        p(feat), p(ws), p(gd), p(gc), A.stream())
+    L.wb_rf_table_scatter(s.desc, s.rays, p(s.t_rec_t), p(s.t_rec_ray), s.S, p(scale_t), p(ws), None,
+                          A.stream())
     torch.cuda.synchronize()
     pl = planes()
     _inside("p1 grad_dens", gd.cpu().numpy(), *bw["dens"], report)
@@ -428,10 +428,10 @@ def test_precision0_no_samples_touches_nothing(W):
     g = torch.zeros((1, 4), device="cuda")
     A, L, p = s.A, s.L, s.A.ptr
     blob = s.blob(0)
-    A.check(L.wb_rf_shade_fwd(C.byref(s.desc), p(blob), C.c_int32(0), C.byref(s.rays), p(s.t_rec_t), p(s.t_rec_ray), C.c_int64(0), p(shaded),
-                              None, None, A.stream()))
-    A.check(L.wb_rf_shade_bwd(C.byref(s.desc), p(blob), C.c_int32(0), C.byref(s.rays), p(s.t_rec_t), p(s.t_rec_ray), C.c_int64(0), p(g), None,
-                              None, None, None, p(gd), p(gc), A.stream()))
+    L.wb_rf_shade_fwd(s.desc, p(blob), 0, s.rays, p(s.t_rec_t), p(s.t_rec_ray), 0, p(shaded),
+                      None, None, A.stream())
+    L.wb_rf_shade_bwd(s.desc, p(blob), 0, s.rays, p(s.t_rec_t), p(s.t_rec_ray), 0, p(g), None,
+                      None, None, None, p(gd), p(gc), A.stream())
     torch.cuda.synchronize()
     for t in [shaded, gd, gc] + s.grads:
         assert bool((t == sentinel).all())
@@ -451,11 +451,11 @@ def test_unfused_triplane_vs_interval_reference(W, fdim):
     gp = (C.c_void_p * (3 * nl))(*[t.data_ptr() for t in gplanes])
     coords = dev(s.pos)
     feats = torch.empty((s.S, 3 * nl * fdim), dtype=torch.float32, device="cuda")
-    A.check(L.wb_triplane_fwd(p(coords), C.c_int64(s.S), C.c_int32(nl), C.c_int32(fdim), res, pp, p(feats), A.stream()))
+    L.wb_triplane_fwd(p(coords), s.S, nl, fdim, res, pp, p(feats), A.stream())
     rng = np.random.default_rng(fdim)
     go = rng.standard_normal((s.S, 3 * nl * fdim)).astype(np.float32)
     go[rng.random(go.shape) < 0.1] = 0.0
-    A.check(L.wb_triplane_bwd(p(coords), C.c_int64(s.S), C.c_int32(nl), C.c_int32(fdim), res, pp, p(dev(go)), gp, A.stream()))
+    L.wb_triplane_bwd(p(coords), s.S, nl, fdim, res, pp, p(dev(go)), gp, A.stream())
     torch.cuda.synchronize()
     report = [case.name]
     _inside("feats", feats.cpu().numpy(), *RF.triplanar_features(s.tp, s.pos), report)

@@ -247,8 +247,8 @@ def test_sdf_train_accumulates_and_n0(W):
     A = W._cabi
     d, _, _ = step.fd
     gptrs = (C.c_void_p * 1)(step.g_feats[0].data_ptr())
-    A.check(A.lib().wb_sdf_train(None, C.byref(d), C.c_int32(lod), A.ptr(c), A.ptr(g), C.c_int64(0), C.c_float(1e-3), gptrs,
-                                 A.ptr(step.g_dec), A.ptr(step.loss_buf), A.stream()))
+    A.lib().wb_sdf_train(None, d, lod, A.ptr(c), A.ptr(g), 0, 1e-3, gptrs,
+                         A.ptr(step.g_dec), A.ptr(step.loss_buf), A.stream())
     torch.cuda.synchronize()
     for a, b in zip(step.g_feats + [step.g_dec, step.loss_buf], twice):
         assert torch.equal(a, b)

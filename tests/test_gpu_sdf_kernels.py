@@ -156,8 +156,8 @@ def test_sdf_train_contract(W):
             import ctypes as C
             A = W._cabi
             gptrs = (C.c_void_p * len(gf))(*[t.data_ptr() for t in gf])
-            A.check(A.lib().wb_sdf_train(C.byref(fd[1].desc()), C.byref(fd[0]), C.c_int32(lod), A.ptr(c), A.ptr(g), C.c_int64(n),
-                                         C.c_float(1.0), gptrs, A.ptr(gp), A.ptr(loss), A.stream()))
+            A.lib().wb_sdf_train(fd[1].desc(), fd[0], lod, A.ptr(c), A.ptr(g), n,
+                                 1.0, gptrs, A.ptr(gp), A.ptr(loss), A.stream())
         torch.cuda.synchronize()
     rng = np.random.default_rng(0)
     init_f = [np.float32(2.0 ** -8) * rng.integers(-64, 64, f.shape).astype(np.float32) for f in field.feats]

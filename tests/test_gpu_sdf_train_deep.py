@@ -152,8 +152,8 @@ def test_deep_contract(W):
     import ctypes as C
     A = W._cabi
     gptrs = (C.c_void_p * len(gf))(*[t.data_ptr() for t in gf])
-    A.check(A.lib().wb_sdf_train(C.byref(fd[1].desc()), C.byref(fd[0]), C.c_int32(lod), A.ptr(c), A.ptr(g), C.c_int64(0),
-                                 C.c_float(1.0), gptrs, A.ptr(gp), A.ptr(loss), A.stream()))
+    A.lib().wb_sdf_train(fd[1].desc(), fd[0], lod, A.ptr(c), A.ptr(g), 0,
+                         1.0, gptrs, A.ptr(gp), A.ptr(loss), A.stream())
     torch.cuda.synchronize()
     assert all(np.array_equal(a.cpu().numpy(), b) for a, b in zip(gf, init_f)) and np.array_equal(gp.cpu().numpy(), init_p)
     assert float(loss) == 0.25

@@ -176,17 +176,17 @@ class Setup:
         self.t_rec_t, self.t_rec_ray = torch.from_numpy(self.rec_t).cuda(), torch.from_numpy(self.rec_ray).cuda()
         L = self.A.lib()
         self.L = L
-        nblob = int(L.wb_rf_param_blob_floats(C.byref(self.desc), C.c_int32(1)))
+        nblob = int(L.wb_rf_param_blob_floats(self.desc, 1))
         assert nblob > 0, L.wb_last_error()
         self.blob = torch.empty(nblob, dtype=torch.float32, device="cuda")
-        self.A.check(L.wb_rf_pack_params(C.byref(self.desc), C.c_int32(1), self.A.ptr(self.blob), self.A.stream()))
+        L.wb_rf_pack_params(self.desc, 1, self.A.ptr(self.blob), self.A.stream())
         r16 = lambda v: -(-v // 16) * 16
         self.Kp0, self.Kc = r16(dens[0]), r16(col[0])
         self.planes = (min(self.lod_idx, c.L) if c.multiscale == "cat" else 1)
-        wsb = int(L.wb_rf_workspace_bytes(C.byref(self.desc), C.c_int32(1), C.c_int64(c.R), C.c_int64(S), C.c_int32(1 if c.backward else 0)))
+        wsb = int(L.wb_rf_workspace_bytes(self.desc, 1, c.R, S, 1 if c.backward else 0))
         assert wsb > 0
         self.ws = torch.zeros(wsb, dtype=torch.uint8, device="cuda")
-        fb = int(L.wb_rf_feat_bytes(C.byref(self.desc), C.c_int32(1), C.c_int64(S))) if c.backward else self.Kp0 * 2 * S + 256
+        fb = int(L.wb_rf_feat_bytes(self.desc, 1, S)) if c.backward else self.Kp0 * 2 * S + 256
         assert fb > 0, L.wb_last_error()
         self.feat = torch.full((fb,), 0xFF, dtype=torch.uint8, device="cuda")
         self.view = T.view_embedding(self.d[self.rec_ray], *c.view)
@@ -194,9 +194,9 @@ class Setup:
     # ---- calls ----------------------------------------------------------------------------------------------------
     def forward(self):
         shaded = torch.full((max(self.S, 1), 4), 7.0, dtype=torch.float32, device="cuda")
-        self.A.check(self.L.wb_rf_shade_fwd(C.byref(self.desc), self.A.ptr(self.blob), C.c_int32(1), C.byref(self.rays), self.A.ptr(self.t_rec_t),
-                                            self.A.ptr(self.t_rec_ray), C.c_int64(self.S), self.A.ptr(shaded), self.A.ptr(self.feat),
-                                            self.A.ptr(self.ws), self.A.stream()))
+        self.L.wb_rf_shade_fwd(self.desc, self.A.ptr(self.blob), 1, self.rays, self.A.ptr(self.t_rec_t),
+                               self.A.ptr(self.t_rec_ray), self.S, self.A.ptr(shaded), self.A.ptr(self.feat),
+                               self.A.ptr(self.ws), self.A.stream())
         torch.cuda.synchronize()
         return shaded.cpu().numpy().astype(np.float64)
 
@@ -213,7 +213,7 @@ class Setup:
     def loss_scale(self, g):
         absmax = torch.tensor([float(np.abs(g).max()) if g.size else 0.0], dtype=torch.float32, device="cuda")
         scale = torch.empty(1, dtype=torch.float32, device="cuda")
-        self.A.check(self.L.wb_rf_loss_scale(self.A.ptr(absmax), self.A.ptr(scale), self.A.stream()))
+        self.L.wb_rf_loss_scale(self.A.ptr(absmax), self.A.ptr(scale), self.A.stream())
         return scale
 
     def zeros_grads(self):
@@ -222,9 +222,9 @@ class Setup:
     def decoder_bwd(self, g, scale):
         gd, gc, _ = self.zeros_grads()
         tg = torch.from_numpy(np.ascontiguousarray(g, np.float32)).cuda()
-        self.A.check(self.L.wb_rf_decoder_bwd(C.byref(self.desc), self.A.ptr(self.blob), C.byref(self.rays), self.A.ptr(self.t_rec_t),
-                                              self.A.ptr(self.t_rec_ray), C.c_int64(self.S), self.A.ptr(tg), self.A.ptr(scale), self.A.ptr(self.feat),
-                                              self.A.ptr(self.ws), self.A.ptr(gd), self.A.ptr(gc), self.A.stream()))
+        self.L.wb_rf_decoder_bwd(self.desc, self.A.ptr(self.blob), self.rays, self.A.ptr(self.t_rec_t),
+                                 self.A.ptr(self.t_rec_ray), self.S, self.A.ptr(tg), self.A.ptr(scale), self.A.ptr(self.feat),
+                                 self.A.ptr(self.ws), self.A.ptr(gd), self.A.ptr(gc), self.A.stream())
         torch.cuda.synchronize()
         off = (self.R * self.Kc * 2 + 255) // 256 * 256          # dL/dfeat planes behind the per-ray rows (include/wispb200.h)
         n = self.planes * self.S * self.c.F
@@ -233,17 +233,17 @@ class Setup:
 
     def table_scatter(self, scale):
         gt = torch.zeros_like(self.t_table)
-        self.A.check(self.L.wb_rf_table_scatter(C.byref(self.desc), C.byref(self.rays), self.A.ptr(self.t_rec_t), self.A.ptr(self.t_rec_ray),
-                                                C.c_int64(self.S), self.A.ptr(scale), self.A.ptr(self.ws), self.A.ptr(gt), self.A.stream()))
+        self.L.wb_rf_table_scatter(self.desc, self.rays, self.A.ptr(self.t_rec_t), self.A.ptr(self.t_rec_ray),
+                                   self.S, self.A.ptr(scale), self.A.ptr(self.ws), self.A.ptr(gt), self.A.stream())
         torch.cuda.synchronize()
         return gt.cpu().numpy().astype(np.float64)
 
     def shade_bwd(self, g, scale):
         gd, gc, gt = self.zeros_grads()
         tg = torch.from_numpy(np.ascontiguousarray(g, np.float32)).cuda()
-        self.A.check(self.L.wb_rf_shade_bwd(C.byref(self.desc), self.A.ptr(self.blob), C.c_int32(1), C.byref(self.rays), self.A.ptr(self.t_rec_t),
-                                            self.A.ptr(self.t_rec_ray), C.c_int64(self.S), self.A.ptr(tg), self.A.ptr(scale), self.A.ptr(self.feat),
-                                            self.A.ptr(self.ws), self.A.ptr(gt), self.A.ptr(gd), self.A.ptr(gc), self.A.stream()))
+        self.L.wb_rf_shade_bwd(self.desc, self.A.ptr(self.blob), 1, self.rays, self.A.ptr(self.t_rec_t),
+                               self.A.ptr(self.t_rec_ray), self.S, self.A.ptr(tg), self.A.ptr(scale), self.A.ptr(self.feat),
+                               self.A.ptr(self.ws), self.A.ptr(gt), self.A.ptr(gd), self.A.ptr(gc), self.A.stream())
         torch.cuda.synchronize()
         return gd.cpu().numpy().astype(np.float64), gc.cpu().numpy().astype(np.float64), gt.cpu().numpy().astype(np.float64)
 
@@ -329,9 +329,9 @@ def _backward_checks(s: Setup, report, rng):
 def test_tc_decoders_vs_interval_reference(W, case):
     s = Setup(W, case)
     report = [case_id(case)]
-    supported = int(s.L.wb_rf_precision_supported(C.byref(s.desc), C.c_int32(1), C.c_int32(1)))
+    supported = int(s.L.wb_rf_precision_supported(s.desc, 1, 1))
     assert supported == int(case.backward)
-    assert int(s.L.wb_rf_precision_supported(C.byref(s.desc), C.c_int32(1), C.c_int32(0))) == 1
+    assert int(s.L.wb_rf_precision_supported(s.desc, 1, 0)) == 1
     _forward_checks(s, report)
     if case.backward:
         _backward_checks(s, report, np.random.default_rng(case.seed + 7))
@@ -359,13 +359,13 @@ def test_tc_no_samples_touches_nothing(W):
     gd, gc, gt = (torch.full_like(t, sentinel) for t in (s.t_fd, s.t_fc, s.t_table))
     g = torch.zeros((1, 4), device="cuda"); scale = torch.ones(1, device="cuda")
     A, L, p = s.A, s.L, s.A.ptr
-    A.check(L.wb_rf_shade_fwd(C.byref(s.desc), p(s.blob), C.c_int32(1), C.byref(s.rays), p(s.t_rec_t), p(s.t_rec_ray), C.c_int64(0), p(shaded),
-                              p(s.feat), p(s.ws), A.stream()))
-    A.check(L.wb_rf_decoder_bwd(C.byref(s.desc), p(s.blob), C.byref(s.rays), p(s.t_rec_t), p(s.t_rec_ray), C.c_int64(0), p(g), p(scale), p(s.feat),
-                                p(s.ws), p(gd), p(gc), A.stream()))
-    A.check(L.wb_rf_table_scatter(C.byref(s.desc), C.byref(s.rays), p(s.t_rec_t), p(s.t_rec_ray), C.c_int64(0), p(scale), p(s.ws), p(gt), A.stream()))
-    A.check(L.wb_rf_shade_bwd(C.byref(s.desc), p(s.blob), C.c_int32(1), C.byref(s.rays), p(s.t_rec_t), p(s.t_rec_ray), C.c_int64(0), p(g), p(scale),
-                              p(s.feat), p(s.ws), p(gt), p(gd), p(gc), A.stream()))
+    L.wb_rf_shade_fwd(s.desc, p(s.blob), 1, s.rays, p(s.t_rec_t), p(s.t_rec_ray), 0, p(shaded),
+                      p(s.feat), p(s.ws), A.stream())
+    L.wb_rf_decoder_bwd(s.desc, p(s.blob), s.rays, p(s.t_rec_t), p(s.t_rec_ray), 0, p(g), p(scale), p(s.feat),
+                        p(s.ws), p(gd), p(gc), A.stream())
+    L.wb_rf_table_scatter(s.desc, s.rays, p(s.t_rec_t), p(s.t_rec_ray), 0, p(scale), p(s.ws), p(gt), A.stream())
+    L.wb_rf_shade_bwd(s.desc, p(s.blob), 1, s.rays, p(s.t_rec_t), p(s.t_rec_ray), 0, p(g), p(scale),
+                      p(s.feat), p(s.ws), p(gt), p(gd), p(gc), A.stream())
     torch.cuda.synchronize()
     for t in (shaded, gd, gc, gt):
         assert bool((t == sentinel).all())
@@ -409,9 +409,9 @@ def test_ray_rows_flag_applies_to_the_next_backward_only(W):
     want = s.decoder_bwd(g, scale)
     A, L, p = s.A, s.L, s.A.ptr
     gd, gc, _ = s.zeros_grads()
-    A.check(L.wb_rf_workspace_holds_ray_rows(C.c_int32(1)))
-    A.check(L.wb_rf_decoder_bwd(C.byref(s.desc), p(s.blob), C.byref(s.rays), p(s.t_rec_t), p(s.t_rec_ray), C.c_int64(0), p(gd), p(scale),
-                                p(s.feat), p(s.ws), p(gd), p(gc), A.stream()))
+    L.wb_rf_workspace_holds_ray_rows(1)
+    L.wb_rf_decoder_bwd(s.desc, p(s.blob), s.rays, p(s.t_rec_t), p(s.t_rec_ray), 0, p(gd), p(scale),
+                        p(s.feat), p(s.ws), p(gd), p(gc), A.stream())
     s.ws.fill_(0xFF)                          # a fresh workspace: 0xFFFF is an fp16 NaN
     got = s.decoder_bwd(g, scale)
     bw = T.Reference(s.dec, X, s.view).backward(g, float(scale.item()), s.planes, 2, wgrad_n=s.wgrad_n())
@@ -440,7 +440,7 @@ def test_loss_scale_formula(W):
     absmax = torch.tensor(vals, dtype=torch.float32, device="cuda")
     out = torch.empty_like(absmax)
     for i in range(len(vals)):
-        A.check(A.lib().wb_rf_loss_scale(C.c_void_p(absmax.data_ptr() + 4 * i), C.c_void_p(out.data_ptr() + 4 * i), A.stream()))
+        A.lib().wb_rf_loss_scale(C.c_void_p(absmax.data_ptr() + 4 * i), C.c_void_p(out.data_ptr() + 4 * i), A.stream())
     got = out.cpu().numpy()
     want = np.array([_scale_formula(np.float32(v)) for v in vals], np.float32)
     bad = got != want

@@ -1,6 +1,6 @@
 """CPU tests of the product's host side: the C-ABI library loads and exports every symbol include/wispb200.h declares,
-the ctypes struct layouts match the header, the host-side SPC builder matches the oracle, and compute entry points
-refuse to run without an H100 (no CPU fallback)."""
+the ctypes prototypes and struct layouts match the header, mistyped calls are refused, the host-side SPC builder matches the
+oracle, and compute entry points refuse to run without an H100 (no CPU fallback)."""
 import ctypes as C
 import os
 import re
@@ -14,12 +14,40 @@ import wisp_b200 as W
 from oracle import oracle as O
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+STRUCTS = {"wb_nef_desc": W._cabi.NefDesc, "wb_rays": W._cabi.RaysDesc, "wb_octree": W._cabi.OctreeDesc, "wb_sdf_desc": W._cabi.SdfDesc,
+           "wb_sdf_state": W._cabi.SdfState, "wb_adam_segment": W._cabi.AdamSegment, "wb_rmsprop_segment": W._cabi.RMSpropSegment}
+# C type in the header (spaces around '*' removed) -> ctypes type; every other data pointer is c_void_p
+CTYPES = {"int32_t": C.c_int32, "int": C.c_int, "int64_t": C.c_int64, "uint32_t": C.c_uint32, "float": C.c_float, "double": C.c_double,
+          "wb_stream": C.c_void_p, "const char*": C.c_char_p, "const float*const*": C.POINTER(C.c_void_p), "float*const*": C.POINTER(C.c_void_p)}
+
+
+def _header():
+    src = open(os.path.join(ROOT, "include", "wispb200.h")).read()
+    return re.sub(r"/\*.*?\*/", "", src, flags=re.S)
 
 
 def header_functions():
-    src = open(os.path.join(ROOT, "include", "wispb200.h")).read()
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return sorted(set(re.findall(r"\b(wb_[a-z0-9_]+)\s*\(", src)))
+    return sorted(set(re.findall(r"\b(wb_[a-z0-9_]+)\s*\(", _header())))
+
+
+def header_prototypes():
+    """name -> (return type, [parameter types]) of every declaration in the header, in header order."""
+    norm = lambda t: re.sub(r"\s*\*\s*", "*", re.sub(r"\s+", " ", t.strip()))
+    out = {}
+    for ret, name, params in re.findall(r"([A-Za-z_][\w ]*?\**)\s*\b(wb_[a-z0-9_]+)\s*\(([^)]*)\)\s*;", _header()):
+        ps = [p.strip() for p in params.split(",")] if params.strip() not in ("", "void") else []
+        out[name] = (norm(ret), [norm(re.match(r"(.*?\*?)\s*\w+$", p).group(1)) for p in ps])
+    return out
+
+
+def ctype(t: str):
+    if t in CTYPES:
+        return CTYPES[t]
+    m = re.fullmatch(r"(?:const )?(wb_\w+)\*", t)
+    if m:
+        return C.POINTER(STRUCTS[m.group(1)])
+    assert re.fullmatch(r"(?:const )?\w+\*", t), t
+    return C.c_void_p
 
 
 def test_library_exports_every_declared_symbol():
@@ -31,14 +59,38 @@ def test_library_exports_every_declared_symbol():
     assert sorted(W._cabi.EXPORTS) == names
 
 
+def test_prototypes_match_header():
+    """PROTOTYPES is every declaration of the header through the type mapping, in header order; lib() installs each one, and
+    exactly the entry points returning a wb_status raise on a nonzero result."""
+    A = W._cabi
+    decl = header_prototypes()
+    assert sorted(decl) == header_functions() and list(decl) == A.EXPORTS
+    L = A.lib()
+    for name, (ret, params) in decl.items():
+        restype, argtypes = ctype(ret), [ctype(p) for p in params]
+        assert A.PROTOTYPES[name] == (restype, argtypes), name
+        fn = getattr(L, name)
+        assert fn.restype is restype and list(fn.argtypes) == argtypes, name
+        status = ret == "int" and name not in ("wb_version", "wb_rf_precision_supported")
+        assert fn.errcheck is (A._raise_on_status if status else None), name
+
+
+def test_mistyped_calls_are_refused():
+    """ctypes refuses a descriptor of another kind and a float for an integer before the library is entered."""
+    A = W._cabi
+    L = A.lib()
+    with pytest.raises(C.ArgumentError):
+        L.wb_rf_precision_supported(A.RaysDesc(), 0, 0)
+    with pytest.raises(C.ArgumentError):
+        L.wb_rf_precision_supported(A.NefDesc(), 0.0, 0)
+    assert L.wb_rf_precision_supported(A.NefDesc(), 0, 0) == 1          # precision 0 runs every decoder
+
+
 def test_struct_layouts_match_header(tmp_path):
     """Compile include/wispb200.h with the C compiler and compare sizeof/offsetof of EVERY descriptor struct with the ctypes mirrors."""
     import subprocess
-    A = W._cabi
-    structs = {"wb_nef_desc": A.NefDesc, "wb_rays": A.RaysDesc, "wb_octree": A.OctreeDesc, "wb_sdf_desc": A.SdfDesc, "wb_sdf_state": A.SdfState,
-               "wb_adam_segment": A.AdamSegment}
     lines, mine = [], []
-    for cname, cls in structs.items():
+    for cname, cls in STRUCTS.items():
         lines.append(f'printf("%zu\\n", sizeof({cname}));'); mine.append(C.sizeof(cls))
         for fname, _ in cls._fields_:
             lines.append(f'printf("%zu\\n", offsetof({cname}, {fname}));'); mine.append(getattr(cls, fname).offset)

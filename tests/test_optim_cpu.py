@@ -7,10 +7,8 @@ of wb_adamw_step / wb_rmsprop_step:
     and MultiStepLR under its SDFTrainer.step) reproduces the golden's parameters after every step;
   - the schedule against torch.optim.lr_scheduler.MultiStepLR (a repeated milestone and a milestone at iteration 1 included) and
     against the golden's recorded rates;
-  - the ctypes layout of wb_rmsprop_segment, the refusal without a device, optimizer="sgd"."""
-import ctypes as C
+  - the refusal without a device, optimizer="sgd"."""
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -147,17 +145,6 @@ def test_schedule_is_the_goldens():
             assert np.allclose(lrs[t - 1], [lr0 * f, lr0 * glw * f, lr0 * f], rtol=1e-15, atol=0.0), (case, t)
 
 
-def test_rmsprop_segment_layout_matches_header(tmp_path):
-    cls = W._cabi.RMSpropSegment
-    lines = ['printf("%zu\\n", sizeof(wb_rmsprop_segment));'] + [f'printf("%zu\\n", offsetof(wb_rmsprop_segment, {n}));' for n, _ in cls._fields_]
-    mine = [C.sizeof(cls)] + [getattr(cls, n).offset for n, _ in cls._fields_]
-    src = tmp_path / "lay.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "wispb200.h"\nint main(void){ ' + " ".join(lines) + ' return 0; }')
-    exe = tmp_path / "lay"
-    subprocess.run(["/usr/bin/gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
-    assert mine == [int(v) for v in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
-
-
 @pytest.mark.skipif(torch.cuda.is_available(), reason="the refusal of a machine without a device")
 def test_no_device_is_an_error():
     A = W._cabi
@@ -167,9 +154,9 @@ def test_no_device_is_an_error():
         s.param, s.grad, s.numel, s.lr, s.weight_decay = t[0].data_ptr(), t[1].data_ptr(), 8, 1e-3, 0.0
     a[0].exp_avg, a[0].exp_avg_sq, r[0].square_avg = t[2].data_ptr(), t[3].data_ptr(), t[2].data_ptr()
     with pytest.raises(A.WispB200Error):
-        A.check(A.lib().wb_adamw_step(a, C.c_int32(1), C.c_float(0.9), C.c_float(0.999), C.c_float(1e-8), C.c_int32(1), C.c_float(1.0), C.c_int32(1), None))
+        A.lib().wb_adamw_step(a, 1, 0.9, 0.999, 1e-8, 1, 1.0, 1, None)
     with pytest.raises(A.WispB200Error):
-        A.check(A.lib().wb_rmsprop_step(r, C.c_int32(1), C.c_float(0.99), C.c_float(1e-8), C.c_float(0.0), C.c_float(1.0), C.c_int32(1), None))
+        A.lib().wb_rmsprop_step(r, 1, 0.99, 1e-8, 0.0, 1.0, 1, None)
     assert torch.equal(t[0], torch.zeros(8))
     for opt in (W.NativeAdamW([(t[0], 1e-3, 0.0)]), W.NativeRMSprop([(t[0], 1e-3, 0.0)]), W.NativeRMSprop([(t[0], 1e-3, 0.0)], momentum=0.9)):
         with pytest.raises(A.WispB200Error):

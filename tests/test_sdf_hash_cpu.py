@@ -51,34 +51,38 @@ def test_hash_training_footprint_boundary():
     assert ops.sdf_train_smem_bytes(ops.sdf_field(_hash_sdf(H=128, nh=3))) < 0
 
 
-def _call_eval(d):
+def _refused_eval(d) -> str:
+    """wb_sdf_eval of the description fails with WB_ERR_INVALID: -> its message."""
     c = torch.zeros(4, 3)
     out = torch.zeros(4, 1)
-    return A.lib().wb_sdf_eval(None, C.byref(d), C.c_int32(d.num_lods - 1), A.ptr(c), C.c_int64(4), A.ptr(out), None)
+    with pytest.raises(A.WispB200Error) as e:
+        A.lib().wb_sdf_eval(None, d, d.num_lods - 1, A.ptr(c), 4, A.ptr(out), None)
+    assert e.value.status == -1
+    return str(e.value)
 
 
-def test_hash_description_is_validated():
+def test_hash_description_refusals_raise():
     d, _, keep = ops.sdf_field(_hash_sdf())
     bad = A.make_grid_desc(keep[1], [4, 8, 16, 32], [0] * 5, 1000)        # not a power of two: wb_make_grid refuses it
     d.hash = C.pointer(bad)
-    assert _call_eval(d) == -1 and b"power of two" in A.lib().wb_last_error()
+    assert "power of two" in _refused_eval(d)
     d, _, keep = ops.sdf_field(_hash_sdf())
     d.feature_dim = 4                                              # disagrees with the hash description
-    assert _call_eval(d) == -1 and b"hash field" in A.lib().wb_last_error()
+    assert "hash field" in _refused_eval(d)
     d, _, keep = ops.sdf_field(_hash_sdf())
     h2 = A.make_grid_desc(torch.zeros(64, 2), [4, 8, 16, 32], [0, 16, 32, 48, 64], 2 ** 10)
     d.hash, d.feature_dim = C.pointer(h2), 2                       # F = 2: outside the native range
-    assert _call_eval(d) == -1 and b"4 or 8" in A.lib().wb_last_error()
+    assert "4 or 8" in _refused_eval(d)
 
 
-def test_sdf_trace_refuses_hash_fields():
+def test_sdf_trace_raises_on_hash_fields():
     d, _, keep = ops.sdf_field(_hash_sdf())
     rays = A.RaysDesc()
     rays.num_rays = 1
     st = A.SdfState()
-    rc = A.lib().wb_sdf_trace(None, C.byref(d), C.c_int32(3), C.byref(rays), None, C.c_int64(1), None, C.c_int32(8), C.c_float(1.0),
-                              C.c_double(1e-4), C.c_int32(0), C.byref(st), None, None, None, None, None, None, None)
-    assert rc == -1 and b"phase by phase" in A.lib().wb_last_error()
+    with pytest.raises(A.WispB200Error, match="phase by phase") as e:
+        A.lib().wb_sdf_trace(None, d, 3, rays, None, 1, None, 8, 1.0, 1e-4, 0, st, None, None, None, None, None, None, None)
+    assert e.value.status == -1
 
 
 def test_sdf_step_hash_needs_a_device():

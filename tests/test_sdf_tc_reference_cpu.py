@@ -99,7 +99,7 @@ def test_footprint_matches_library(F, ms, L, pm, pf, H, nh):
     pos = 0 if pm == 0 else 3 if pm == 1 else 6 * pf + (3 if pm == 3 else 0)
     feat = F if ms else F * L
     want = TR.footprint(pos + feat, pos, feat, H, nh)
-    got = int(A.lib().wb_sdf_train_tc_smem_bytes(C.byref(d)))
+    got = int(A.lib().wb_sdf_train_tc_smem_bytes(d))
     assert got == want, (got, want)
     if (F, H, nh) == (16, 128, 2):
         assert 170 * 1024 < got <= 227 * 1024

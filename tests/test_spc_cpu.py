@@ -1,9 +1,7 @@
 """CPU tests of the SPC render path's host side: SPCField's colour sources against the reference class (through tests/golden/spc_trace.npz
 everywhere, and the unmodified class itself where the reference checkout is present), PackedSPCTracer's channel negotiation against
-the reference's BaseTracer, install() on the real PackedSPCTracer, and the ctypes prototype of wb_spc_trace against the header."""
-import ctypes as C
+the reference's BaseTracer and install() on the real PackedSPCTracer."""
 import os
-import re
 import subprocess
 import sys
 
@@ -41,22 +39,6 @@ def test_colour_sources_match_the_reference_golden(name, src):
     idx = torch.tensor([off, off + 3, off + exp.shape[0] - 1])
     rgb = nef(ridx_hit=idx, channels="rgb")
     assert rgb.shape == (3, 1, 3) and np.array_equal(rgb[:, 0].numpy(), exp[[0, 3, exp.shape[0] - 1], :3])
-
-
-def test_spc_trace_prototype_matches_header():
-    """_cabi's argtypes of wb_spc_trace are the parameter types the header declares, in order."""
-    src = open(os.path.join(ROOT, "include", "wispb200.h")).read()
-    m = re.search(r"\bint\s+wb_spc_trace\s*\(([^)]*)\)\s*;", src)
-    assert m, "wb_spc_trace is not declared in include/wispb200.h"
-    A = W._cabi
-    ctype = {"const wb_octree*": C.POINTER(A.OctreeDesc), "const wb_rays*": C.POINTER(A.RaysDesc), "int32_t": C.c_int32, "int64_t": C.c_int64,
-             "const float*": C.c_void_p, "float*": C.c_void_p, "uint8_t*": C.c_void_p, "wb_stream": C.c_void_p}
-    params = [re.sub(r"\s+", " ", p.strip()) for p in m.group(1).split(",")]
-    types = [re.sub(r"\s*\*\s*", "*", re.match(r"(.*?\*?)\s*\w+$", p).group(1)) for p in params]
-    assert [ctype[t] for t in types] == A.SPC_TRACE_ARGTYPES
-    L = A.lib()
-    assert L.wb_spc_trace.argtypes == A.SPC_TRACE_ARGTYPES and L.wb_spc_trace.restype is C.c_int
-    assert "wb_spc_trace" in A.EXPORTS
 
 
 def test_no_cpu_fallback():
