@@ -347,6 +347,10 @@ int64_t wb_rf_param_blob_floats(const wb_nef_desc* nef, int32_t precision);
  * activation tiles and weight-gradient accumulators fit in shared memory (decoders with up to one hidden density and two hidden
  * colour layers may split the accumulators over several passes).  Host-side query, no device work. */
 int wb_rf_precision_supported(const wb_nef_desc* nef, int32_t precision, int32_t backward);
+/* *shaped = 1 when the precision-1 forward (backward == 0), or the decoder backward with the fused hash-table scatter
+ * (backward == 1), of this decoder runs a kernel instance compiled for its layer widths (the app/nerf 64-wide decoders), 0 when it
+ * runs the instance that reads the widths at run time.  Host-side query, no device work. */
+int wb_rf_tc_shaped(const wb_nef_desc* nef, int32_t backward, int32_t* shaped);
 int wb_rf_pack_params(const wb_nef_desc* nef, int32_t precision, float* blob, wb_stream s);
 /* precision 1 scratch: workspace = per-ray view-embedding rows (+ dL/dfeat planes when backward != 0);
  * feat = the gathered grid features the forward saves for the backward (2*Kp0 bytes per sample).  Both 0 for precision 0. */

@@ -126,6 +126,7 @@ PROTOTYPES = {
     "wb_rf_march_fill": (_int, [_rays, _i32, _p, _u32, _p, _p, _p, _p, _p, _p]),
     "wb_rf_param_blob_floats": (_i64, [_nef, _i32]),
     "wb_rf_precision_supported": (_int, [_nef, _i32, _i32]),
+    "wb_rf_tc_shaped": (_int, [_nef, _i32, _p]),
     "wb_rf_pack_params": (_int, [_nef, _i32, _p, _p]),
     "wb_rf_workspace_bytes": (_i64, [_nef, _i32, _i64, _i64, _i32]),
     "wb_rf_feat_bytes": (_i64, [_nef, _i32, _i64]),

@@ -62,6 +62,13 @@ extern "C" int wb_rf_precision_supported(const wb_nef_desc* nef, int32_t precisi
     if (precision != 1 || nef == nullptr) return 0;
     return wb_tc_supported(nef, backward);
 }
+extern "C" int wb_rf_tc_shaped(const wb_nef_desc* nef, int32_t backward, int32_t* shaped)
+{
+    WB_CHECK_ARG(nef != nullptr && shaped != nullptr, "null pointer");
+    int v = 0; const int rc = wb_tc_shaped(nef, backward, &v);
+    *shaped = v;
+    return rc;
+}
 
 struct WbMlp {
     int nl_d, nl_c;                      // linear layers: density, colour

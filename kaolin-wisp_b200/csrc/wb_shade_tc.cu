@@ -35,6 +35,7 @@
 #include "wb_tc.cuh"
 #include <math.h>
 #include <type_traits>
+#include <utility>
 
 #define TC_ML 16
 constexpr int TC_ROWS = 64;                 // samples per sub-tile (wgmma M)
@@ -342,6 +343,58 @@ __device__ __forceinline__ void tile_gather(const WbGrid& g, uint8_t* tile, int 
 __device__ __forceinline__ void tile_zero(uint8_t* tile, int r, int f0, int f1) { for (int f = f0; f < f1; ++f) tile_store1(tile, r, f, 0.0f); }
 
 // ---------------------------------------------------------------------------------------------------------------
+// decoder geometry as a kernel template parameter: the layer counts and padded widths, read from WbTc at run time (TcShapeRt) or
+// fixed at compile time (TcShape).  A TcShape walks the layers unrolled, with the layer index and the widths as integral
+// constants, so every wgmma chain and backward round gets its width at compile time and the kernel holds only the code its layers
+// run: the run-time kernels switch over the widths 16 .. NMAX in every layer and inline each case's chains and epilogues, hundreds
+// of KB of SASS that a 64-sample tile walks through in every round.
+// ---------------------------------------------------------------------------------------------------------------
+template <int L> using TcInt = std::integral_constant<int, L>;
+// layer l + D: an int, or for a compile-time layer index the TcInt of its neighbour
+template <int D> __device__ __forceinline__ int tc_step(int l) { return l + D; }
+template <int D, int L> __device__ __forceinline__ TcInt<L + D> tc_step(TcInt<L>) { return {}; }
+struct TcShapeRt {
+    static constexpr bool fixed = false;
+    static __device__ __forceinline__ int nl_d(const WbTc& m) { return m.nl_d; }
+    static __device__ __forceinline__ int nl_c(const WbTc& m) { return m.nl_c; }
+    static __device__ __forceinline__ int Kp(const WbTc& m, int l) { return m.Kp[l]; }
+    static __device__ __forceinline__ int Np(const WbTc& m, int l) { return m.Np[l]; }
+};
+template <int... V> struct TcList {
+    // 0 outside the list: the neighbour of the first / last layer, named only in branches that are dead for that layer
+    static __host__ __device__ __forceinline__ constexpr int at(int i) { const int v[] = { V... }; return i >= 0 && i < (int)sizeof...(V) ? v[i] : 0; }
+};
+template <int ND, int NC, class KP, class NP>
+struct TcShape {
+    static constexpr bool fixed = true;
+    static __device__ __forceinline__ int nl_d(const WbTc&) { return ND; }
+    static __device__ __forceinline__ int nl_c(const WbTc&) { return NC; }
+    static __device__ __forceinline__ int Kp(const WbTc&, int l) { return KP::at(l); }
+    static __device__ __forceinline__ int Np(const WbTc&, int l) { return NP::at(l); }
+    template <int L> static __device__ __forceinline__ TcInt<KP::at(L)> Kp(const WbTc&, TcInt<L>) { return {}; }
+    template <int L> static __device__ __forceinline__ TcInt<NP::at(L)> Np(const WbTc&, TcInt<L>) { return {}; }
+    template <bool REV, class F, int... L> static __device__ __forceinline__ void layers_(F& f, std::integer_sequence<int, L...>)
+    {
+        (f(TcInt<REV ? ND + NC - 1 - L : L>()), ...);
+    }
+    // f(TcInt<l>()) for every layer, first to last (REV: last to first)
+    template <bool REV, class F> static __device__ __forceinline__ void layers(const WbTc&, F&& f)
+    {
+        layers_<REV>(f, std::make_integer_sequence<int, ND + NC>());
+    }
+    // the kernels of this shape run a decoder exactly when its geometry is this one (every other WbTc field stays a run-time value)
+    static bool matches(const WbTc& m)
+    {
+        if (m.nl_d != ND || m.nl_c != NC) return false;
+        for (int l = 0; l < ND + NC; ++l) if (m.Kp[l] != KP::at(l) || m.Np[l] != NP::at(l)) return false;
+        return true;
+    }
+};
+// app/nerf with 64-wide decoders and the 16-LOD F = 2 hash grid (bench.py's config 2): density 32 -> 64 -> 16, colour
+// 15 + 27 (view embedding, 4 frequencies) -> 64 -> 64 -> 3
+using TcShapeNerf64 = TcShape<2, 3, TcList<32, 64, 48, 64, 64>, TcList<64, 16, 64, 64, 16>>;
+
+// ---------------------------------------------------------------------------------------------------------------
 // wgmma chains of one group
 // ---------------------------------------------------------------------------------------------------------------
 struct TcCtx {
@@ -422,6 +475,13 @@ __device__ __forceinline__ void tc_chain_n(const TcCtx& c, int N, uint64_t da, u
         default: tc_chain<NMAX, TA, TB>(c, da, db, nk, aadv, badv, bias, epi); break;
     }
 }
+// N known at compile time (TcShape)
+template <int TA, int TB, int NMAX = 128, int N, class Epi>
+__device__ __forceinline__ void tc_chain_n(const TcCtx& c, TcInt<N>, uint64_t da, uint64_t db, int nk, uint32_t aadv, uint32_t badv,
+                                           const __half* bias, Epi&& epi)
+{
+    tc_chain<N, TA, TB>(c, da, db, nk, aadv, badv, bias, epi);
+}
 // fragments -> fp32 scratch tile, columns [0, ncols); the caller synchronises the group before reading rows
 #define TC_FRAG_TO_SCRATCH(c, d, ncols)                                                                          \
     do {                                                                                                         \
@@ -433,62 +493,32 @@ __device__ __forceinline__ void tc_chain_n(const TcCtx& c, int N, uint64_t da, u
     } while (0)
 
 // forward layer l: D = bias + X_l . W_l^T   (A: input tile K-major, B: weight pack K-major)
-template <int NMAX, class Epi>
-__device__ __forceinline__ void tc_fwd_layer(const WbTc& m, const TcCtx& c, int l, int N, Epi&& epi)
+template <int NMAX, class S, class LT, class NT, class Epi>
+__device__ __forceinline__ void tc_fwd_layer(const WbTc& m, const TcCtx& c, LT l, NT N, Epi&& epi)
 {
     const uint32_t sb = tc_smem_u32(c.sub + m.tile_off[l]), wb = tc_smem_u32(c.blob);
-    const int Np = m.Np[l];
-    tc_chain_n<0, 0, NMAX>(c, N, tc_desc(sb, TC_SLAB, 128), tc_desc(wb + m.w_off[l], Np * 16, 128), m.Kp[l] / 16, (2 * TC_SLAB) >> 4,
+    const int Np = S::Np(m, l);
+    tc_chain_n<0, 0, NMAX>(c, N, tc_desc(sb, TC_SLAB, 128), tc_desc(wb + m.w_off[l], Np * 16, 128), S::Kp(m, l) / 16, (2 * TC_SLAB) >> 4,
                      (2 * Np * 16) >> 4, m.has_bias ? reinterpret_cast<const __half*>(c.blob + m.b_off[l]) : nullptr, epi);
 }
 
 // Decoders of one 64-sample sub-tile, starting from an X0 tile that the group has already written.
 // Returns (per row, both column halves) the density-decoder output df[16] and the colour pre-activations c3[3].
-template <int NMAX>
+template <int NMAX, class S>
 __device__ __forceinline__ void tc_decoders(const WbTc& m, const TcCtx& c, const TcIn& in, int64_t ray, float df[16], float c3[3])
 {
-    const int nl = m.nl_d + m.nl_c;
-    for (int l = 0; l < nl; ++l) {
-        const bool last_d = (l == m.nl_d - 1), last_c = (l == nl - 1);
-        tc_publish(c);
-        if (!last_d && !last_c) {
-            // hidden layer: relu(acc) -> next input tile (F2FP.RELU), straight from the fragments; Np[l] == Kp[l+1], padded outputs
-            // are relu(0 + 0) = 0
-            uint8_t* tn = c.sub + m.tile_off[l + 1];
-            tc_fwd_layer<NMAX>(m, c, l, m.Np[l], [&](auto& d) {
-                constexpr int NR = sizeof(d) / sizeof(float);
-#pragma unroll
-                for (int i = 0; i < NR; i += 2) {
-                    const int row = tc_frag_row(c.wl, i), col = tc_frag_col(c.wl, i);
-                    *reinterpret_cast<uint32_t*>(tn + (col >> 3) * TC_SLAB + row * 16 + (col & 7) * 2) = tc_pack2_relu(d[i], d[i + 1]);
-                }
-            });
-            continue;
-        }
-        tc_fwd_layer<NMAX>(m, c, l, 16, [&](auto& d) { TC_FRAG_TO_SCRATCH(c, d, 16); });      // both heads are <= 16 wide
-        tc_sync(c);
-        const float* srow = c.scr + c.r * TC_SCR_LD;
-        if (last_d) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) df[j] = srow[j];
-            // colour input = [df[1:], embed(ray_d)], zero padded (nerf.py:248-259): the per-ray row already holds the
-            // embedding and the zero padding, only the first dout-1 (<= 15) features are per-sample.  16-byte chunk ch of the
-            // row is written by column half ch & 1.
-            uint8_t* tcol = c.sub + m.tile_off[l + 1];
-            const int nd = m.O[l] - 1, nch = m.Kp[l + 1] / 8;
-            const uint4* re = in.ray_embed + ray * nch;
-            uint4 q = __ldg(re + c.h);
-            __half* hq = reinterpret_cast<__half*>(&q);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                // feature 8*h + j <- df[8*h + j + 1]; select without dynamic register indexing
-                const float dv = c.h == 0 ? df[(j + 1) & 15] : df[(j + 9) & 15];
-                if (8 * c.h + j < nd) hq[j] = __float2half_rn(dv);
-            }
-            *reinterpret_cast<uint4*>(tcol + c.h * TC_SLAB + c.r * 16) = q;
-            for (int ch = 2 + c.h; ch < nch; ch += 2) *reinterpret_cast<uint4*>(tcol + ch * TC_SLAB + c.r * 16) = __ldg(re + ch);
-        } else {
-            c3[0] = srow[0]; c3[1] = srow[1]; c3[2] = srow[2];
+    const int nl = S::nl_d(m) + S::nl_c(m);
+    if constexpr (S::fixed) {
+        S::template layers<false>(m, [&](auto l) {
+#define TC_NEXT_LAYER return
+#include "wb_shade_tc_fwd_layer.cuh"
+#undef TC_NEXT_LAYER
+        });
+    } else {
+        for (int l = 0; l < nl; ++l) {
+#define TC_NEXT_LAYER continue
+#include "wb_shade_tc_fwd_layer.cuh"
+#undef TC_NEXT_LAYER
         }
     }
 }
@@ -497,8 +527,9 @@ __device__ __forceinline__ void tc_decoders(const WbTc& m, const TcCtx& c, const
 // forward kernel: CTA = TC_FWD_GROUPS groups, each walking its own 64-sample sub-tiles; several CTAs per SM overlap gather,
 // MMA chains and epilogues
 // ---------------------------------------------------------------------------------------------------------------
-template <int MINB, bool GX, int NMAX>   // MINB: resident CTAs per SM the register allocation is bounded for; GX: triplanar / octree
-                                         // feature grid (wb_featx.cuh) instead of the hash grid; NMAX: widest padded layer (64 or 128)
+template <int MINB, bool GX, int NMAX, class S = TcShapeRt>   // MINB: resident CTAs per SM the register allocation is bounded for;
+                                         // GX: triplanar / octree feature grid (wb_featx.cuh) instead of the hash grid; NMAX: widest
+                                         // padded layer (64 or 128); S: decoder geometry
 __global__ void __launch_bounds__(TC_FWD_GROUPS * TC_GROUP, MINB)
 wb_shade_fwd_tc_kernel(WbGrid g, WbGridX gx, WbTc m, const uint8_t* __restrict__ blob, TcIn in, float4* __restrict__ shaded)
 {
@@ -513,7 +544,7 @@ wb_shade_fwd_tc_kernel(WbGrid g, WbGridX gx, WbTc m, const uint8_t* __restrict__
     tc_mbar_wait(&bar, 0);
     TcCtx c; tc_ctx_init(c, m, smem);
     uint8_t* t0 = c.sub + m.tile_off[0];
-    const int nch0 = m.Kp[0] / 8;
+    const int nch0 = S::Kp(m, 0) / 8;
     const int64_t ntiles = (in.S + TC_ROWS - 1) / TC_ROWS;
     for (int64_t tile = (int64_t)blockIdx.x * TC_FWD_GROUPS + c.g; tile < ntiles; tile += (int64_t)gridDim.x * TC_FWD_GROUPS) {
         int64_t s = tile * TC_ROWS + c.r;
@@ -538,7 +569,7 @@ wb_shade_fwd_tc_kernel(WbGrid g, WbGridX gx, WbTc m, const uint8_t* __restrict__
                 for (int ch = c.h; ch < nch0; ch += 2) in.x0_save[(int64_t)ch * in.S + s] = *reinterpret_cast<const uint4*>(t0 + ch * TC_SLAB + c.r * 16);
         }
         float df[16], c3[3];
-        tc_decoders<NMAX>(m, c, in, ray, df, c3);
+        tc_decoders<NMAX, S>(m, c, in, ray, df, c3);
         if (valid && c.h == 0) {
             const float r = 1.0f / (1.0f + expf(-c3[0])), gg = 1.0f / (1.0f + expf(-c3[1])), b = 1.0f / (1.0f + expf(-c3[2]));
             shaded[s] = make_float4(r, gg, b, fmaxf(df[0], 0.0f));
@@ -555,6 +586,20 @@ static int tc_launch_ray_embed(const WbTc& m, const wb_rays* rays, void* workspa
     return WB_OK;
 }
 
+// CTAs per SM of the forward: more groups in flight hide the gather and chain latencies
+static int tc_fwd_per_sm(const WbTc& m, int grid_kind)
+{
+    const bool wide = m.maxw > 64;
+    int per_sm = max(1, min(3, TC_SMEM_MAX / (m.smem_bytes + 1024)));
+    if (grid_kind == 2) per_sm = min(per_sm, 2);        // the octree gather keeps more state per thread (up to 32 accumulators)
+    return wide ? min(per_sm, 2) : max(per_sm, 2);
+}
+// the app/nerf decoder on the hash grid: the forward instance compiled for its geometry
+static bool tc_fwd_nerf64(const WbTc& m, int grid_kind, int per_sm)
+{
+    return m.maxw <= 64 && grid_kind == 0 && per_sm == 3 && TcShapeNerf64::matches(m);
+}
+
 int wb_tc_shade_fwd(const wb_nef_desc* nef, const float* blob, const wb_rays* rays, const float* rec_t, const int32_t* rec_ray,
                     int64_t S, float* shaded, void* feat_save, void* workspace, cudaStream_t st)
 {
@@ -564,20 +609,20 @@ int wb_tc_shade_fwd(const wb_nef_desc* nef, const float* blob, const wb_rays* ra
     WB_CHECK_ARG(workspace != nullptr, "precision 1 needs the workspace (wb_rf_workspace_bytes)");
     rc = tc_launch_ray_embed(m, rays, workspace, st); if (rc) return rc;
     TcIn in = { rays->origins, rays->dirs, rec_t, rec_ray, S, reinterpret_cast<const uint4*>(workspace), reinterpret_cast<uint4*>(feat_save), nullptr };
-    // CTAs per SM: more groups in flight hide the gather and chain latencies.  The register bound of the instantiation must match,
-    // or the hardware silently runs fewer.
+    // CTAs per SM (tc_fwd_per_sm): the register bound of the instantiation must match, or the hardware silently runs fewer.
     // Decoders up to 64 wide: 2 or 3 CTAs (85 registers per thread); wider ones: 1 or 2 (a 128-wide accumulator is 64 registers).
     const bool wide = m.maxw > 64;
-    int per_sm = max(1, min(3, TC_SMEM_MAX / (m.smem_bytes + 1024)));
-    if (gx.kind == 2) per_sm = min(per_sm, 2);        // the octree gather keeps more state per thread (up to 32 accumulators)
-    per_sm = wide ? min(per_sm, 2) : max(per_sm, 2);
-    auto kern = wide ? (gx.kind != 0 ? (per_sm == 2 ? wb_shade_fwd_tc_kernel<2, true, 128> : wb_shade_fwd_tc_kernel<1, true, 128>)
+    const int per_sm = tc_fwd_per_sm(m, gx.kind);
+    const bool nerf64 = tc_fwd_nerf64(m, gx.kind, per_sm);
+    auto kern = nerf64 ? wb_shade_fwd_tc_kernel<3, false, 64, TcShapeNerf64>
+              : wide ? (gx.kind != 0 ? (per_sm == 2 ? wb_shade_fwd_tc_kernel<2, true, 128> : wb_shade_fwd_tc_kernel<1, true, 128>)
                                      : (per_sm == 2 ? wb_shade_fwd_tc_kernel<2, false, 128> : wb_shade_fwd_tc_kernel<1, false, 128>))
                      : (gx.kind != 0 ? (per_sm == 3 ? wb_shade_fwd_tc_kernel<3, true, 64> : wb_shade_fwd_tc_kernel<2, true, 64>)
                                      : (per_sm == 3 ? wb_shade_fwd_tc_kernel<3, false, 64> : wb_shade_fwd_tc_kernel<2, false, 64>));
     {   // function attributes are driver calls that can wait behind other driver work (e.g. an NVML poll): set them once, not per launch
         static int64_t done_for[2][2][4] = { { { -1, -1, -1, -1 }, { -1, -1, -1, -1 } }, { { -1, -1, -1, -1 }, { -1, -1, -1, -1 } } };
-        int64_t& done = done_for[wide ? 1 : 0][gx.kind != 0 ? 1 : 0][per_sm];
+        static int64_t done_nerf64 = -1;
+        int64_t& done = nerf64 ? done_nerf64 : done_for[wide ? 1 : 0][gx.kind != 0 ? 1 : 0][per_sm];
         if (done != WB_ATTR_KEY(m.smem_bytes)) {
             WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, m.smem_bytes));
             done = WB_ATTR_KEY(m.smem_bytes);
@@ -733,10 +778,18 @@ __device__ __forceinline__ void tc_bwd_round_n(int Kp, A&&... a)
         default: tc_bwd_rounds_seq<128, D16 ? 16 : 128>(a...); break;
     }
 }
+// Kp known at compile time (TcShape): the case of the switch above
+template <bool D16, int K, class... A>
+__device__ __forceinline__ void tc_bwd_round_n(TcInt<K>, A&&... a)
+{
+    if constexpr (K <= 64) tc_bwd_round<K, D16 ? 16 : K>(a...);
+    else tc_bwd_rounds_seq<K, D16 ? 16 : K>(a...);
+}
 
 // wmask: layers whose weight gradients this launch accumulates; emit: this launch produces dL/dfeat (planes, or FUSE: the hash-table
 // scatter of an F == 2 'cat' grid in the last epilogue).  Wide decoders whose accumulators do not all fit run several launches.
-template <int NG, bool FUSE>
+// S: decoder geometry.
+template <int NG, bool FUSE, class S = TcShapeRt>
 __global__ void __launch_bounds__(NG * TC_GROUP, 1)
 wb_mlp_bwd_tc_kernel(WbTc m, const uint8_t* __restrict__ blob, TcIn in, const float4* __restrict__ g_shaded, TcGrads G,
                      unsigned wmask, int emit, WbGrid g, float* __restrict__ gtable)
@@ -777,7 +830,7 @@ wb_mlp_bwd_tc_kernel(WbTc m, const uint8_t* __restrict__ blob, TcIn in, const fl
         for (int ch = c.h; ch < nch0; ch += 2)                     // saved density-decoder input row (coalesced 16 B per lane)
             *reinterpret_cast<uint4*>(t0 + ch * TC_SLAB + c.r * 16) = __ldg(in.x0_saved + (int64_t)ch * in.S + s);
         float df[16], c3[3];
-        tc_decoders<128>(m, c, in, ray, df, c3);
+        tc_decoders<128, S>(m, c, in, ray, df, c3);
         const float4 go = valid ? __ldg(g_shaded + s) : make_float4(0, 0, 0, 0);
         // ---- colour decoder, last layer: dY = dL/d(pre-sigmoid), zero padded ----
         if (c.h == 0) {
@@ -786,101 +839,17 @@ wb_mlp_bwd_tc_kernel(WbTc m, const uint8_t* __restrict__ blob, TcIn in, const fl
             tile_store8(dyt, c.r, 0, v);
         }
         for (int sl = 1 + c.h; sl < m.Np[nl - 1] / 8; sl += 2) tile_store8(dyt, c.r, sl, z8);
-        for (int l = nl - 1; l >= 0; --l) {
-            tc_publish(c);
-            const int I = m.I[l], O = m.O[l], Kp = m.Kp[l], Np = m.Np[l];
-            const uint32_t xb = tc_smem_u32(c.sub + m.tile_off[l]);
-            // weight grad acc_l^T[out, in] += dY_l^T . X_l and, from the constant-one slab, acc_l^T[out, I] += dY_l^T . 1, one round per
-            // block of 64 outputs; the data grad dX_l = dY_l . W_l joins the round of the last block
-            const bool wg = m.acc_l[l] >= 0, bg = m.src_b[l] >= 0, dg = l > 0 || emit;
-            float* al = acc + m.acc_l[l];
-            const uint64_t xw = tc_desc(xb, 128, TC_SLAB), xone = tc_desc(xb + (uint32_t)(Kp / 8) * TC_SLAB, 128, TC_SLAB);
-            const uint64_t dyd = tc_desc(dyb, TC_SLAB, 128), wd = tc_desc(wb + m.w_off[l], 128, Np * 16);
-            auto rounds = [&](auto d16, auto&& depi) {
-                const int nmb = wg ? (Np + 63) / 64 : 1;
-                for (int b = 0; b < nmb; ++b) {
-                    const int mb = 64 * b;
-                    tc_bwd_round_n<decltype(d16)::value>(Kp, c, wg, bg, dg && b == nmb - 1, tc_desc(dyb + (uint32_t)(mb / 8) * TC_SLAB, 128, TC_SLAB),
-                                                         xw, xone, dyd, wd, Np / 16,
-                        [&](auto& d) {
-                            constexpr int NR = sizeof(d) / sizeof(float);
-#pragma unroll
-                            for (int i = 0; i < NR; ++i) {
-                                const int o = mb + tc_frag_row(c.wl, i), k = tc_frag_col(c.wl, i);
-                                if (o < O && k < I) al[o * (I + 1) + k] += d[i];
-                            }
-                        },
-                        [&](auto& d) {
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const int o = mb + tc_frag_row(c.wl, i);
-                                if (o < O && tc_frag_col(c.wl, i) == 0) al[o * (I + 1) + I] += d[i];
-                            }
-                        },
-                        depi);
-                }
-            };
-            if (!dg) {
-                if (wg) rounds(std::false_type(), [](auto&) {});
-                break;
-            }
-            if (l == m.nl_d) {
-                // first colour layer: inputs [df[1:dout], embed(ray_d)]; only the first dout-1 <= 15 carry gradient (nerf.py:259)
-                rounds(std::true_type(), [&](auto& d) { TC_FRAG_TO_SCRATCH(c, d, 16); });
-                tc_sync(c);
-                const float* v = c.scr + c.r * TC_SCR_LD;
-                const int dout = m.O[m.nl_d - 1];
-                float gdf[16];
-                gdf[0] = (df[0] > 0.0f) ? go.w * scale : 0.0f;   // relu' of density (nerf.py:263)
-#pragma unroll
-                for (int j = 1; j < 16; ++j) gdf[j] = (j < dout) ? v[j - 1] : 0.0f;
-                if (c.h == 0) tile_store8(dyt, c.r, 0, gdf); else tile_store8(dyt, c.r, 1, gdf + 8);
-                for (int sl = 2 + c.h; sl < m.Np[l - 1] / 8; sl += 2) tile_store8(dyt, c.r, sl, z8);
-            } else if (l == 0 && FUSE) {
-                // dL/d(grid features) -> hash table: column half h holds features [16h, 16h+16) = LODs 8h .. 8h+7; a warp = 32
-                // consecutive samples of one half
-                rounds(std::false_type(), [&](auto& d) { TC_FRAG_TO_SCRATCH(c, d, 32); });
-                tc_sync(c);
-                const float* v = c.scr + c.r * TC_SCR_LD + c.h * 16;
-                const float3 p = wb_ray_point(in.origins, in.dirs, ray, __ldg(in.rec_t + s));
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                    const int lv = c.h * 8 + q;
-                    if (lv < G.planes) tc_scatter_level_f2(g, lv, p, valid, v[2 * q], v[2 * q + 1], inv_scale, lane, gtable);
-                }
-            } else if (l == 0) {
-                // dL/d(grid features) -> fp16 planes [plane][S][width] (still loss-scaled), straight from the fragments
-                const int W = G.width, nfe = G.planes * W;
-                const int64_t srow0 = tile * TC_ROWS;
-                rounds(std::false_type(), [&](auto& d) {
-                    constexpr int NR = sizeof(d) / sizeof(float);
-#pragma unroll
-                    for (int i = 0; i < NR; i += 2) {
-                        const int64_t sr = srow0 + tc_frag_row(c.wl, i);
-                        const int fe = tc_frag_col(c.wl, i);
-                        if (sr >= s_end || fe >= nfe) continue;
-                        if (W == 2) reinterpret_cast<__half2*>(G.dfeat)[(int64_t)(fe >> 1) * in.S + sr] = __floats2half2_rn(d[i], d[i + 1]);
-                        else {
-                            G.dfeat[((int64_t)(fe / W) * in.S + sr) * W + (fe % W)] = __float2half_rn(d[i]);
-                            if (fe + 1 < nfe) G.dfeat[((int64_t)((fe + 1) / W) * in.S + sr) * W + ((fe + 1) % W)] = __float2half_rn(d[i + 1]);
-                        }
-                    }
-                });
-            } else {
-                // hidden layer input: apply relu' from the retained activation tile, write the next dY (Np[l-1] == Kp[l])
-                const uint8_t* xt = c.sub + m.tile_off[l];
-                rounds(std::false_type(), [&](auto& d) {
-                    constexpr int NR = sizeof(d) / sizeof(float);
-                    const __half2 z2 = __float2half2_rn(0.0f);
-#pragma unroll
-                    for (int i = 0; i < NR; i += 2) {
-                        const int row = tc_frag_row(c.wl, i), col = tc_frag_col(c.wl, i);
-                        const int off = (col >> 3) * TC_SLAB + row * 16 + (col & 7) * 2;
-                        // relu'(x) as a 16-bit lane mask of the retained fp16 activation (>= 0 by construction)
-                        const uint32_t a = *reinterpret_cast<const uint32_t*>(xt + off);
-                        *reinterpret_cast<uint32_t*>(dyt + off) = tc_pack2(d[i], d[i + 1]) & __hgt2_mask(*reinterpret_cast<const __half2*>(&a), z2);
-                    }
-                });
+        if constexpr (S::fixed) {
+            S::template layers<true>(m, [&](auto l) {
+#define TC_END_LAYERS return
+#include "wb_shade_tc_bwd_layer.cuh"
+#undef TC_END_LAYERS
+            });
+        } else {
+            for (int l = nl - 1; l >= 0; --l) {
+#define TC_END_LAYERS break
+#include "wb_shade_tc_bwd_layer.cuh"
+#undef TC_END_LAYERS
             }
         }
     }
@@ -1041,6 +1010,13 @@ static int tc_bwd_passes(WbTc* m, unsigned masks[TC_ML])
     return n;
 }
 
+// fused table scatter: F == 2 'cat' hash grids with <= 16 live LODs (32 features: the scratch tile), when the pass planned in *m
+// runs two groups per CTA
+static bool tc_bwd_fuses(const wb_nef_desc* nef, const WbTc& m, int planes)
+{
+    return nef->grid_kind == 0 && nef->feature_dim == 2 && nef->multiscale == 0 && planes <= 16 && m.groups > 1;
+}
+
 // decoder backward: dL/d(shaded) -> weight gradients + dL/dfeat planes in the workspace (or, fused, the hash-table scatter)
 int wb_tc_decoder_bwd_ex(const wb_nef_desc* nef, const float* blob, const wb_rays* rays, const float* rec_t, const int32_t* rec_ray,
                          int64_t S, int64_t s_begin, int64_t s_end, const float* g_shaded, const float* scale, const void* feat_saved,
@@ -1068,14 +1044,17 @@ int wb_tc_decoder_bwd_ex(const wb_nef_desc* nef, const float* blob, const wb_ray
         const bool emit = p == npass - 1;
         // fused table scatter: F == 2 'cat' hash grids with <= 16 live LODs (32 features: the scratch tile), when the pass runs two
         // groups per CTA; with one group per SM the stand-alone scatter kernel runs beside the decoder CTAs instead
-        const bool fuse = emit && grad_table != nullptr && nef->grid_kind == 0 && nef->feature_dim == 2 && nef->multiscale == 0 &&
-                          planes <= 16 && m.groups > 1;
+        const bool fuse = emit && grad_table != nullptr && tc_bwd_fuses(nef, m, planes);
         WbGrid g; memset(&g, 0, sizeof(g));
         if (fuse) { rc = wb_make_grid(nef, &g); if (rc) return rc; }
-        auto kern = m.groups == 2 ? (fuse ? wb_mlp_bwd_tc_kernel<2, true> : wb_mlp_bwd_tc_kernel<2, false>) : wb_mlp_bwd_tc_kernel<1, false>;
+        // the app/nerf decoder: the instance compiled for its geometry
+        const bool nerf64 = fuse && TcShapeNerf64::matches(m);
+        auto kern = nerf64 ? wb_mlp_bwd_tc_kernel<2, true, TcShapeNerf64>
+                  : m.groups == 2 ? (fuse ? wb_mlp_bwd_tc_kernel<2, true> : wb_mlp_bwd_tc_kernel<2, false>) : wb_mlp_bwd_tc_kernel<1, false>;
         {
             static int64_t done_for[2][2] = { { -1, -1 }, { -1, -1 } };
-            int64_t& done = done_for[m.groups - 1][fuse ? 1 : 0];
+            static int64_t done_nerf64 = -1;
+            int64_t& done = nerf64 ? done_nerf64 : done_for[m.groups - 1][fuse ? 1 : 0];
             if (done != WB_ATTR_KEY(TC_SMEM_MAX)) {        // the passes of one call differ in size: allow the largest once
                 WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
                 done = WB_ATTR_KEY(TC_SMEM_MAX);
@@ -1118,6 +1097,23 @@ int wb_tc_table_scatter(const wb_nef_desc* nef, const wb_rays* rays, const float
         else wb_table_scatter_kernel<0><<<grid2, 256, 0, st>>>(g, in, dfeat, levels, scale, grad_table);
         WB_LAUNCH_CHECK();
     }
+    return WB_OK;
+}
+
+// *shaped = 1 when the forward (backward == 0) or the decoder backward with the fused table scatter (backward == 1) of this decoder
+// runs an instance compiled for its geometry, as wb_tc_shade_fwd / wb_tc_decoder_bwd_ex choose it; 0 when it runs the run-time one
+int wb_tc_shaped(const wb_nef_desc* nef, int backward, int* shaped)
+{
+    WB_CHECK_ARG(shaped != nullptr, "null pointer");
+    *shaped = 0;
+    WbTc m; int rc = wb_tc_make(nef, backward != 0, &m); if (rc) return rc;
+    if (!backward) { *shaped = tc_fwd_nerf64(m, nef->grid_kind, tc_fwd_per_sm(m, nef->grid_kind)) ? 1 : 0; return WB_OK; }
+    int planes, width; tc_dfeat_shape(nef, &planes, &width);
+    unsigned masks[TC_ML];
+    const int npass = tc_bwd_passes(&m, masks);
+    tc_bwd_layout(&m, masks[npass - 1], 1);
+    { WbTc m2 = m; if (tc_bwd_layout(&m2, masks[npass - 1], 2)) m = m2; }
+    *shaped = tc_bwd_fuses(nef, m, planes) && TcShapeNerf64::matches(m) ? 1 : 0;
     return WB_OK;
 }
 

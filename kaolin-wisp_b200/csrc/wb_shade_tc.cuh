@@ -3,6 +3,7 @@
 #include "wb_common.cuh"
 
 int wb_tc_supported(const wb_nef_desc* nef, int backward);
+int wb_tc_shaped(const wb_nef_desc* nef, int backward, int* shaped);
 int wb_tc_blob_floats(const wb_nef_desc* nef);
 int wb_tc_pack(const wb_nef_desc* nef, float* blob, cudaStream_t st);
 int64_t wb_tc_workspace_bytes(const wb_nef_desc* nef, int64_t R, int64_t S, int backward);

@@ -1,12 +1,14 @@
 #!/usr/bin/env python
 """Compare the SASS of the kernels in two object files / shared libraries instruction by instruction.
 
-    python tools/sass_equal.py OLD.o NEW.o [--appended TYPE ...] [substring ...]
+    python tools/sass_equal.py OLD.o NEW.o [--appended TYPE ...] [--tparam TYPE ...] [substring ...]
 
 Used when a change must leave GPU-validated kernels untouched (no GPU at hand): template parameters with a `false` default are
 folded away, so `kernel<3>` in OLD is matched with `kernel<3, false>` in NEW, and a kernel that only gained that parameter
 (`kernel` -> `kernel<false>`) with its old self.  --appended TYPE folds away a trailing parameter of struct type TYPE that NEW's
 kernels gained (`kernel(a, b)` -> `kernel(a, b, TYPE)`); such a kernel's SASS can only be identical when the instance ignores it.
+--tparam TYPE folds away a trailing template argument TYPE that NEW's kernels gained as a defaulted class parameter
+(`kernel<3>` -> `kernel<3, TYPE>`).
 Exit code 1 if any matched kernel differs or is missing."""
 import re
 import subprocess
@@ -27,12 +29,18 @@ def functions(path):
 
 def main():
     old, new = functions(sys.argv[1]), functions(sys.argv[2])
-    rest, appended = sys.argv[3:], []
-    while "--appended" in rest:
-        i = rest.index("--appended")
-        appended.append(rest[i + 1]); del rest[i:i + 2]
+    rest, appended, tparams = sys.argv[3:], [], []
+    for opt, into in (("--appended", appended), ("--tparam", tparams)):
+        while opt in rest:
+            i = rest.index(opt)
+            into.append(rest[i + 1]); del rest[i:i + 2]
     want = rest
     tails = [f"{len(t)}{t}" for t in appended]
+
+    def strip(kk):
+        for t in tparams:
+            kk = kk.replace(f"{len(t)}{t}E", "E")
+        return kk
 
     def fold(kk):
         kk = re.sub(r"I(Lb0E)+Ev", "", re.sub(r"(ELb0)+EE", "EE", kk))
@@ -44,7 +52,7 @@ def main():
     for k, v in sorted(old.items()):
         if want and not any(w in k for w in want):
             continue
-        match = [kk for kk in new if kk == k or fold(kk) == k]
+        match = [kk for kk in new if k in (kk, fold(kk), strip(kk), fold(strip(kk)))]
         if not match:
             print(f"{k[:70]:70s} MISSING in {sys.argv[2]}"); bad += 1; continue
         same = v == new[match[0]]
