@@ -536,7 +536,7 @@ int wb_spc_trace(const wb_octree* oct, int32_t level, const wb_rays* rays, const
  * +inf when no triangle has a nonzero normal, and for a point with a NaN coordinate.
  * A bounding-volume hierarchy (LBVH over centroid Morton codes) is built per call in `workspace` and culls, conservatively,
  * the pairs that cannot set the fp32 minimum or a stab flag; the result is the reference's, not an approximation of it.
- * tris: f64 [T, 9] (V[F] row-major), points: f64 [N, 3], out: f64 [N].  T < 2^31; T = 0 gives +inf.  N = 0 launches nothing.
+ * tris: f64 [T, 9] (V[F] row-major), points: f64 [N, 3], out: f64 [N].  T <= 2^29; T = 0 gives +inf.  N = 0 launches nothing.
  * Launches (wb_launch_count): 6 for T >= 2 (the CUB radix sort counted as one), 5 for T = 1, 1 for T = 0. */
 /* Workspace bytes of a wb_mesh_sdf call over num_triangles triangles (any number of points); < 0 on a bad count or, for T >= 1, when
  * the radix sort's size query of the current device fails (reason in wb_last_error()).  Launches nothing. */

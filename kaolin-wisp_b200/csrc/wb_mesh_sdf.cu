@@ -163,8 +163,26 @@ __global__ void wb_msdf_karras_kernel(const uint64_t* __restrict__ k, int64_t n,
     if (i == 0) parent[0] = -1;
 }
 
-// Box of one triangle, rounded outward to fp32; a triangle with a NaN coordinate gets the whole space, since the reference's stab
-// gives it a negative hit in every direction (its NaN t fails `t >= 0`).
+__device__ __forceinline__ double fdot(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+__device__ __forceinline__ void fcross(const double* a, const double* b, double* r)
+{
+    r[0] = a[1] * b[2] - a[2] * b[1];
+    r[1] = a[2] * b[0] - a[0] * b[2];
+    r[2] = a[0] * b[1] - a[1] * b[0];
+}
+// fp32 reciprocal of the fp32-rounded squared length, widened (the reference's idot2: __frcp_rn)
+__device__ __forceinline__ double finv2(const double* a) { return (double)__frcp_rn((float)(a[0] * a[0] + a[1] * a[1] + a[2] * a[2])); }
+// (float)x is inf from FLT_MAX + half an ulp = 0x1.ffffffp127 on; tri_box's overflow exemption starts 2^-40 below that
+constexpr double kMsdfN2Exempt = 0x1.ffffffp127 * (1.0 - 0x1p-40);
+
+// Box of one triangle, rounded outward to fp32.  Two kinds of triangle get the whole space instead:
+//  - one with a NaN coordinate, since the reference's stab gives it a negative hit in every direction (its NaN t fails `t >= 0`);
+//  - one whose fp32 |n|^2 overflows (|n|^2 >= ~3.4e38, edges of ~4.3e9 and longer): its idot2(n) is 0, so the face distance is 0
+//    for every point whose projection falls inside the triangle, however far the point is.  nvcc may contract n's products into
+//    FMAs differently here and in wb_msdf_pair: each component can then differ by ~2^-52 |e10| |e02|, so |n|^2 by less than
+//    2^-48 |e10|^2 |e02|^2.  The test below exempts with a margin of 2^-40 |e10|^2 |e02|^2 and a relative 2^-40, so no triangle
+//    whose idot2(n) the pair test takes as 0 can keep its box.  The others it exempts (|n|^2 within ~2^-40 of the threshold, or
+//    |e10| |e02| >= ~2^84) only lose culling.
 __device__ __forceinline__ void tri_box(const double* v, float4& lo, float4& hi)
 {
     double l[3], h[3];
@@ -174,7 +192,11 @@ __device__ __forceinline__ void tri_box(const double* v, float4& lo, float4& hi)
         h[a] = fmax(v[a], fmax(v[3 + a], v[6 + a]));
         nan |= isnan(v[a]) || isnan(v[3 + a]) || isnan(v[6 + a]);
     }
-    if (nan) {
+    const double e10[3] = {v[3] - v[0], v[4] - v[1], v[5] - v[2]};
+    const double e02[3] = {v[0] - v[6], v[1] - v[7], v[2] - v[8]};
+    double nor[3];
+    fcross(e10, e02, nor);
+    if (nan || !(fdot(nor, nor) + 0x1p-40 * fdot(e10, e10) * fdot(e02, e02) < kMsdfN2Exempt)) {
         lo = make_float4(-INFINITY, -INFINITY, -INFINITY, 0.0f);
         hi = make_float4(INFINITY, INFINITY, INFINITY, 0.0f);
         return;
@@ -210,21 +232,12 @@ __global__ void wb_msdf_refit_kernel(const double* __restrict__ tris_in, const u
     }
 }
 
-__device__ __forceinline__ double fdot(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
-__device__ __forceinline__ void fcross(const double* a, const double* b, double* r)
-{
-    r[0] = a[1] * b[2] - a[2] * b[1];
-    r[1] = a[2] * b[0] - a[0] * b[2];
-    r[2] = a[0] * b[1] - a[1] * b[0];
-}
 // |a x - b|^2 for the edge parameter x
 __device__ __forceinline__ double fdist2(const double* a, double x, const double* b)
 {
     const double t0 = a[0] * x - b[0], t1 = a[1] * x - b[1], t2 = a[2] * x - b[2];
     return t0 * t0 + t1 * t1 + t2 * t2;
 }
-// fp32 reciprocal of the fp32-rounded squared length, widened (the reference's idot2: __frcp_rn)
-__device__ __forceinline__ double finv2(const double* a) { return (double)__frcp_rn((float)(a[0] * a[0] + a[1] * a[1] + a[2] * a[2])); }
 // the edge parameter clamped in fp32 (fmaxf(0, fminf(t, 1)))
 __device__ __forceinline__ double fclamp01(double t) { return (double)fmaxf(0.0f, fminf((float)t, 1.0f)); }
 __device__ __forceinline__ double fsign(double x) { return (double)copysignf(1.0f, (float)x); }
@@ -310,10 +323,13 @@ __device__ __forceinline__ bool box_line(const float4* __restrict__ box, int nod
 
 // One thread per point.  Culling bounds, with S = max|p_i| + max|vertex coordinate| and E the longest edge:
 //  - distance: a subtree is skipped when its box's squared distance d2 satisfies d2 (1 - 2^-20) - 2^-40 S^2 > best.  Every distance
-//    the pair test can return for a triangle in the box is at least d2 (1 - 2^-22) - (double rounding, < 2^-45 S^2): the fp32
-//    reciprocal idot2 and the fp32 rounding of the result each lose at most 2^-24 relative, and a face distance taken when the
-//    projection lies just outside the triangle (a sign flipped by rounding) is short by at most the rounding of that sign's dot
-//    product.  So a skipped triangle can never lower the fp32 minimum.
+//    the pair test can return for a triangle in the box is at least d2 (1 - 2^-21) - (double rounding, < 2^-45 S^2): the fp32
+//    rounding of the result loses at most 2^-24 relative; the fp32 reciprocal idot2 loses at most 2^-24 for a normal |n|^2 and
+//    at most about 2^-22 when fp32 |n|^2 (down to ~2.9e-39) or its reciprocal (|n|^2 in [2^126, FLT_MAX]) is subnormal; below
+//    that the reciprocal is inf and the face distance inf or NaN, never short; and a face distance taken when the projection lies
+//    just outside the triangle (a sign flipped by rounding) is short by at most the rounding of that sign's dot product.  So a
+//    skipped triangle can never lower the fp32 minimum.  The one exception is a triangle whose fp32 |n|^2 overflows: its idot2 is
+//    0 and its face distance 0 at any distance, so tri_box gives it the whole space, which only its ancestors' boxes inherit.
 //  - stab: a box is searched only when the line meets it grown by m = 2^-30 S + 2^-40 E^2 (S + E) / 1e-8.  The test rejects
 //    |det| < 1e-8, and for |det| >= 1e-8 the barycentric u, v it accepts are off the exact ones by less than
 //    10 2^-53 E (S + E) / |det|: the line then passes within 2^-40 E^2 (S + E) / 1e-8 of the triangle, inside the grown box.
@@ -399,9 +415,12 @@ __global__ void __launch_bounds__(kMsdfThreads) wb_msdf_query_kernel(const doubl
 
 }  // namespace
 
+// Node ids and the box offsets 2 node are int: the last leaf's, 2 (2T - 2), fits for T <= 2^29 (a workspace of ~90 GB).
+constexpr int64_t kMsdfMaxTriangles = (int64_t)1 << 29;
+
 extern "C" int64_t wb_mesh_sdf_workspace_bytes(int64_t num_triangles)
 {
-    if (num_triangles < 0 || num_triangles >= ((int64_t)1 << 31)) {
+    if (num_triangles < 0 || num_triangles > kMsdfMaxTriangles) {
         wb_set_error("%s: num_triangles out of range", __func__);
         return -1;
     }
@@ -417,7 +436,7 @@ extern "C" int wb_mesh_sdf(const double* tris, int64_t num_triangles, const doub
                            int64_t workspace_bytes, double* out, wb_stream s)
 {
     const int64_t T = num_triangles, N = num_points;
-    WB_CHECK_ARG(T >= 0 && T < ((int64_t)1 << 31), "num_triangles out of range");
+    WB_CHECK_ARG(T >= 0 && T <= kMsdfMaxTriangles, "num_triangles out of range");
     WB_CHECK_ARG(N >= 0 && N < ((int64_t)1 << 31) * kMsdfThreads, "num_points out of range");
     if (N == 0) return WB_OK;
     WB_CHECK_ARG(points && out && (tris || T == 0), "null pointer");

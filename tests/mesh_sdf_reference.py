@@ -12,7 +12,11 @@ against 0) lies farther from its threshold than a float64 error bound on that va
 so FMA contraction or another summation order cannot cross it).  `tol` is the distance bound that follows: 1 fp32 ulp, plus, when
 the minimum comes from an edge branch or an ambiguous one, the displacement of one fp32 ulp of the edge parameter (2^-24 |edge|), plus
 the absolute float64 rounding of the pair arithmetic (256 ulps of the coordinates' magnitude, which only matters for points on the
-surface); it is inf when a triangle whose normal is zero up to rounding would set the minimum if it took part.
+surface), plus, when a pair with a nonzero normal can take its other face/edge branch under another rounding (some c_k . p_k
+within its bound of 0 and none surely negative) and that branch would give less than the minimum, the difference; it is
+inf when a triangle whose normal is zero up to rounding would set the minimum if it took part.
+pair_d2, stab_hits and tri_box expose the per-pair distance, the per-pair stab test and wb_mesh_sdf's leaf box, for checks of the
+kernel's culling bounds.
 """
 from __future__ import annotations
 
@@ -27,6 +31,7 @@ STAB_DIRS = np.array([[1.0, 0.0, 0.0], [0.0, 1.0, 0.0], [0.0, 0.0, 1.0],
 EPS = 2.0 ** -53
 K = 64 * EPS            # error bound factor on |products|
 F32 = np.float32
+N2_EXEMPT = float.fromhex("0x1.ffffffp127") * (1.0 - 2.0 ** -40)     # wb_mesh_sdf.cu's kMsdfN2Exempt
 
 
 def _dot(a, b):
@@ -62,12 +67,11 @@ def _dist2(a, x, b):
     return _dot(t, t)
 
 
-def _chunk(P, tris):
-    """All pairs of the points P [n, 3] with the triangles [T, 9]."""
-    n, T = P.shape[0], tris.shape[0]
+def _pairs(P, tris):
+    """The distance half of the rule for all pairs of the points P [n, 3] with the triangles [T, 9]: the edges, the normal, the
+    p_k, the three c_k . p_k, the branch sum s, the edge and face distances and the fp32 d2 [n, T] (NaN for a zero normal)."""
     v0, v1, v2 = tris[:, 0:3], tris[:, 3:6], tris[:, 6:9]
     e10, e21, e02 = v1 - v0, v2 - v1, v0 - v2
-    e20 = -e02
     nor = _cross(e10, e02)
     c = [_cross(e10, nor), _cross(e21, nor), _cross(e02, nor)]
     es = [e10, e21, e02]
@@ -83,6 +87,77 @@ def _chunk(P, tris):
         d2 = np.where(d2 < 0.0, 0.0, d2)
         valid = np.any(nor != 0.0, axis=1)
         d2 = np.where(valid[None], d2, np.nan).astype(F32)           # a zero normal: ignored by fminf
+    return es, nor, p, dots, s, edge, face, d2
+
+
+def _stab(p0, e10, e20, qv, d):
+    """Moller-Trumbore along direction d for the pairs p0 [n, T, 3] x (e10, e20) [T, 3]: det [T], whether it is tested, and u, w, t
+    [n, T]."""
+    pv = _cross(np.broadcast_to(d, e20.shape), e20)
+    det = _dot(e10, pv)
+    tested = ~((det > -1e-8) & (det < 1e-8))
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+        inv_det = 1.0 / det
+        u = _dot(p0, pv[None]) * inv_det[None]
+        w = _dot(np.broadcast_to(d, qv.shape), qv) * inv_det[None]
+        t = _dot(e20[None], qv) * inv_det[None]
+    return det, tested, u, w, t
+
+
+def pair_d2(P, tris):
+    """The rule's fp32 squared distance of every pair of the points P [n, 3] with the triangles [T, 9] -> [n, T]; NaN where the
+    triangle's normal is exactly zero (the pair adds nothing to the fminf)."""
+    return _pairs(np.asarray(P, np.float64).reshape(-1, 3), np.asarray(tris, np.float64).reshape(-1, 9))[-1]
+
+
+def stab_hits(P, tris, i):
+    """The rule's Moller-Trumbore test along stab direction i for every pair -> (hit [n, T]: tested and inside the triangle, t)."""
+    P, tris = np.asarray(P, np.float64).reshape(-1, 3), np.asarray(tris, np.float64).reshape(-1, 9)
+    e10, e20 = tris[:, 3:6] - tris[:, 0:3], tris[:, 6:9] - tris[:, 0:3]
+    p0 = P[:, None, :] - tris[None, :, 0:3]
+    _, tested, u, w, t = _stab(p0, e10, e20, _cross(p0, e10[None]), STAB_DIRS[i])
+    with np.errstate(invalid="ignore"):
+        return tested[None] & ~((u < 0.0) | (u > 1.0)) & ~((w < 0.0) | (u + w > 1.0)), t
+
+
+def _f32_down(x):
+    with np.errstate(over="ignore"):
+        f = x.astype(F32)
+    return np.where(f.astype(np.float64) > x, np.nextafter(f, F32(-np.inf)), f)
+
+
+def _f32_up(x):
+    with np.errstate(over="ignore"):
+        f = x.astype(F32)
+    return np.where(f.astype(np.float64) < x, np.nextafter(f, F32(np.inf)), f)
+
+
+def outward_box(tris):
+    """Each triangle's [T, 9] bounding box rounded outward to fp32 -> (lo, hi) fp32 [T, 3]."""
+    tris = np.asarray(tris, np.float64).reshape(-1, 3, 3)
+    return _f32_down(tris.min(1)), _f32_up(tris.max(1))
+
+
+def tri_box(tris):
+    """wb_mesh_sdf's leaf box: the outward-rounded box, or the whole space for a triangle with a NaN coordinate (its stab hits are
+    all negative) or one whose fp32 |n|^2 overflows (idot2(n) = 0: the face distance is 0 wherever the projection falls inside),
+    with the kernel's margin for another FMA contraction of n."""
+    tris = np.asarray(tris, np.float64).reshape(-1, 9)
+    lo, hi = outward_box(tris)
+    e10, e02 = tris[:, 3:6] - tris[:, 0:3], tris[:, 0:3] - tris[:, 6:9]
+    nor = _cross(e10, e02)
+    with np.errstate(over="ignore", invalid="ignore"):          # the overflow test with its FMA margin, as the kernel writes it
+        whole = np.isnan(tris).any(1) | ~(_dot(nor, nor) + 2.0 ** -40 * _dot(e10, e10) * _dot(e02, e02) < N2_EXEMPT)
+    lo[whole], hi[whole] = -np.inf, np.inf
+    return lo, hi
+
+
+def _chunk(P, tris):
+    """All pairs of the points P [n, 3] with the triangles [T, 9]."""
+    n = P.shape[0]
+    es, nor, p, dots, s, edge, face, d2 = _pairs(P, tris)
+    e10, e21, e02 = es
+    e20 = -e02
     d2_for_min = np.where(np.isnan(d2), np.inf, d2)
     best = d2_for_min.min(axis=1)
     # a nearly zero normal may be exactly zero under another rounding (FMA): such a pair may or may not take part
@@ -106,6 +181,23 @@ def _chunk(P, tris):
     # the float64 rounding of the pair's own arithmetic, absolute: it dominates for points on the surface (distances ~1e-17)
     scale = np.abs(P).max(1) + np.abs(tris).max()
     edge_term = edge_term + K * scale * 4
+    # a pair with a nonzero normal whose branch can flip under another rounding may take its other branch; that only matters where
+    # the other value undercuts the minimum by more than the terms above, e.g. a triangle whose fp32 |n|^2 underflows (face
+    # distance inf or NaN) at a point on one of its edge lines (c_k . p_k = 0 here, tiny and negative under FMA: an edge distance
+    # instead).  The face branch needs all three signs +1, so the branch can flip when some sign is ambiguous and none is surely
+    # -1.  A zero normal is left out: the kernel drops that pair before either branch.
+    amb_any, neg_sure = np.zeros(d2.shape, bool), np.zeros(d2.shape, bool)
+    for k in range(3):
+        amb_k = np.abs(dots[k]) <= 2 * K * (_norm(es[k]) * _norm(e10) * _norm(e02))[None] * _norm(p[k])
+        amb_any |= amb_k
+        neg_sure |= ~amb_k & (_sign32(dots[k]) < 0.0)
+    amb = amb_any & ~neg_sure & np.any(nor != 0.0, axis=1)[None]
+    with np.errstate(invalid="ignore", over="ignore"):
+        other = np.where(amb, np.where(s < 2.0, face, edge), np.inf).astype(F32)
+    other = np.where(np.isnan(other), np.inf, other).min(axis=1)
+    with np.errstate(invalid="ignore"):
+        undercut = np.sqrt(best.astype(np.float64)) - np.sqrt(np.maximum(other, F32(0.0)).astype(np.float64))
+    edge_term = edge_term + np.where(other < best, undercut, 0.0)
     edge_term = np.where(dist_ok, edge_term, np.inf)
 
     # the stab: per direction, whether a positive / negative hit is certain or possible under the error bounds
@@ -113,17 +205,11 @@ def _chunk(P, tris):
     n10, n20, np0 = _norm(e10), _norm(e20), _norm(p[0])
     qv = _cross(p[0], e10[None])
     for i, d in enumerate(STAB_DIRS):
-        pv = _cross(np.broadcast_to(d, e20.shape), e20)
-        det = _dot(e10, pv)
+        det, tested, u, w, t = _stab(p[0], e10, e20, qv, d)
         derr = K * n10 * n20
-        tested = ~((det > -1e-8) & (det < 1e-8))
         sure_test = np.abs(det) >= 1e-8 + derr
         sure_skip = np.abs(det) < 1e-8 - derr
         with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
-            inv_det = 1.0 / det
-            u = _dot(p[0], pv[None]) * inv_det[None]
-            w = _dot(np.broadcast_to(d, qv.shape), qv) * inv_det[None]
-            t = _dot(e20[None], qv) * inv_det[None]
             ad = np.abs(det)[None]
             su = K * (np0 * n20[None] + np.abs(u) * (n10 * n20)[None]) / ad
             sw = K * (np0 * n10[None] + np.abs(w) * (n10 * n20)[None]) / ad

@@ -41,7 +41,8 @@ def against_restatement(got, V, F, P):
     bad = ~(err <= ref["tol"])
     assert not bad.any(), (int(bad.sum()), got[bad][:5], ref["sdf"][bad][:5], ref["tol"][bad][:5])
     ok = ref["sign_ok"]
-    assert np.array_equal(got[ok] < 0, ref["inside"][ok]), int(((got < 0) != ref["inside"])[ok].sum())
+    neg = np.signbit(got)          # an inside point at distance 0 is -0.0
+    assert np.array_equal(neg[ok], ref["inside"][ok]), int((neg != ref["inside"])[ok].sum())
     return ref
 
 

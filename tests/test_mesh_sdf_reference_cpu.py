@@ -61,6 +61,17 @@ def test_restatement_empty_mesh_and_nan():
     assert r["sdf"][0] == -0.5 and r["sdf"][1] == np.inf
 
 
+def test_restatement_tol_ignores_zero_normal_triangles():
+    """A triangle with an exactly zero normal adds nothing to the rule, so its edge distance must not widen tol: at (0.5, 0.5, 0.5),
+    on a collinear triangle inside an icosphere of radius 0.7, the value is the sphere's distance to fp32 precision."""
+    V, F = MS.icosphere(2, 0.7)
+    n = V.shape[0]
+    V = np.concatenate([V, [[0.125, 0.125, 0.125], [0.25, 0.25, 0.25], [0.5, 0.5, 0.5]]])
+    F = np.concatenate([F, [[n, n + 1, n + 2]]])
+    r = R.mesh_sdf(V[F].reshape(-1, 9), np.array([[0.5, 0.5, 0.5]]))
+    assert 0.05 < abs(r["sdf"][0]) < 0.2 and r["tol"][0] < 1e-6, (r["sdf"], r["tol"])
+
+
 @pytest.mark.parametrize("case", ["icosphere", "torus", "cube", "open", "noisy_sphere"])
 def test_restatement_against_reference_kernel_golden(case):
     """On a seeded subsample: the reference kernel's distance inside the restatement's bound of its own value, and its sign on every
