@@ -544,6 +544,19 @@ int64_t wb_mesh_sdf_workspace_bytes(int64_t num_triangles);
 int wb_mesh_sdf(const double* tris, int64_t num_triangles, const double* points, int64_t num_points, void* workspace,
                 int64_t workspace_bytes, double* out, wb_stream s);
 
+/* ------------------------------------------------------------------------------------------------
+ * wisp.ops.spc.mesh_to_octree (wisp/ops/spc/conversions.py:91-109; sampler wisp/ops/mesh/sample_surface.py): the occupancy of
+ * num_samples area-weighted surface samples and their jittered copies at `level`, in ONE launch, no sample materialised.
+ * Sample i (a 64-bit counter) draws a face by inverse CDF (the f with cdf[f] <= U * cdf[T] < cdf[f + 1], U a 53-bit uniform),
+ * u = sqrtf(r1), v = r2, x = ((1-u) a + (u (1-v)) b) + (u v) c and xj = x + (r * 2 - 1) / 2^(level+1) per axis, all fp32 op by op;
+ * x and xj are quantized as spc.quantize_points does (floor(clamp(2^level (p + 1) / 2, 0, 2^level - 1))) and their bits set.
+ * Draws come from the counter-based stream keyed by (seed, sample, draw) (DESIGN.md "Sampling contract").
+ * tris: f32 [T, 9] (V[F] row-major); cdf: f64 [T + 1], the exclusive prefix sum of the face areas with cdf[T] > 0 their total;
+ * bits: uint32 [(8^level + 31)/32], ORed into (zero it first), the layout of wb_octree_build_bits (bit x<<2L | y<<L | z).
+ * 1 <= level <= 10, T >= 1.  num_samples = 0 launches nothing. */
+int wb_mesh_octree_bits(const float* tris, const double* cdf, int64_t num_triangles, int64_t num_samples, int32_t level,
+                        uint32_t seed, uint32_t* bits, wb_stream s);
+
 #ifdef __cplusplus
 }
 #endif

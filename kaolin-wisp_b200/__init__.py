@@ -6,7 +6,7 @@ libwispb200.so (hand-written CUDA behind a C ABI, include/wispb200.h).  There is
 """
 from . import _cabi, ops, spc, parallel, raygen                                                   # noqa: F401
 from ._cabi import WispB200Error                                                # noqa: F401
-from .ops import compute_sdf                                                    # noqa: F401
+from .ops import compute_sdf, mesh_to_octree                                    # noqa: F401
 from .core import Rays, RenderBuffer                                            # noqa: F401
 from .accelstructs import OctreeAS, AxisAlignedBBoxAS, ASQueryResults, ASRaymarchResults, ASRaytraceResults   # noqa: F401
 from .grids import HashGrid, MultiTable, TriplanarGrid, TriplanarFeatureVolume, OctreeGrid, CodebookOctreeGrid                                         # noqa: F401

@@ -155,6 +155,7 @@ PROTOTYPES = {
     "wb_spc_trace": (_int, [_oct, _i32, _rays, _p, _i64, _i64, _p, _p, _p, _p, _p]),
     "wb_mesh_sdf_workspace_bytes": (_i64, [_i64]),
     "wb_mesh_sdf": (_int, [_p, _i64, _p, _i64, _p, _i64, _p, _p]),
+    "wb_mesh_octree_bits": (_int, [_p, _p, _i64, _i64, _i32, _u32, _p, _p]),
 }
 EXPORTS = list(PROTOTYPES)
 # int results that are answers, not a wb_status; every other int result raises WispB200Error when nonzero

@@ -14,6 +14,7 @@ What is patched (reference file:line -> native replacement):
   ImageNeuralField.rgb (no-grad)                (image_nef.py:77-97)               wb_image_eval
   NeuralRadianceField.prune                     (nerf.py:175-212)                  ops.prune_field
   wisp.ops.mesh.compute_sdf                     (ops/mesh/compute_sdf.py:18-45)    wb_mesh_sdf (ops.compute_sdf)
+  wisp.ops.spc(.conversions).mesh_to_octree     (ops/spc/conversions.py:91-109)    wb_mesh_octree_bits (ops.mesh_to_octree)
 Every replacement keeps the reference signature, falls back to the original method for configurations outside the native
 path (unknown embedders, activations, grids), and keeps the attributes other wisp code reads (`prev_num_samples`, `bg_color`).
 SPCField itself is not patched: its Kaolin calls build the octree (like OctreeAS's constructor) and its rgba() is plain torch.
@@ -44,6 +45,17 @@ def _patch(cls, name, fn):
     fn.__name__ = name
     fn.__wrapped__ = _ORIG[key][1]
     setattr(cls, name, fn)
+
+
+def _mesh_to_octree(mod):
+    """The replacement of `mod`.mesh_to_octree: levels 1..10 of float32 vertices go to ops.mesh_to_octree, the rest to the original."""
+    key = (mod.__name__, "mesh_to_octree")
+
+    def mesh_to_octree(vertices, faces, level, num_samples=100000000):
+        if not (isinstance(level, int) and 1 <= level <= 10) or vertices.dtype != torch.float32:
+            return _ORIG[key][1](vertices, faces, level, num_samples)
+        return ops.mesh_to_octree(vertices, faces, level, num_samples)
+    return mesh_to_octree
 
 
 def uninstall() -> None:
@@ -175,6 +187,16 @@ def install() -> bool:
         mesh_ops = None
     if mesh_ops is not None:
         _patch(mesh_ops, "compute_sdf", lambda V, F, points, split_size=10 ** 6: ops.compute_sdf(V, F, points, split_size))
+
+    # ---- mesh octree of OctreeAS.from_mesh (wisp.ops.spc) and of mesh_to_spc (its own module's global) --------------------
+    try:
+        import wisp.ops.spc as spc_ops
+        import wisp.ops.spc.conversions as spc_conversions
+    except Exception:
+        spc_ops = None
+    if spc_ops is not None:
+        for mod in (spc_ops, spc_conversions):
+            _patch(mod, "mesh_to_octree", _mesh_to_octree(mod))
 
     # ---- pruning -------------------------------------------------------------------------------------------------
     orig_prune = NeuralRadianceField.prune

@@ -11,6 +11,7 @@ from typing import List, Optional, Sequence
 import torch
 
 from . import _cabi as A
+from . import spc
 from .core import RenderBuffer
 
 # Optional per-stage device timing (bench.py): when PROFILE is a list, every native stage appends
@@ -1471,3 +1472,52 @@ def compute_sdf(V: torch.Tensor, F: torch.Tensor, points: torch.Tensor, split_si
     with _stage("mesh_sdf"):
         L.wb_mesh_sdf(A.ptr(tris), tris.shape[0], A.ptr(pts), pts.shape[0], A.ptr(ws), nbytes, A.ptr(out), A.stream())
     return out
+
+
+# --------------------------------------------------------------------------------------------------------------
+# mesh octree (wisp/ops/spc/conversions.py:91-109): the octree OctreeAS.from_mesh builds, app/nglod's first step
+# --------------------------------------------------------------------------------------------------------------
+def mesh_to_octree(vertices: torch.Tensor, faces: torch.Tensor, level: int, num_samples: int = 10 ** 8,
+                   seed: Optional[int] = None) -> torch.Tensor:
+    """wisp.ops.spc.mesh_to_octree (conversions.py:91-109) -> the uint8 octree of `level` on the current CUDA device: the cells of
+    num_samples area-weighted surface samples and of their jittered copies, drawn from the reference's distribution in one
+    wb_mesh_octree_bits launch over a dense bitmask (no sample is materialised), then spc.points_to_octree of the set cells.
+    vertices: float32 [#V, 3] (what OctreeAS.from_mesh passes), faces: integer [#F, 3], on any device.  The face areas are the
+    reference's fp32 ones (0.5 |cross(v0 - v1, v1 - v2)|); their float64 prefix sum is the CDF the kernel inverts.
+    seed: of the counter-based stream (DESIGN.md "Sampling contract"); None takes one from torch's default generator, so
+    torch.manual_seed reproduces the octree.  Raises WispB200Error without a CUDA device, for a level outside 1..10, non-float32
+    vertices, no faces, num_samples < 1, or a total area that is zero or not finite (the reference's Categorical refuses it)."""
+    if not torch.cuda.is_available():
+        raise A.WispB200Error("mesh_to_octree needs a CUDA device (H100, sm_90a); there is no CPU fallback")
+    if isinstance(level, bool) or int(level) != level or not 1 <= int(level) <= 10:
+        raise A.WispB200Error(f"mesh_to_octree: level must be 1..10 (the dense bitmask's limit), got {level!r}")
+    level = int(level)
+    if vertices.dtype != torch.float32 or vertices.dim() != 2 or vertices.shape[1] != 3:
+        raise A.WispB200Error(f"mesh_to_octree: vertices must be float32 [#V, 3], got {vertices.dtype} {tuple(vertices.shape)}")
+    if faces.dtype.is_floating_point or faces.dtype == torch.bool or faces.dim() != 2 or faces.shape[1] != 3 or faces.shape[0] == 0:
+        raise A.WispB200Error(f"mesh_to_octree: faces must be integer [#F >= 1, 3], got {faces.dtype} {tuple(faces.shape)}")
+    if int(num_samples) < 1:
+        raise A.WispB200Error(f"mesh_to_octree: num_samples must be >= 1, got {num_samples}")
+    if seed is None:
+        seed = int(torch.randint(0, 2 ** 31 - 1, (1,)))
+    dev = torch.device("cuda", torch.cuda.current_device())
+    tris = vertices.to(dev)[faces.to(dev, torch.int64)]                                  # [T, 3, 3]
+    A.require_device(tris)
+    area = torch.norm(torch.cross(tris[:, 0] - tris[:, 1], tris[:, 1] - tris[:, 2], dim=1), p=2, dim=1) * 0.5
+    cdf = torch.zeros(tris.shape[0] + 1, dtype=torch.float64, device=dev)
+    torch.cumsum(area.double(), 0, out=cdf[1:])
+    total = float(cdf[-1])
+    if not (total > 0.0 and total != float("inf")):
+        raise A.WispB200Error(f"mesh_to_octree: the total face area is {total} (it must be positive and finite)")
+    tris = tris.reshape(-1, 9)
+    bits = torch.zeros((8 ** level + 31) // 32, dtype=torch.int32, device=dev)
+    with _stage("mesh_octree"):
+        A.lib().wb_mesh_octree_bits(A.ptr(tris), A.ptr(cdf), tris.shape[0], int(num_samples), level,
+                                    int(seed) & 0xFFFFFFFF, A.ptr(bits), A.stream())
+    words = torch.nonzero(bits).reshape(-1)
+    set_bits = (bits[words, None] >> torch.arange(32, dtype=torch.int32, device=dev)) & 1
+    w, b = torch.nonzero(set_bits, as_tuple=True)
+    idx = words[w] * 32 + b
+    mask = (1 << level) - 1
+    points = torch.stack([idx >> (2 * level), (idx >> level) & mask, idx & mask], 1).to(torch.int16)
+    return spc.points_to_octree(points, level)
