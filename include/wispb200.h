@@ -9,7 +9,17 @@
  *     and returns 0 on success or a negative wb_status; wb_last_error() describes the last failure of the
  *     calling thread.  The reference raises from AT_ERROR/AT_CUDA_CHECK instead
  *     (wisp/csrc/ops/hashgrid_interpolate.cpp:66-68, uniform_sample_cuda.cu:95);
- *   - layouts are the reference's: row-major, float32 unless stated, int64 ridx, bool(u8) masks.
+ *   - layouts are the reference's: row-major, float32 unless stated, int64 ridx, bool(u8) masks;
+ *   - every launch, copy and memset of a call goes to that stream, none to the legacy default stream; work the library forks onto
+ *     its own side stream (the chunked precision-1 backward of wb_rf_shade_bwd) joins the caller's stream before the call returns;
+ *   - entry points may be called concurrently from several host threads, on one device or on several: the library's shared state
+ *     (per-device side streams and events, dynamic shared-memory limits, which are only ever raised) is guarded, the error text and
+ *     the wb_rf_workspace_holds_ray_rows hint are per thread;
+ *   - every stream-taking entry point can be captured into a CUDA graph (wb_sdf_trace's cooperative launch included) over buffers
+ *     allocated before the capture; a count -> scan -> fill chain is captured with the fill's outputs sized to a capacity, since
+ *     the caller reads the total on the host between the stages.  A captured wb_rf_shade_bwd never forks onto the shared side
+ *     stream: it runs the one-stream schedule (the same sums up to the order of the atomic additions), so captures and eager calls
+ *     of other threads cannot mix.  tests/test_gpu_stream_contract.py checks all of this per entry, the chunked backward included.
  *
  * Each group cites the reference interface it replaces (paths relative to the kaolin-wisp checkout).
  */

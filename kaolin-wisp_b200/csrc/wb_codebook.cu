@@ -141,7 +141,7 @@ extern "C" int wb_codebook_rows_bwd(const float* logits, const float* dictionary
     const int smem = (K * F + 8 * 32) * 4;          // dictionary gradient + one dE row per warp
     cudaStream_t st = (cudaStream_t)s;
     auto kern = K <= 256 ? wb_codebook_rows_bwd_kernel<8> : wb_codebook_rows_bwd_kernel<32>;
-    if (smem > 48 * 1024) WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    WB_CUDA(wb_allow_smem(kern, smem));
     kern<<<(unsigned)ctas, 256, smem, st>>>(logits, dictionary, dE, rows, K, F, g_logits, g_dictionary);
     WB_LAUNCH_CHECK();
     return WB_OK;

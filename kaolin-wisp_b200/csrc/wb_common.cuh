@@ -27,9 +27,14 @@ void wb_count_launch(int n = 1);
         wb_count_launch(); } while (0)
 
 int wb_num_sms();          // multiprocessor count of the CURRENT device (cached per device)
-int wb_cur_device();       // cudaGetDevice: function attributes (dynamic shared memory size) are per device -- the once-only caches
-                           // around cudaFuncSetAttribute fold it into their key (WB_ATTR_KEY)
-#define WB_ATTR_KEY(bytes) ((int64_t)(bytes) * 64 + wb_cur_device())
+int wb_cur_device();       // cudaGetDevice
+// Lets `kernel` launch with `bytes` of dynamic shared memory on the current device: raises its cudaFuncAttributeMaxDynamicSharedMemorySize
+// when the limit set so far for this (kernel, device) is lower, never lowers it.  Thread-safe: a call that needs less than another
+// thread's launch of the same kernel cannot undercut that launch between its attribute set and the launch itself.  The attribute is a
+// driver call that can wait behind other driver work (e.g. an NVML poll): it runs once per (kernel, device, larger size), not per launch.
+cudaError_t wb_allow_smem_fn(const void* kernel, int64_t bytes);
+template <class K> cudaError_t wb_allow_smem(K* kernel, int64_t bytes) { return wb_allow_smem_fn((const void*)kernel, bytes); }
+inline cudaError_t wb_allow_smem(const void* kernel, int64_t bytes) { return wb_allow_smem_fn(kernel, bytes); }
 
 // ---------------------------------------------------------------------------------------------
 // Jitter contract: counter-based stream keyed by (seed, ray, step).

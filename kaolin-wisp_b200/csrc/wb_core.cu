@@ -3,6 +3,9 @@
 #include "wb_featx.cuh"
 #include <stdarg.h>
 #include <atomic>
+#include <map>
+#include <mutex>
+#include <utility>
 #include <math.h>
 
 static thread_local char g_err[512] = "";
@@ -14,6 +17,18 @@ void wb_set_error(const char* fmt, ...) {
 void wb_count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
 int wb_cur_device() { int dev = 0; cudaGetDevice(&dev); return dev < 0 ? 0 : (dev & 63); }
+cudaError_t wb_allow_smem_fn(const void* kernel, int64_t bytes) {
+    if (bytes <= 48 * 1024) return cudaSuccess;                  // the default limit of every kernel
+    static std::mutex mu;
+    static std::map<std::pair<const void*, int>, int64_t> allowed;
+    const int dev = wb_cur_device();
+    std::lock_guard<std::mutex> lock(mu);
+    int64_t& cur = allowed[std::make_pair(kernel, dev)];
+    if (cur >= bytes) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e == cudaSuccess) cur = bytes;
+    return e;
+}
 int wb_num_sms() {
     static std::atomic<int> sms[64];
     const int dev = wb_cur_device();

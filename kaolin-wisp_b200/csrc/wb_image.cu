@@ -447,7 +447,7 @@ extern "C" int64_t wb_image_smem_bytes(const wb_nef_desc* grid, int32_t hidden_d
 template <class K>
 static int img_launch(K kern, const WbImg& m, int smem, int64_t work, wb_stream s)
 {
-    WB_CUDA(cudaFuncSetAttribute((const void*)kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    WB_CUDA(wb_allow_smem((const void*)kern, smem));
     int per_sm = 0;
     WB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)kern, WB_IMG_THREADS, smem));
     WB_CHECK_ARG(per_sm >= 1, "image kernel does not fit on an SM");

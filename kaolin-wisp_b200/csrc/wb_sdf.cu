@@ -372,13 +372,13 @@ extern "C" int wb_sdf_eval(const wb_octree* oct, const wb_sdf_desc* nef, int32_t
     const int smem = m.smem_floats * 4;
     int64_t ctas = (N + WB_SDF_THREADS - 1) / WB_SDF_THREADS; const int64_t cap = (int64_t)wb_num_sms() * 8; if (ctas > cap) ctas = cap;
     if (hash) {
-        if (smem > 48 * 1024) WB_CUDA(cudaFuncSetAttribute(wb_sdf_eval_hash_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        WB_CUDA(wb_allow_smem(wb_sdf_eval_hash_kernel, smem));
         wb_sdf_eval_hash_kernel<<<(unsigned)ctas, WB_SDF_THREADS, smem, (cudaStream_t)s>>>(hg, m, lod_idx + 1, coords, N, out);
         WB_LAUNCH_CHECK();
         return WB_OK;
     }
     auto kern = sdf_fast_shape(m) ? wb_sdf_eval_kernel<16, 1> : wb_sdf_eval_kernel<0, 0>;
-    if (smem > 48 * 1024) WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    WB_CUDA(wb_allow_smem(kern, smem));
     kern<<<(unsigned)ctas, WB_SDF_THREADS, smem, (cudaStream_t)s>>>(oc, m, lod_idx + 1, coords, N, out);
     WB_LAUNCH_CHECK();
     return WB_OK;
@@ -431,7 +431,7 @@ extern "C" int wb_sdf_trace(const wb_octree* oct, const wb_sdf_desc* nef, int32_
     rc = sdf_scan_packs(T, num_steps, st); if (rc) return rc;
     const int smem = m.smem_floats * 4;
     const void* kern = sdf_fast_shape(m) ? (const void*)wb_sdf_trace_kernel<16, 1> : (const void*)wb_sdf_trace_kernel<0, 0>;
-    if (smem > 48 * 1024) WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    WB_CUDA(wb_allow_smem(kern, smem));
     int per_sm = 0;
     WB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, WB_SDF_THREADS, smem));
     WB_CHECK_ARG(per_sm >= 1, "sphere-trace kernel does not fit on an SM");

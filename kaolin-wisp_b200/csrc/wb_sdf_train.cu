@@ -501,7 +501,7 @@ extern "C" int wb_sdf_train(const wb_octree* oct, const wb_sdf_desc* nef, int32_
         D.T = tile; D.SX = sdf_deep_stride(m.in_pad); D.SH = sdf_deep_stride(m.H);
         D.acc_off = (m.smem_floats + 3) & ~3; D.tile_off = 2 * D.acc_off; D.red_off = D.tile_off + tile * (D.SX + m.nh * D.SH + 1);
         const void* kern = hash ? (const void*)wb_sdf_train_deep_kernel<true> : (const void*)wb_sdf_train_deep_kernel<false>;
-        WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        WB_CUDA(wb_allow_smem(kern, smem));
         int per_sm = 0;
         WB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, WB_SDF_DEEP_THREADS, smem));
         WB_CHECK_ARG(per_sm >= 1, "training kernel does not fit on an SM");
@@ -517,7 +517,7 @@ extern "C" int wb_sdf_train(const wb_octree* oct, const wb_sdf_desc* nef, int32_
     T.gw_off = T.xs_off + WB_SDF_TRAIN_TILE * m.in_pad + WB_SDF_TRAIN_TILE;
     T.red_off = T.gw_off + (fast ? 0 : m.H * (m.in_pad + 1));
     const void* kern = hash ? (const void*)wb_sdf_train_kernel<0, 0, true> : fast ? (const void*)wb_sdf_train_kernel<16, 1> : (const void*)wb_sdf_train_kernel<0, 0>;
-    if (smem > 48 * 1024) WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    WB_CUDA(wb_allow_smem(kern, smem));
     int per_sm = 0;
     WB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, WB_SDF_TRAIN_TILE, smem));
     WB_CHECK_ARG(per_sm >= 1, "training kernel does not fit on an SM");

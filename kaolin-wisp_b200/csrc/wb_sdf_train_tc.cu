@@ -376,7 +376,7 @@ extern "C" int wb_sdf_train_tc(const wb_octree* oct, const wb_sdf_desc* nef, int
     int nl = lod_idx + 1;
     const void* kern = hash ? (const void*)wb_sdf_train_tc_kernel<0, true>
                      : (m.multiscale == 1 && m.F == 16) ? (const void*)wb_sdf_train_tc_kernel<16, false> : (const void*)wb_sdf_train_tc_kernel<0, false>;
-    WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    WB_CUDA(wb_allow_smem(kern, smem));
     int per_sm = 0;
     WB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, STC_THREADS, smem));
     WB_CHECK_ARG(per_sm >= 1, "training kernel does not fit on an SM");

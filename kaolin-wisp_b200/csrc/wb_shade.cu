@@ -356,7 +356,7 @@ static int wb_shade_fwd_launch(const WbGrid& g, const WbGridX& gx, const WbMlp& 
 {
     const size_t smem = (size_t)(m.fwd_floats + m.act_cols * (NT + 1)) * sizeof(float);
     if (smem > 227 * 1024) return 1;
-    { static int64_t done_for = -1; if (done_for != WB_ATTR_KEY(smem)) { WB_CUDA(cudaFuncSetAttribute(wb_shade_fwd_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); done_for = WB_ATTR_KEY(smem); } }
+    WB_CUDA(wb_allow_smem(wb_shade_fwd_kernel<NT>, (int64_t)smem));
     const int64_t ntiles = (in.S + NT - 1) / NT;
     int per_sm = (int)((227 * 1024) / (smem + 1024)); if (per_sm < 1) per_sm = 1; if (per_sm > 8) per_sm = 8;
     int64_t grid = (int64_t)wb_num_sms() * per_sm; if (grid > ntiles) grid = ntiles;
@@ -553,7 +553,7 @@ static int wb_shade_bwd_launch(const WbGrid& g, const WbGridX& gx, const WbMlp& 
 {
     const size_t smem = (size_t)(m.act_cols + 2 * m.maxw) * (NT + 1) * sizeof(float);
     if (smem > 227 * 1024) return 1;
-    { static int64_t done_for = -1; if (done_for != WB_ATTR_KEY(smem)) { WB_CUDA(cudaFuncSetAttribute(wb_shade_bwd_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); done_for = WB_ATTR_KEY(smem); } }
+    WB_CUDA(wb_allow_smem(wb_shade_bwd_kernel<NT>, (int64_t)smem));
     const int64_t ntiles = (in.S + NT - 1) / NT;
     int per_sm = (int)((227 * 1024) / (smem + 1024)); if (per_sm < 1) per_sm = 1; if (per_sm > 8) per_sm = 8;
     int64_t grid = (int64_t)wb_num_sms() * per_sm; if (grid > ntiles) grid = ntiles;

@@ -34,6 +34,7 @@
 #include "wb_shade_tc.cuh"
 #include "wb_tc.cuh"
 #include <math.h>
+#include <mutex>
 #include <type_traits>
 #include <utility>
 
@@ -619,15 +620,7 @@ int wb_tc_shade_fwd(const wb_nef_desc* nef, const float* blob, const wb_rays* ra
                                      : (per_sm == 2 ? wb_shade_fwd_tc_kernel<2, false, 128> : wb_shade_fwd_tc_kernel<1, false, 128>))
                      : (gx.kind != 0 ? (per_sm == 3 ? wb_shade_fwd_tc_kernel<3, true, 64> : wb_shade_fwd_tc_kernel<2, true, 64>)
                                      : (per_sm == 3 ? wb_shade_fwd_tc_kernel<3, false, 64> : wb_shade_fwd_tc_kernel<2, false, 64>));
-    {   // function attributes are driver calls that can wait behind other driver work (e.g. an NVML poll): set them once, not per launch
-        static int64_t done_for[2][2][4] = { { { -1, -1, -1, -1 }, { -1, -1, -1, -1 } }, { { -1, -1, -1, -1 }, { -1, -1, -1, -1 } } };
-        static int64_t done_nerf64 = -1;
-        int64_t& done = nerf64 ? done_nerf64 : done_for[wide ? 1 : 0][gx.kind != 0 ? 1 : 0][per_sm];
-        if (done != WB_ATTR_KEY(m.smem_bytes)) {
-            WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, m.smem_bytes));
-            done = WB_ATTR_KEY(m.smem_bytes);
-        }
-    }
+    WB_CUDA(wb_allow_smem(kern, m.smem_bytes));
     const int64_t ntiles = (S + TC_ROWS - 1) / TC_ROWS, nctas = (ntiles + TC_FWD_GROUPS - 1) / TC_FWD_GROUPS;
     int64_t grid = (int64_t)wb_num_sms() * per_sm; if (grid > nctas) grid = nctas;
     if (grid == 0) return WB_OK;
@@ -1051,15 +1044,7 @@ int wb_tc_decoder_bwd_ex(const wb_nef_desc* nef, const float* blob, const wb_ray
         const bool nerf64 = fuse && TcShapeNerf64::matches(m);
         auto kern = nerf64 ? wb_mlp_bwd_tc_kernel<2, true, TcShapeNerf64>
                   : m.groups == 2 ? (fuse ? wb_mlp_bwd_tc_kernel<2, true> : wb_mlp_bwd_tc_kernel<2, false>) : wb_mlp_bwd_tc_kernel<1, false>;
-        {
-            static int64_t done_for[2][2] = { { -1, -1 }, { -1, -1 } };
-            static int64_t done_nerf64 = -1;
-            int64_t& done = nerf64 ? done_nerf64 : done_for[m.groups - 1][fuse ? 1 : 0];
-            if (done != WB_ATTR_KEY(TC_SMEM_MAX)) {        // the passes of one call differ in size: allow the largest once
-                WB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
-                done = WB_ATTR_KEY(TC_SMEM_MAX);
-            }
-        }
+        WB_CUDA(wb_allow_smem(kern, TC_SMEM_MAX));         // the passes of one call differ in size: allow the largest once
         const int64_t nctas = ((s_end - s_begin + s_begin % TC_ROWS + TC_ROWS - 1) / TC_ROWS + m.groups - 1) / m.groups;
         int64_t grid = (int64_t)wb_num_sms(); if (grid > nctas) grid = nctas;         // 1 CTA / SM: shared memory holds the tiles and accumulators
         kern<<<(unsigned)grid, m.groups * TC_GROUP, m.smem_bytes, st>>>(m, reinterpret_cast<const uint8_t*>(blob), in,
@@ -1123,18 +1108,24 @@ int wb_tc_shaped(const wb_nef_desc* nef, int backward, int* shaped)
 // memory: two of its CTAs fit beside a decoder CTA) runs on a side stream.
 constexpr int64_t TC_CHUNKED_MIN_S = 1 << 20;
 constexpr int TC_CHUNKS = 4;
-struct TcSide { cudaStream_t stream; cudaEvent_t ev[TC_CHUNKS + 1]; bool ok; };      // one event per chunk + the join
-static TcSide* tc_side_stream()
+// One side stream and one set of fork / join events per device, shared by every caller on that device.  `mu` is held from the creation
+// check to the end of a call's enqueue loop: an event recorded by one thread must not be re-recorded by another before this thread's
+// cudaStreamWaitEvent has captured it, or a scatter would wait for another caller's decoder chunk instead of its own.
+struct TcSide { std::mutex mu; cudaStream_t stream; cudaEvent_t ev[TC_CHUNKS + 1]; bool ok; };      // one event per chunk + the join
+static TcSide* tc_side_stream_locked(TcSide& s)
 {
-    static TcSide side[64];
-    int dev = 0; if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
-    TcSide& s = side[dev];
     if (!s.ok) {
         if (cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) != cudaSuccess) return nullptr;
         for (int i = 0; i <= TC_CHUNKS; ++i) if (cudaEventCreateWithFlags(&s.ev[i], cudaEventDisableTiming) != cudaSuccess) return nullptr;
         s.ok = true;
     }
     return &s;
+}
+static TcSide* tc_side_slot()
+{
+    static TcSide side[64];
+    int dev = 0; if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
+    return &side[dev];
 }
 
 int wb_tc_shade_bwd(const wb_nef_desc* nef, const float* blob, const wb_rays* rays, const float* rec_t, const int32_t* rec_ray,
@@ -1150,7 +1141,14 @@ int wb_tc_shade_bwd(const wb_nef_desc* nef, const float* blob, const wb_rays* ra
             tc_bwd_layout(&m, masks[0], 1);
             wide = !tc_bwd_layout(&m, masks[0], 2);
         }
-        if (wide && (side = tc_side_stream()) != nullptr) {
+        // A call being captured into a graph runs the one-stream schedule (the same sums up to the order of the atomic additions): the
+        // shared side stream would otherwise join the capture, and another thread's eager call on it would be mixed into the graph.
+        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+        if (wide && cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap != cudaStreamCaptureStatusNone) wide = false;
+        TcSide* slot = wide ? tc_side_slot() : nullptr;
+        std::unique_lock<std::mutex> lock;
+        if (slot) { lock = std::unique_lock<std::mutex>(slot->mu); side = tc_side_stream_locked(*slot); }
+        if (side != nullptr) {
             const int64_t per = ((S + TC_CHUNKS - 1) / TC_CHUNKS + TC_ROWS - 1) / TC_ROWS * TC_ROWS;
             int rc = WB_OK, c = 0;
             for (int64_t s0 = 0; s0 < S && rc == WB_OK; s0 += per, ++c) {

@@ -73,7 +73,7 @@ extern "C" int wb_tc_selftest(const void* a_img, int a_bytes, const void* b_img,
     WB_CHECK_ARG((N == 8 || (N % 16 == 0 && N >= 16 && N <= 128)) && K % 16 == 0 && (mode & 3) <= 2 && a_bytes % 16 == 0 && b_bytes % 16 == 0, "bad shape");
     const size_t smem = ((a_bytes + 1023) & ~1023) + b_bytes + 1024;
     WB_CHECK_ARG(smem <= 200 * 1024, "tiles too large");
-    WB_CUDA(cudaFuncSetAttribute(wb_tc_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    WB_CUDA(wb_allow_smem(wb_tc_selftest_kernel, (int64_t)smem));
     wb_tc_selftest_kernel<<<1, 256, smem, (cudaStream_t)s>>>(reinterpret_cast<const uint4*>(a_img), a_bytes, reinterpret_cast<const uint4*>(b_img), b_bytes, D, N, K, mode);
     WB_LAUNCH_CHECK();
     return WB_OK;
