@@ -356,6 +356,7 @@ template <int D> __device__ __forceinline__ int tc_step(int l) { return l + D; }
 template <int D, int L> __device__ __forceinline__ TcInt<L + D> tc_step(TcInt<L>) { return {}; }
 struct TcShapeRt {
     static constexpr bool fixed = false;
+    static constexpr int kp0 = 0;                  // padded width of the first layer, when known at compile time
     static __device__ __forceinline__ int nl_d(const WbTc& m) { return m.nl_d; }
     static __device__ __forceinline__ int nl_c(const WbTc& m) { return m.nl_c; }
     static __device__ __forceinline__ int Kp(const WbTc& m, int l) { return m.Kp[l]; }
@@ -368,6 +369,7 @@ template <int... V> struct TcList {
 template <int ND, int NC, class KP, class NP>
 struct TcShape {
     static constexpr bool fixed = true;
+    static constexpr int kp0 = KP::at(0);
     static __device__ __forceinline__ int nl_d(const WbTc&) { return ND; }
     static __device__ __forceinline__ int nl_c(const WbTc&) { return NC; }
     static __device__ __forceinline__ int Kp(const WbTc&, int l) { return KP::at(l); }
@@ -815,16 +817,46 @@ wb_mlp_bwd_tc_kernel(WbTc m, const uint8_t* __restrict__ blob, TcIn in, const fl
     const int64_t tile0 = in.s_begin / TC_ROWS, ntiles = (s_end + TC_ROWS - 1) / TC_ROWS;
     const float z8[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
     const int lane = threadIdx.x & 31;
-    for (int64_t tile = tile0 + (int64_t)blockIdx.x * NG + c.g; tile < ntiles; tile += (int64_t)gridDim.x * NG) {
+    // TcShape instances load the next tile's saved rows, ray index and incoming gradient while this tile runs, so that their latency
+    // is spent under this tile's rounds and table scatter instead of at the start of the next tile (app/nerf: shade_bwd 16.3 -> 15.7 ms
+    // on H100, DESIGN.md section 4).  PF: saved-row chunks per thread (the two threads of a row split them); 0 for the run-time shape,
+    // which loads at the start of each tile.
+    constexpr int PF = S::kp0 / 16;
+    uint4 xr_n[PF > 0 ? PF : 1];
+    int64_t ray_n = 0;
+    float4 go_n = make_float4(0, 0, 0, 0);
+    auto fetch = [&](int64_t t) {
+        int64_t sn = t * TC_ROWS + c.r;
+        const bool vn = sn < s_end;
+        if (!vn) sn = s_end - 1;
+        ray_n = __ldg(in.rec_ray + sn);
+#pragma unroll
+        for (int i = 0; i < PF; ++i) xr_n[i] = __ldg(in.x0_saved + (int64_t)(c.h + 2 * i) * in.S + sn);
+        go_n = vn ? __ldg(g_shaded + sn) : make_float4(0, 0, 0, 0);
+    };
+    const int64_t tile_first = tile0 + (int64_t)blockIdx.x * NG + c.g, tile_step = (int64_t)gridDim.x * NG;
+    if constexpr (PF > 0) { if (tile_first < ntiles) fetch(tile_first); }
+    for (int64_t tile = tile_first; tile < ntiles; tile += tile_step) {
         int64_t s = tile * TC_ROWS + c.r;
         const bool valid = s < s_end;
         if (!valid) s = s_end - 1;
-        const int64_t ray = __ldg(in.rec_ray + s);
-        for (int ch = c.h; ch < nch0; ch += 2)                     // saved density-decoder input row (coalesced 16 B per lane)
-            *reinterpret_cast<uint4*>(t0 + ch * TC_SLAB + c.r * 16) = __ldg(in.x0_saved + (int64_t)ch * in.S + s);
         float df[16], c3[3];
-        tc_decoders<128, S>(m, c, in, ray, df, c3);
-        const float4 go = valid ? __ldg(g_shaded + s) : make_float4(0, 0, 0, 0);
+        int64_t ray;
+        float4 go;
+        if constexpr (PF > 0) {
+            ray = ray_n;
+            go = go_n;
+#pragma unroll
+            for (int i = 0; i < PF; ++i) *reinterpret_cast<uint4*>(t0 + (c.h + 2 * i) * TC_SLAB + c.r * 16) = xr_n[i];
+            if (tile + tile_step < ntiles) fetch(tile + tile_step);
+            tc_decoders<128, S>(m, c, in, ray, df, c3);
+        } else {
+            ray = __ldg(in.rec_ray + s);
+            for (int ch = c.h; ch < nch0; ch += 2)                 // saved density-decoder input row (coalesced 16 B per lane)
+                *reinterpret_cast<uint4*>(t0 + ch * TC_SLAB + c.r * 16) = __ldg(in.x0_saved + (int64_t)ch * in.S + s);
+            tc_decoders<128, S>(m, c, in, ray, df, c3);
+            go = valid ? __ldg(g_shaded + s) : make_float4(0, 0, 0, 0);
+        }
         // ---- colour decoder, last layer: dY = dL/d(pre-sigmoid), zero padded ----
         if (c.h == 0) {
             const float r = 1.0f / (1.0f + expf(-c3[0])), gg = 1.0f / (1.0f + expf(-c3[1])), b = 1.0f / (1.0f + expf(-c3[2]));
