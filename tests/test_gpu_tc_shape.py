@@ -1,6 +1,8 @@
 """The tensor-core decoder launches pick the kernel instances compiled for the app/nerf geometry (TcShapeNerf64 in wb_shade_tc.cu)
-exactly for decoders of that geometry: the bench-shaped decoder of test_gpu_tc_decoders.py (SIZE_CASE) and race_L13_pos run them, so
-that suite checks their results; other widths and embeddings keep the run-time instances."""
+exactly for decoders of that geometry: the bench-shaped decoder of test_gpu_tc_decoders.py (SIZE_CASE) and race_L13_pos run them;
+other widths and embeddings keep the run-time instances.  The geometry is the padded one, so the shaped instances serve a family of
+decoders: tests/test_gpu_tc_shape_family.py sweeps the selection against a mirror of it, checks members of that family inside the
+interval reference and runs the shaped kernels at coordinate, run and tile edges."""
 import ctypes as C
 
 import pytest
