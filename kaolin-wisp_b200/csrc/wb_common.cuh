@@ -26,6 +26,11 @@ void wb_count_launch(int n = 1);
         wb_set_error("%s: kernel launch failed: %s", __func__, cudaGetErrorString(e__)); return WB_ERR_CUDA; } \
         wb_count_launch(); } while (0)
 
+inline int wb_round_up(int v, int m) { return (v + m - 1) / m * m; }
+inline int64_t wb_align256(int64_t bytes) { return (bytes + 255) / 256 * 256; }       // workspace carve-outs
+// width of a position / view embedding (positional_embedder.py:51-66): mode 0 none, 1 identity, 2 sin/cos bands, 3 both
+inline int wb_embed_dim(int mode, int freq) { return mode == 0 ? 0 : mode == 1 ? 3 : mode == 2 ? 6 * freq : 3 + 6 * freq; }
+
 int wb_num_sms();          // multiprocessor count of the CURRENT device (cached per device)
 int wb_cur_device();       // cudaGetDevice
 // Lets `kernel` launch with `bytes` of dynamic shared memory on the current device: raises its cudaFuncAttributeMaxDynamicSharedMemorySize
@@ -210,6 +215,15 @@ __device__ __forceinline__ void wb_corner_setup(const WbGrid& g, int l, float cx
 }
 
 int wb_make_grid(const wb_nef_desc* d, WbGrid* g);     // host: validate + derive per-level constants
+// host: the decoders of a wb_nef_desc as the fp32 (WbMlp) and tensor-core (WbTc) shade planners both read them, before each applies
+// its own head-width limit and padding; a layer narrower than 1 or wider than max_width is refused with the message width_msg
+struct WbDecoders {
+    int nl_d, nl_c;                                                  // linear layers: density, colour
+    int I[2 * WB_MAX_LAYERS], O[2 * WB_MAX_LAYERS];                  // layer l's widths, the density layers first
+    int src_w[2 * WB_MAX_LAYERS], src_b[2 * WB_MAX_LAYERS];          // offsets into the packed nn.Linear parameter vectors (b = -1: no bias)
+    int feat_dim, pos_dim, view_dim;                                 // grid features, position and view embedding widths
+};
+int wb_make_decoders(const wb_nef_desc* d, int max_width, const char* width_msg, WbDecoders* dec);
 int wb_make_march(const wb_rays* rays, int n, const float* jitter, uint32_t seed, WbMarch* m);
 int wb_make_oct(const wb_octree* o, int level, WbOct* out);
 

@@ -85,6 +85,30 @@ int wb_make_grid(const wb_nef_desc* d, WbGrid* g) {
     return WB_OK;
 }
 
+int wb_make_decoders(const wb_nef_desc* d, int max_width, const char* width_msg, WbDecoders* dec) {
+    WB_CHECK_ARG(d->dens_layers >= 1 && d->dens_layers <= WB_MAX_LAYERS && d->col_layers >= 1 && d->col_layers <= WB_MAX_LAYERS, "unsupported decoder depth");
+    WB_CHECK_ARG(d->dens_params && d->col_params, "null decoder parameters");
+    memset(dec, 0, sizeof(*dec));
+    dec->nl_d = d->dens_layers; dec->nl_c = d->col_layers;
+    dec->feat_dim = d->multiscale == 0 ? d->num_lods * d->feature_dim : d->feature_dim;
+    dec->pos_dim = wb_embed_dim(d->pos_mode, d->pos_freq); dec->view_dim = wb_embed_dim(d->view_mode, d->view_freq);
+    WB_CHECK_ARG(d->dens_dims[0] == dec->feat_dim + dec->pos_dim, "decoder_density input width != grid features + position embedding");
+    WB_CHECK_ARG(d->col_dims[0] == d->dens_dims[d->dens_layers] - 1 + dec->view_dim, "decoder_color input width != density feats - 1 + view embedding");
+    WB_CHECK_ARG(d->col_dims[d->col_layers] == 3, "decoder_color output must be 3 wide");
+    int srcd = 0, srcc = 0;
+    for (int l = 0; l < dec->nl_d + dec->nl_c; ++l) {
+        const bool dens = l < dec->nl_d;
+        const int I = dens ? d->dens_dims[l] : d->col_dims[l - dec->nl_d];
+        const int O = dens ? d->dens_dims[l + 1] : d->col_dims[l - dec->nl_d + 1];
+        WB_CHECK_ARG(I >= 1 && I <= max_width && O >= 1 && O <= max_width, width_msg);
+        dec->I[l] = I; dec->O[l] = O;
+        int& src = dens ? srcd : srcc;
+        dec->src_w[l] = src; src += I * O;
+        if (d->has_bias) { dec->src_b[l] = src; src += O; } else dec->src_b[l] = -1;
+    }
+    return WB_OK;
+}
+
 int wb_make_gridx(const wb_nef_desc* d, bool backward, WbGridX* x) {
     WB_CHECK_ARG(d != nullptr, "null descriptor");
     memset(x, 0, sizeof(*x));

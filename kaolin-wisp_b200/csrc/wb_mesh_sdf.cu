@@ -41,15 +41,13 @@ struct MsdfWs {
     size_t bounds, keys_in, keys_out, cub, cub_bytes, tris, box, child, parent, flag, total;
 };
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 int msdf_layout(int64_t T, MsdfWs* w)
 {
     size_t cub_bytes = 0;
     if (T > 0 && cub::DeviceRadixSort::SortKeys(nullptr, cub_bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)T, 0, 62) != cudaSuccess)
         return -1;
     size_t o = 0;
-    auto take = [&](size_t bytes) { const size_t at = o; o = align256(o + bytes); return at; };
+    auto take = [&](size_t bytes) { const size_t at = o; o = wb_align256(o + bytes); return at; };
     const size_t nodes = T > 0 ? (size_t)(2 * T - 1) : 0, inner = T > 1 ? (size_t)(T - 1) : 0;
     w->bounds = take(8 * sizeof(uint32_t));
     w->keys_in = take((size_t)T * sizeof(uint64_t));

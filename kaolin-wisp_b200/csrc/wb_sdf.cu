@@ -364,8 +364,7 @@ extern "C" int wb_sdf_eval(const wb_octree* oct, const wb_sdf_desc* nef, int32_t
     if (N == 0) return WB_OK;
     WbSdf m; WbGrid hg; int rc = wb_make_sdf(nef, &m, &hg); if (rc) return rc;
     const bool hash = hg.table != nullptr;
-    WB_CHECK_ARG(lod_idx >= 0 && lod_idx < m.num_lods, "lod_idx out of range");
-    WB_CHECK_ARG(hash || m.multiscale == 1 || lod_idx == m.num_lods - 1, "'cat' octree grids feed the decoder all LODs: lod_idx must be num_lods-1");
+    rc = sdf_check_lod(m, hash, lod_idx); if (rc) return rc;
     WbOct oc; memset(&oc, 0, sizeof(oc));
     if (!hash) { rc = wb_make_oct(oct, m.base_lod + lod_idx, &oc); if (rc) return rc; }
     WB_CHECK_ARG(coords && out, "null pointer");

@@ -1,8 +1,9 @@
 // wb_sdf.cuh -- the NeuralSDF(OctreeGrid | HashGrid) field shared by wb_sdf.cu (evaluation, sphere tracing) and wb_sdf_train.cu
-// (training step): host-side description, the decoder's shared-memory image, the position embedding and the octree and hash-grid
-// feature gathers.
+// and wb_sdf_train_tc.cu (training steps): host-side description, the decoder's shared-memory image, the position embedding, the
+// octree and hash-grid feature gathers, and the host route of the training launches.
 #pragma once
 #include "wb_common.cuh"
+#include "wb_featx.cuh"
 
 constexpr int WB_SDF_MAX_IN = 132;        // 3 + 6*freq position embedding + features
 constexpr int WB_SDF_MAX_H = 128;
@@ -18,8 +19,6 @@ struct WbSdf {
     const float* params;                                                     // packed [W0, b0, W1, b1, ..., Wout, bout] (nn.Linear layout)
     int smem_floats;
 };
-
-static inline int sdf_embed_dim(int mode, int freq) { return mode == 0 ? 0 : mode == 1 ? 3 : mode == 2 ? 6 * freq : 3 + 6 * freq; }
 
 // hg: the hash grid of a hash field (d->hash != NULL), validated by wb_make_grid; hg->table == nullptr for an octree field
 static inline int wb_make_sdf(const wb_sdf_desc* d, WbSdf* m, WbGrid* hg)
@@ -45,7 +44,7 @@ static inline int wb_make_sdf(const wb_sdf_desc* d, WbSdf* m, WbGrid* hg)
         m->half_round = d->half_round;
     }
     m->F = d->feature_dim; m->base_lod = d->base_lod; m->num_lods = d->num_lods; m->multiscale = d->multiscale;
-    m->pos_mode = d->pos_mode; m->pos_freq = d->pos_freq; m->pos_dim = sdf_embed_dim(d->pos_mode, d->pos_freq);
+    m->pos_mode = d->pos_mode; m->pos_freq = d->pos_freq; m->pos_dim = wb_embed_dim(d->pos_mode, d->pos_freq);
     m->feat_dim = d->multiscale ? d->feature_dim : d->feature_dim * d->num_lods;
     m->in_dim = m->pos_dim + m->feat_dim; m->in_pad = (m->in_dim + 3) & ~3;
     WB_CHECK_ARG(m->in_dim <= WB_SDF_MAX_IN, "decoder input too wide");
@@ -230,3 +229,49 @@ __device__ __forceinline__ void sdf_hash_scatter(const WbGrid& g, float* gt, int
 
 // the app/nglod shape (nglod_octree.yaml): 'sum' grid of 16 features, identity position input, one hidden layer
 static inline bool sdf_fast_shape(const WbSdf& m) { return m.multiscale == 1 && m.F == 16 && m.pos_mode == 1 && m.nh == 1; }
+
+// lod_idx of a call on the field m (hash: a hash field): one of its LODs, and the finest for a 'cat' octree grid
+static inline int sdf_check_lod(const WbSdf& m, bool hash, int lod_idx)
+{
+    WB_CHECK_ARG(lod_idx >= 0 && lod_idx < m.num_lods, "lod_idx out of range");
+    WB_CHECK_ARG(hash || m.multiscale == 1 || lod_idx == m.num_lods - 1, "'cat' octree grids feed the decoder all LODs: lod_idx must be num_lods-1");
+    return WB_OK;
+}
+
+// The gradient target of a training launch.  Hash field: gx->gptr[0] = grad_feats[0], the 16-byte aligned codebook gradient (*oc and
+// the rest of *gx stay zero).  Octree field: the octree at the loss LOD and a WbGridX of kind 2 over LODs 0..lod_idx with gradients
+// grad_feats[k], 16-byte aligned too when `aligned` (the float4 scatter of the fp32 fast shape).
+static inline int sdf_grad_target(const wb_octree* oct, const WbSdf& m, bool hash, int lod_idx, float* const* grad_feats, bool aligned,
+                                  WbOct* oc, WbGridX* gx)
+{
+    memset(oc, 0, sizeof(*oc)); memset(gx, 0, sizeof(*gx));
+    if (hash) {
+        WB_CHECK_ARG(grad_feats[0] != nullptr && (reinterpret_cast<uintptr_t>(grad_feats[0]) & 15u) == 0, "hash field: null or unaligned table gradient");
+        gx->gptr[0] = grad_feats[0];
+        return WB_OK;
+    }
+    const int rc = wb_make_oct(oct, m.base_lod + lod_idx, oc); if (rc) return rc;
+    gx->kind = 2; gx->nl = lod_idx + 1; gx->sum = m.multiscale; gx->C = m.F;
+    gx->octree = oc->octree; gx->prefix = oc->prefix; gx->points = m.points; gx->trinkets = m.trinkets;
+    gx->base_lod = m.base_lod; gx->half_round = m.half_round;
+    for (int k = 0; k <= lod_idx; ++k) {
+        WB_CHECK_ARG(grad_feats[k] != nullptr, "null gradient level");
+        WB_CHECK_ARG(!aligned || (reinterpret_cast<uintptr_t>(grad_feats[k]) & 15u) == 0, "gradient levels must be 16-byte aligned");
+        gx->ptr[k] = m.feats[k]; gx->gptr[k] = grad_feats[k];
+    }
+    return WB_OK;
+}
+
+// One launch of a grid-stride training kernel: `threads` per CTA, one CTA per `tile` of the N samples, capped at the CTAs the device
+// holds at once with `smem` bytes of dynamic shared memory each.  args: the kernel's parameters, as cudaLaunchKernel takes them.
+static inline int sdf_train_launch(const void* kern, void** args, int threads, int smem, int64_t N, int tile, cudaStream_t st)
+{
+    WB_CUDA(wb_allow_smem(kern, smem));
+    int per_sm = 0;
+    WB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+    WB_CHECK_ARG(per_sm >= 1, "training kernel does not fit on an SM");
+    int64_t ctas = (N + tile - 1) / tile; const int64_t cap = (int64_t)wb_num_sms() * per_sm; if (ctas > cap) ctas = cap;
+    WB_CUDA(cudaLaunchKernel(kern, dim3((unsigned)ctas), dim3(threads), args, (size_t)smem, st));
+    wb_count_launch();
+    return WB_OK;
+}

@@ -16,7 +16,6 @@
 // A hash field (NeuralSDF(HashGrid), the HASH instances) runs the same kernels with the hash-grid gather of wb_sdf.cuh and the
 // scatter below in place of the octree's; everything else (tiles, summation orders, footprint) is unchanged.
 #include "wb_sdf.cuh"
-#include "wb_featx.cuh"
 
 constexpr int WB_SDF_TRAIN_TILE = 128;
 
@@ -473,27 +472,11 @@ extern "C" int wb_sdf_train(const wb_octree* oct, const wb_sdf_desc* nef, int32_
     const bool hash = hg.table != nullptr;
     int tile = 0; const int smem = sdf_train_plan(m, &tile);
     WB_CHECK_ARG(smem > 0, "decoder weights, their gradient accumulators and a 32-sample tile exceed shared memory (wb_sdf_train_smem_bytes < 0)");
-    WB_CHECK_ARG(lod_idx >= 0 && lod_idx < m.num_lods, "lod_idx out of range");
-    WB_CHECK_ARG(hash || m.multiscale == 1 || lod_idx == m.num_lods - 1, "'cat' octree grids feed the decoder all LODs: lod_idx must be num_lods-1");
+    rc = sdf_check_lod(m, hash, lod_idx); if (rc) return rc;
     WB_CHECK_ARG(coords && sdf_gt && grad_feats && grad_params && loss_out && N >= 0, "null pointer");
     if (N == 0) return WB_OK;
-    WbOct oc; memset(&oc, 0, sizeof(oc));
     const bool fast = !hash && sdf_fast_shape(m);
-    WbGridX gx; memset(&gx, 0, sizeof(gx));
-    if (hash) {                                            // kind 0: the hash grid of hg; its gradient is the one codebook table
-        WB_CHECK_ARG(grad_feats[0] != nullptr && (reinterpret_cast<uintptr_t>(grad_feats[0]) & 15u) == 0, "hash field: null or unaligned table gradient");
-        gx.gptr[0] = grad_feats[0];
-    } else {
-        rc = wb_make_oct(oct, m.base_lod + lod_idx, &oc); if (rc) return rc;
-        gx.kind = 2; gx.nl = lod_idx + 1; gx.sum = m.multiscale; gx.C = m.F;
-        gx.octree = oc.octree; gx.prefix = oc.prefix; gx.points = m.points; gx.trinkets = m.trinkets;
-        gx.base_lod = m.base_lod; gx.half_round = m.half_round;
-        for (int k = 0; k <= lod_idx; ++k) {
-            WB_CHECK_ARG(grad_feats[k] != nullptr, "null gradient level");
-            WB_CHECK_ARG(!fast || (reinterpret_cast<uintptr_t>(grad_feats[k]) & 15u) == 0, "gradient levels must be 16-byte aligned");
-            gx.ptr[k] = m.feats[k]; gx.gptr[k] = grad_feats[k];
-        }
-    }
+    WbOct oc; WbGridX gx; rc = sdf_grad_target(oct, m, hash, lod_idx, grad_feats, fast, &oc, &gx); if (rc) return rc;
     int nl = lod_idx + 1;
     if (m.nh > 1) {
         WbSdfTrainDeep D;
@@ -501,15 +484,8 @@ extern "C" int wb_sdf_train(const wb_octree* oct, const wb_sdf_desc* nef, int32_
         D.T = tile; D.SX = sdf_deep_stride(m.in_pad); D.SH = sdf_deep_stride(m.H);
         D.acc_off = (m.smem_floats + 3) & ~3; D.tile_off = 2 * D.acc_off; D.red_off = D.tile_off + tile * (D.SX + m.nh * D.SH + 1);
         const void* kern = hash ? (const void*)wb_sdf_train_deep_kernel<true> : (const void*)wb_sdf_train_deep_kernel<false>;
-        WB_CUDA(wb_allow_smem(kern, smem));
-        int per_sm = 0;
-        WB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, WB_SDF_DEEP_THREADS, smem));
-        WB_CHECK_ARG(per_sm >= 1, "training kernel does not fit on an SM");
-        int64_t ctas = (N + tile - 1) / tile; const int64_t cap = (int64_t)wb_num_sms() * per_sm; if (ctas > cap) ctas = cap;
         void* args[] = { &oc, &m, &gx, &nl, &D, &hg };
-        WB_CUDA(cudaLaunchKernel(kern, dim3((unsigned)ctas), dim3(WB_SDF_DEEP_THREADS), args, (size_t)smem, (cudaStream_t)s));
-        wb_count_launch();
-        return WB_OK;
+        return sdf_train_launch(kern, args, WB_SDF_DEEP_THREADS, smem, N, tile, (cudaStream_t)s);
     }
     WbSdfTrain T;
     T.coords = coords; T.gt = sdf_gt; T.N = N; T.inv_count = inv_count; T.gparams = grad_params; T.loss = loss_out;
@@ -517,13 +493,6 @@ extern "C" int wb_sdf_train(const wb_octree* oct, const wb_sdf_desc* nef, int32_
     T.gw_off = T.xs_off + WB_SDF_TRAIN_TILE * m.in_pad + WB_SDF_TRAIN_TILE;
     T.red_off = T.gw_off + (fast ? 0 : m.H * (m.in_pad + 1));
     const void* kern = hash ? (const void*)wb_sdf_train_kernel<0, 0, true> : fast ? (const void*)wb_sdf_train_kernel<16, 1> : (const void*)wb_sdf_train_kernel<0, 0>;
-    WB_CUDA(wb_allow_smem(kern, smem));
-    int per_sm = 0;
-    WB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, WB_SDF_TRAIN_TILE, smem));
-    WB_CHECK_ARG(per_sm >= 1, "training kernel does not fit on an SM");
-    int64_t ctas = (N + WB_SDF_TRAIN_TILE - 1) / WB_SDF_TRAIN_TILE; const int64_t cap = (int64_t)wb_num_sms() * per_sm; if (ctas > cap) ctas = cap;
     void* args[] = { &oc, &m, &gx, &nl, &T, &hg };
-    WB_CUDA(cudaLaunchKernel(kern, dim3((unsigned)ctas), dim3(WB_SDF_TRAIN_TILE), args, (size_t)smem, (cudaStream_t)s));
-    wb_count_launch();
-    return WB_OK;
+    return sdf_train_launch(kern, args, WB_SDF_TRAIN_TILE, smem, N, WB_SDF_TRAIN_TILE, (cudaStream_t)s);
 }

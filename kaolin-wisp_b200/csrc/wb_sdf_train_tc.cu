@@ -24,7 +24,6 @@
 // The decoder's fp16 weight packs are built by every CTA from the flat fp32 parameter buffer (the weights change every Adam step: no
 // separate pack launch), and the CTA's accumulators are added to grad_params once at the end.  wgmma.wait_group 0 after every chain.
 #include "wb_sdf.cuh"
-#include "wb_featx.cuh"
 #include "wb_tc.cuh"
 #include <cmath>
 
@@ -44,26 +43,24 @@ struct WbSdfTc {
     int smem;
 };
 
-static int stc_up(int v, int m) { return (v + m - 1) / m * m; }
-
 // shared memory of the launch for the field m (bytes), or -1 when it exceeds an SM's 227 KB
 static int sdf_tc_plan(const WbSdf& m, WbSdfTc* P)
 {
     memset(P, 0, sizeof(*P));
     P->IN = m.in_dim; P->pd = m.pos_dim; P->FD = m.feat_dim; P->H = m.H; P->nh = m.nh;
-    P->Hp = stc_up(m.H, 16); P->K0p = stc_up(m.in_dim, 16);
+    P->Hp = wb_round_up(m.H, 16); P->K0p = wb_round_up(m.in_dim, 16);
     int off = 0;
     for (int l = 0; l < m.nh; ++l) { P->w_off[l] = off; off += P->Hp * (l == 0 ? P->K0p : P->Hp) * 2; }
-    P->b_off = off; off += stc_up(m.nh * P->Hp * 2, 16);
+    P->b_off = off; off += wb_round_up(m.nh * P->Hp * 2, 16);
     P->wo_off = off; off += (P->Hp + 4) * 4;
-    P->acc_off = off = stc_up(off, 128);
+    P->acc_off = off = wb_round_up(off, 128);
     int acc = 0;
     for (int l = 0; l < m.nh; ++l) { P->acc_l[l] = acc; acc += m.H * ((l == 0 ? m.in_dim : m.H) + 1); }
     P->acc_l[m.nh] = acc; acc += m.H;
-    off = stc_up(off + acc * 4, 128);
+    off = wb_round_up(off + acc * 4, 128);
     for (int l = 0; l <= m.nh; ++l) { P->x_off[l] = off; off += ((l == 0 ? P->K0p : P->Hp) / 8 + 1) * STC_SLAB; }
-    P->dy_off = off; off += stc_up(P->Hp, 64) / 8 * STC_SLAB;      // the weight-gradient A operand reads 64 outputs (8 slabs) per pass
-    P->gf_off = off; off += stc_up(STC_ROWS * (P->FD + 1) * 4, 16);
+    P->dy_off = off; off += wb_round_up(P->Hp, 64) / 8 * STC_SLAB;      // the weight-gradient A operand reads 64 outputs (8 slabs) per pass
+    P->gf_off = off; off += wb_round_up(STC_ROWS * (P->FD + 1) * 4, 16);
     P->dys_off = off; off += STC_ROWS * 4;
     P->red_off = off; off += 2 * (STC_THREADS / 32) * 4;
     P->smem = off;
@@ -348,26 +345,11 @@ extern "C" int wb_sdf_train_tc(const wb_octree* oct, const wb_sdf_desc* nef, int
     const bool hash = hg.table != nullptr;
     WbSdfTc P; const int smem = sdf_tc_plan(m, &P);
     WB_CHECK_ARG(smem > 0, "fp16 weights, fp32 gradient accumulators and one 64-sample tile exceed shared memory (wb_sdf_train_tc_smem_bytes < 0)");
-    WB_CHECK_ARG(lod_idx >= 0 && lod_idx < m.num_lods, "lod_idx out of range");
-    WB_CHECK_ARG(hash || m.multiscale == 1 || lod_idx == m.num_lods - 1, "'cat' octree grids feed the decoder all LODs: lod_idx must be num_lods-1");
+    rc = sdf_check_lod(m, hash, lod_idx); if (rc) return rc;
     WB_CHECK_ARG((N == 0 || (coords && sdf_gt)) && grad_feats && grad_params && loss_out && N >= 0, "null pointer");
     WB_CHECK_ARG(std::isfinite(inv_count) && inv_count >= 0.0f, "inv_count must be finite and >= 0");
     if (N == 0) return WB_OK;
-    WbOct oc; memset(&oc, 0, sizeof(oc));
-    WbGridX gx; memset(&gx, 0, sizeof(gx));
-    if (hash) {
-        WB_CHECK_ARG(grad_feats[0] != nullptr && (reinterpret_cast<uintptr_t>(grad_feats[0]) & 15u) == 0, "hash field: null or unaligned table gradient");
-        gx.gptr[0] = grad_feats[0];
-    } else {
-        rc = wb_make_oct(oct, m.base_lod + lod_idx, &oc); if (rc) return rc;
-        gx.kind = 2; gx.nl = lod_idx + 1; gx.sum = m.multiscale; gx.C = m.F;
-        gx.octree = oc.octree; gx.prefix = oc.prefix; gx.points = m.points; gx.trinkets = m.trinkets;
-        gx.base_lod = m.base_lod; gx.half_round = m.half_round;
-        for (int k = 0; k <= lod_idx; ++k) {
-            WB_CHECK_ARG(grad_feats[k] != nullptr, "null gradient level");
-            gx.ptr[k] = m.feats[k]; gx.gptr[k] = grad_feats[k];
-        }
-    }
+    WbOct oc; WbGridX gx; rc = sdf_grad_target(oct, m, hash, lod_idx, grad_feats, false, &oc, &gx); if (rc) return rc;
     // loss scale: a power of two with inv_count * scale in [0.5, 1), so dY ~ 2 (y - gt) whatever the batch size
     int e = 0;
     if (inv_count > 0.0f) frexpf(inv_count, &e);
@@ -376,13 +358,6 @@ extern "C" int wb_sdf_train_tc(const wb_octree* oct, const wb_sdf_desc* nef, int
     int nl = lod_idx + 1;
     const void* kern = hash ? (const void*)wb_sdf_train_tc_kernel<0, true>
                      : (m.multiscale == 1 && m.F == 16) ? (const void*)wb_sdf_train_tc_kernel<16, false> : (const void*)wb_sdf_train_tc_kernel<0, false>;
-    WB_CUDA(wb_allow_smem(kern, smem));
-    int per_sm = 0;
-    WB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, STC_THREADS, smem));
-    WB_CHECK_ARG(per_sm >= 1, "training kernel does not fit on an SM");
-    int64_t ctas = (N + STC_ROWS - 1) / STC_ROWS; const int64_t cap = (int64_t)wb_num_sms() * per_sm; if (ctas > cap) ctas = cap;
     void* args[] = { &oc, &m, &gx, &nl, &P, &hg };
-    WB_CUDA(cudaLaunchKernel(kern, dim3((unsigned)ctas), dim3(STC_THREADS), args, (size_t)smem, (cudaStream_t)s));
-    wb_count_launch();
-    return WB_OK;
+    return sdf_train_launch(kern, args, STC_THREADS, smem, N, STC_ROWS, (cudaStream_t)s);
 }

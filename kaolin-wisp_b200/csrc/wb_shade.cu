@@ -19,7 +19,7 @@
 #include "wb_shade_tc.cuh"
 #include <math.h>
 
-#define WB_ML 16          // max linear layers over both decoders
+#define WB_ML (2 * WB_MAX_LAYERS)     // max linear layers over both decoders
 
 extern "C" int64_t wb_rf_workspace_bytes(const wb_nef_desc* nef, int32_t precision, int64_t R, int64_t S, int32_t backward)
 {
@@ -83,37 +83,23 @@ struct WbMlp {
     int pos_mode, pos_freq, view_mode, view_freq;
 };
 
-static int wb_embed_dim(int mode, int freq) { return mode == 0 ? 0 : mode == 1 ? 3 : mode == 2 ? 6 * freq : 3 + 6 * freq; }
-static int wb_round_up(int v, int m) { return (v + m - 1) / m * m; }
-
 // retain = true: every layer keeps its own input/output columns (backward); false: ping-pong (forward only)
 static int wb_make_mlp(const wb_nef_desc* d, bool retain, WbMlp* m)
 {
-    WB_CHECK_ARG(d->dens_layers >= 1 && d->col_layers >= 1 && d->dens_layers + d->col_layers <= WB_ML, "unsupported decoder depth");
-    WB_CHECK_ARG(d->dens_params && d->col_params, "null decoder parameters");
+    WbDecoders dec; const int rc = wb_make_decoders(d, 256, "layer width out of range (1..256)", &dec); if (rc) return rc;
+    WB_CHECK_ARG(dec.O[dec.nl_d - 1] >= 2, "decoder_density output must be >= 2 wide");
     memset(m, 0, sizeof(*m));
-    m->nl_d = d->dens_layers; m->nl_c = d->col_layers;
-    m->feat_dim = d->multiscale == 0 ? d->num_lods * d->feature_dim : d->feature_dim;
+    m->nl_d = dec.nl_d; m->nl_c = dec.nl_c;
+    m->feat_dim = dec.feat_dim; m->pos_dim = dec.pos_dim; m->view_dim = dec.view_dim;
     m->pos_mode = d->pos_mode; m->pos_freq = d->pos_freq; m->view_mode = d->view_mode; m->view_freq = d->view_freq;
-    m->pos_dim = wb_embed_dim(d->pos_mode, d->pos_freq); m->view_dim = wb_embed_dim(d->view_mode, d->view_freq);
-    WB_CHECK_ARG(d->dens_dims[0] == m->feat_dim + m->pos_dim, "decoder_density input width != grid features + position embedding");
-    const int dout = d->dens_dims[d->dens_layers];
-    WB_CHECK_ARG(dout >= 2, "decoder_density output must be >= 2 wide");
-    WB_CHECK_ARG(d->col_dims[0] == dout - 1 + m->view_dim, "decoder_color input width != density feats - 1 + view embedding");
-    WB_CHECK_ARG(d->col_dims[d->col_layers] == 3, "decoder_color output must be 3 wide");
-    int off = 0, srcd = 0, srcc = 0, maxw = 0;
+    int off = 0, maxw = 0;
     const int nl = m->nl_d + m->nl_c;
     for (int l = 0; l < nl; ++l) {
-        const bool dens = l < m->nl_d;
-        const int I = dens ? d->dens_dims[l] : d->col_dims[l - m->nl_d];
-        const int O = dens ? d->dens_dims[l + 1] : d->col_dims[l - m->nl_d + 1];
-        WB_CHECK_ARG(I >= 1 && I <= 256 && O >= 1 && O <= 256, "layer width out of range (1..256)");
+        const int I = dec.I[l], O = dec.O[l];
         m->I[l] = I; m->O[l] = O; m->Opad[l] = wb_round_up(O, 8); m->Ipad[l] = wb_round_up(I, 8);
         m->w_off[l] = off; off += I * m->Opad[l];
         m->b_off[l] = off; off += m->Opad[l];
-        int& src = dens ? srcd : srcc;
-        m->src_w[l] = src; src += I * O;
-        if (d->has_bias) { m->src_b[l] = src; src += O; } else m->src_b[l] = -1;
+        m->src_w[l] = dec.src_w[l]; m->src_b[l] = dec.src_b[l];
         if (m->Ipad[l] > maxw) maxw = m->Ipad[l];
         if (m->Opad[l] > maxw) maxw = m->Opad[l];
     }

@@ -38,7 +38,7 @@
 #include <type_traits>
 #include <utility>
 
-#define TC_ML 16
+#define TC_ML (2 * WB_MAX_LAYERS)
 constexpr int TC_ROWS = 64;                 // samples per sub-tile (wgmma M)
 constexpr int TC_GROUP = 128;               // threads per sub-tile group: one warpgroup, 64 rows x 2 column halves
 constexpr int TC_SLAB = TC_ROWS * 16;       // bytes of one slab (8 features of every sample of the tile)
@@ -65,9 +65,6 @@ struct WbTc {
     int feat_dim, pos_dim, view_dim, pos_mode, pos_freq, view_mode, view_freq;
 };
 
-static int tc_round_up(int v, int m) { return (v + m - 1) / m * m; }
-static int tc_embed_dim(int mode, int freq) { return mode == 0 ? 0 : mode == 1 ? 3 : mode == 2 ? 6 * freq : 3 + 6 * freq; }
-
 // backward shared-memory plan for `groups` groups that accumulate the weight gradients of the layers in `wmask`;
 // returns false when it does not fit
 static bool tc_bwd_layout(WbTc* m, unsigned wmask, int groups)
@@ -84,7 +81,7 @@ static bool tc_bwd_layout(WbTc* m, unsigned wmask, int groups)
         m->acc_l[l] = -1;
         if ((wmask >> l) & 1u) { m->acc_l[l] = acc; acc += m->O[l] * (m->I[l] + 1); }
     }
-    off += tc_round_up(acc * 4, 16);
+    off += wb_round_up(acc * 4, 16);
     m->group_bytes = off;
     m->groups = groups;
     m->w_smem_off = groups * off;
@@ -95,34 +92,24 @@ static bool tc_bwd_layout(WbTc* m, unsigned wmask, int groups)
 // returns WB_OK, or WB_ERR_INVALID with a message when the configuration does not fit the tensor-core path
 int wb_tc_make(const wb_nef_desc* d, bool backward, WbTc* m)
 {
-    WB_CHECK_ARG(d->dens_layers >= 1 && d->col_layers >= 1 && d->dens_layers + d->col_layers <= TC_ML, "unsupported decoder depth");
-    WB_CHECK_ARG(d->dens_params && d->col_params, "null decoder parameters");
-    memset(m, 0, sizeof(*m));
-    m->nl_d = d->dens_layers; m->nl_c = d->col_layers;
-    m->feat_dim = d->multiscale == 0 ? d->num_lods * d->feature_dim : d->feature_dim;
-    m->pos_mode = d->pos_mode; m->pos_freq = d->pos_freq; m->view_mode = d->view_mode; m->view_freq = d->view_freq;
-    m->pos_dim = tc_embed_dim(d->pos_mode, d->pos_freq); m->view_dim = tc_embed_dim(d->view_mode, d->view_freq);
-    WB_CHECK_ARG(d->dens_dims[0] == m->feat_dim + m->pos_dim, "decoder_density input width != grid features + position embedding");
-    const int dout = d->dens_dims[d->dens_layers];
+    WbDecoders dec; const int rc = wb_make_decoders(d, 128, "tensor-core path: layer widths must be <= 128", &dec); if (rc) return rc;
+    const int dout = dec.O[dec.nl_d - 1];
     WB_CHECK_ARG(dout >= 2 && dout <= 16, "tensor-core path: decoder_density output must be 2..16 wide");
-    WB_CHECK_ARG(d->col_dims[0] == dout - 1 + m->view_dim, "decoder_color input width != density feats - 1 + view embedding");
-    WB_CHECK_ARG(d->col_dims[d->col_layers] == 3, "decoder_color output must be 3 wide");
+    memset(m, 0, sizeof(*m));
+    m->nl_d = dec.nl_d; m->nl_c = dec.nl_c;
+    m->feat_dim = dec.feat_dim; m->pos_dim = dec.pos_dim; m->view_dim = dec.view_dim;
+    m->pos_mode = d->pos_mode; m->pos_freq = d->pos_freq; m->view_mode = d->view_mode; m->view_freq = d->view_freq;
     const int nl = m->nl_d + m->nl_c;
-    int off = 0, srcd = 0, srcc = 0, maxw = 0;
+    int off = 0, maxw = 0;
     for (int l = 0; l < nl; ++l) {
-        const bool dens = l < m->nl_d;
-        const int I = dens ? d->dens_dims[l] : d->col_dims[l - m->nl_d];
-        const int O = dens ? d->dens_dims[l + 1] : d->col_dims[l - m->nl_d + 1];
-        WB_CHECK_ARG(I >= 1 && I <= 128 && O >= 1 && O <= 128, "tensor-core path: layer widths must be <= 128");
-        m->I[l] = I; m->O[l] = O; m->Kp[l] = tc_round_up(I, 16); m->Np[l] = tc_round_up(O, 16);
+        const int I = dec.I[l], O = dec.O[l];
+        m->I[l] = I; m->O[l] = O; m->Kp[l] = wb_round_up(I, 16); m->Np[l] = wb_round_up(O, 16);
         m->w_off[l] = off; off += m->Kp[l] * m->Np[l] * 2;
         m->b_off[l] = off; off += m->Np[l] * 32;
-        int& src = dens ? srcd : srcc;
-        m->src_w[l] = src; src += I * O;
-        if (d->has_bias) { m->src_b[l] = src; src += O; } else m->src_b[l] = -1;
+        m->src_w[l] = dec.src_w[l]; m->src_b[l] = dec.src_b[l];
         maxw = max(maxw, max(m->Kp[l], m->Np[l]));
     }
-    m->blob_bytes = tc_round_up(off, 16);
+    m->blob_bytes = wb_round_up(off, 16);
     m->has_bias = d->has_bias ? 1 : 0;
     m->maxw = maxw;
     if (!backward) {
@@ -154,15 +141,14 @@ static void tc_dfeat_shape(const wb_nef_desc* d, int* planes, int* width)
     *planes = d->multiscale == 0 ? (d->lod_idx < d->num_lods ? d->lod_idx : d->num_lods) : 1;
     if (*planes < 0) *planes = 0;
 }
-static int64_t tc_align256(int64_t b) { return (b + 255) / 256 * 256; }
 
 // workspace layout (bytes): [ray_embed: R * Kc * 2][dfeat: planes * S * F * 2 (backward only)]
 int64_t wb_tc_workspace_bytes(const wb_nef_desc* nef, int64_t R, int64_t S, int backward)
 {
     WbTc m; if (wb_tc_make(nef, false, &m)) return -1;
     int planes, width; tc_dfeat_shape(nef, &planes, &width);
-    int64_t b = tc_align256(R * m.Kp[m.nl_d] * 2);
-    if (backward) b += tc_align256((int64_t)planes * S * width * 2);
+    int64_t b = wb_align256(R * m.Kp[m.nl_d] * 2);
+    if (backward) b += wb_align256((int64_t)planes * S * width * 2);
     return b + 256;
 }
 int wb_tc_supported(const wb_nef_desc* nef, int backward)
@@ -1055,7 +1041,7 @@ int wb_tc_decoder_bwd_ex(const wb_nef_desc* nef, const float* blob, const wb_ray
     if (!ray_rows_ready) { rc = tc_launch_ray_embed(m, rays, workspace, st); if (rc) return rc; }
     int planes, width; tc_dfeat_shape(nef, &planes, &width);
     const int64_t R = rays->num_rays;
-    __half* dfeat = reinterpret_cast<__half*>(reinterpret_cast<uint8_t*>(workspace) + tc_align256(R * m.Kp[m.nl_d] * 2));
+    __half* dfeat = reinterpret_cast<__half*>(reinterpret_cast<uint8_t*>(workspace) + wb_align256(R * m.Kp[m.nl_d] * 2));
     TcIn in = { rays->origins, rays->dirs, rec_t, rec_ray, S, reinterpret_cast<const uint4*>(workspace), nullptr, reinterpret_cast<const uint4*>(feat_saved),
                 s_begin, s_end };
     if (s_end <= s_begin) return WB_OK;
@@ -1098,7 +1084,7 @@ int wb_tc_table_scatter(const wb_nef_desc* nef, const wb_rays* rays, const float
     WB_CHECK_ARG(scale != nullptr && workspace != nullptr && (grad_table != nullptr || gx.kind != 0), "null pointer");
     int planes, width; tc_dfeat_shape(nef, &planes, &width);
     const int64_t R = rays->num_rays;
-    const __half* dfeat = reinterpret_cast<const __half*>(reinterpret_cast<const uint8_t*>(workspace) + tc_align256(R * m.Kp[m.nl_d] * 2));
+    const __half* dfeat = reinterpret_cast<const __half*>(reinterpret_cast<const uint8_t*>(workspace) + wb_align256(R * m.Kp[m.nl_d] * 2));
     TcIn in = { rays->origins, rays->dirs, rec_t, rec_ray, S, nullptr, nullptr, nullptr, s_begin, s_end };
     if (gx.kind != 0) {
         int64_t bx = (S + 255) / 256; const int64_t cap = (int64_t)wb_num_sms() * 16; if (bx > cap) bx = cap;

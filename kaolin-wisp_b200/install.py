@@ -7,7 +7,7 @@ What is patched (reference file:line -> native replacement):
   OctreeAS._raymarch_ray / _voxel / _uniform    (octree_as.py:188-374)             wb_raymarch_*
   TriplanarGrid.interpolate                     (triplanar_grid.py:98-121)         wb_triplane_*
   OctreeGrid.interpolate                        (octree_grid.py:165-219)           wb_octree_interp_*
-  PackedRFTracer.trace                          (packed_rf_tracer.py:84-181)       fused render path (ops.rf_trace)
+  PackedRFTracer.trace                          (packed_rf_tracer.py:84-181)       fused render path (ops.rf_trace_nef)
   PackedSDFTracer.trace                         (packed_sdf_tracer.py:57-174)      wb_sdf_trace
   PackedSPCTracer.trace                         (packed_spc_tracer.py:37-90)       wb_spc_trace (torch + OctreeAS.raytrace below max_level)
   NeuralSDF.sdf (no-grad)                       (neural_sdf.py:120-155)            wb_sdf_eval

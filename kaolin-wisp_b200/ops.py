@@ -995,10 +995,7 @@ class NefSpec:
         if self.kind == "hash":
             d = A.make_grid_desc(grid[0], self.resolutions, self.begin_idxes, self.codebook_size, self.multiscale, self.lod_idx)
         else:
-            d = A.NefDesc()
-            d.grid_kind = GRID_KINDS[self.kind]
-            d.num_lods, d.feature_dim, d.codebook_size = self.num_lods, self.feature_dim, 0
-            d.multiscale, d.lod_idx = (0 if self.multiscale == "cat" else 1), self.num_lods
+            d = self.header()
             d.grid_layout = int(layout)
             for i, r in enumerate(self.resolutions):
                 d.resolutions[i] = int(r)
@@ -1015,6 +1012,16 @@ class NefSpec:
         if not self.fill_decoders(d, dens_flat.data_ptr(), col_flat.data_ptr()):
             raise A.WispB200Error("decoder too deep for the fused path")
         return d, keep
+
+    def header(self):
+        """NefDesc holding the grid fields the decoder checks read: grid kind, LOD count, feature width, multiscale and lod_idx
+        (a triplanar or octree spec's LODs are all in use).  A hash spec's desc() gets the same fields from make_grid_desc."""
+        d = A.NefDesc()
+        d.grid_kind = GRID_KINDS[self.kind]
+        d.num_lods = len(self.resolutions) if self.kind == "hash" else self.num_lods
+        d.feature_dim, d.multiscale = self.feature_dim, (0 if self.multiscale == "cat" else 1)
+        d.lod_idx = self.lod_idx if self.kind == "hash" else self.num_lods
+        return d
 
     def fill_decoders(self, d, dens_params: int, col_params: int) -> bool:
         """The embedding and decoder fields of NefDesc `d`; False (nothing written) when a decoder is deeper than WB_MAX_LAYERS."""
@@ -1233,7 +1240,7 @@ class RFTraceFn(torch.autograd.Function):
         rec_t, rec_delta, rec_ray = march_fill_records(ms, dev)
         S, R = ms.total, ms.rays.num_rays
         shaded = _empty_s(S, (4,), torch.float32, dev)
-        # grad mode is always off inside Function.forward and needs_input_grad ignores torch.no_grad(): the caller (rf_trace)
+        # grad mode is always off inside Function.forward and needs_input_grad ignores torch.no_grad(): the caller (rf_trace_nef)
         # tells us whether a backward pass can follow, so that inference neither saves features nor needs the backward tiles
         need_grad = bool(want_grad) and any(ctx.needs_input_grad[8:])
         Scap = _bucket(S)                                  # byte sizes for the bucketed capacity (layouts still use S)
@@ -1325,14 +1332,8 @@ def precision_supported(spec: NefSpec, nef, precision: int, backward: bool) -> b
     if ans is None:
         # the query looks at widths only: stand-in one-element tensors, no parameter flattening
         dummy = torch.zeros(1)
-        d = A.NefDesc()
-        d.grid_kind = GRID_KINDS[spec.kind]
-        d.num_lods = spec.num_lods if spec.kind != "hash" else len(spec.resolutions)
-        d.feature_dim, d.multiscale = spec.feature_dim, (0 if spec.multiscale == "cat" else 1)
-        d.lod_idx = spec.lod_idx if spec.kind == "hash" else d.num_lods
-        if not spec.fill_decoders(d, dummy.data_ptr(), dummy.data_ptr()):
-            return False
-        ans = bool(A.lib().wb_rf_precision_supported(d, precision, 1 if backward else 0))
+        d = spec.header()
+        ans = spec.fill_decoders(d, dummy.data_ptr(), dummy.data_ptr()) and bool(A.lib().wb_rf_precision_supported(d, precision, 1 if backward else 0))
         _SUPPORT_CACHE[key] = ans
     return ans
 
@@ -1352,12 +1353,6 @@ def rf_trace_nef(ms: MarchState, spec: NefSpec, nef, bg, precision: int = 0):
     dens, col = decoder_params(nef.decoder_density), decoder_params(nef.decoder_color)
     octctx = _grid_context(nef, spec) if spec.kind == "octree" else None
     return RFTraceFn.apply(ms, spec, len(grid), len(dens), bg, precision, torch.is_grad_enabled(), octctx, *grid, *dens, *col)
-
-
-def rf_trace(ms: MarchState, spec: NefSpec, table: torch.Tensor, dens_params: Sequence[torch.Tensor],
-             col_params: Sequence[torch.Tensor], bg, precision: int = 0):
-    """Hash-grid form with explicit tensors -> rgb [R,3], depth [R,1], alpha [R,1], hit [R]."""
-    return RFTraceFn.apply(ms, spec, 1, len(dens_params), bg, precision, torch.is_grad_enabled(), None, table, *dens_params, *col_params)
 
 
 # --------------------------------------------------------------------------------------------------------------
