@@ -89,8 +89,53 @@ static bool tc_bwd_layout(WbTc* m, unsigned wmask, int groups)
     return m->smem_bytes <= TC_SMEM_MAX;
 }
 
-// returns WB_OK, or WB_ERR_INVALID with a message when the configuration does not fit the tensor-core path
-int wb_tc_make(const wb_nef_desc* d, bool backward, WbTc* m)
+// The decoder backward (wb_tc_make): npass passes over the samples, pass p with groups[p] sub-tile groups per CTA accumulating the
+// weight gradients of the layers in mask[p]; the last pass emits dL/dfeat, or where `fuses` may scatter it into the hash table.
+struct TcBwdPlan { int npass; unsigned mask[TC_ML]; int groups[TC_ML]; bool fuses; };
+
+// The passes of decoders m: the layers in order while their accumulators fit beside the tiles of one group, two groups per CTA where
+// they fit (they overlap each other's barrier and MMA latencies).  0 when the backward does not fit: it takes decoders whose whole
+// backward fits two groups per CTA in one pass, and those of the app/nerf depth (one hidden density layer, two hidden colour layers) up
+// to width 128, as long as each layer's accumulator fits beside the tiles of one group; deeper, wider decoders train on the fp32 kernels.
+static int tc_bwd_passes(WbTc m, unsigned masks[TC_ML], int groups[TC_ML])
+{
+    const int nl = m.nl_d + m.nl_c;
+    const bool one_pass = tc_bwd_layout(&m, (1u << nl) - 1u, 2);
+    bool passes = m.nl_d <= 2 && m.nl_c <= 3;
+    for (int l = 0; l < nl && passes; ++l) passes = tc_bwd_layout(&m, 1u << l, 1);
+    if (!one_pass && !passes) return 0;
+    int n = 0; unsigned cur = 0;
+    for (int l = 0; l < nl; ++l) {
+        if (cur && !tc_bwd_layout(&m, cur | (1u << l), 1)) { masks[n++] = cur; cur = 0; }
+        cur |= 1u << l;
+    }
+    masks[n++] = cur;
+    for (int p = 0; p < n; ++p) groups[p] = tc_bwd_layout(&m, masks[p], 2) ? 2 : 1;
+    return n;
+}
+
+// decoders m with the shared-memory plan of pass p
+static WbTc tc_bwd_pass(WbTc m, const TcBwdPlan& b, int p) { tc_bwd_layout(&m, b.mask[p], b.groups[p]); return m; }
+
+// workspace layout (bytes): [ray_embed: R * Kc * 2][dfeat: planes * S * F * 2 (backward only)].  dL/dfeat of R rays: its offset,
+// planes ('cat' -> one per live LOD, 'sum' -> one) and halfs per (plane, sample)
+struct TcDfeat { int64_t off; int planes, width; };
+static TcDfeat tc_dfeat(const wb_nef_desc* d, const WbTc& m, int64_t R)
+{
+    const int planes = d->multiscale == 0 ? (d->lod_idx < d->num_lods ? d->lod_idx : d->num_lods) : 1;
+    return { wb_align256(R * m.Kp[m.nl_d] * 2), planes < 0 ? 0 : planes, d->feature_dim };
+}
+
+// fused table scatter: F == 2 'cat' hash grids with <= 16 live LODs (32 features: the scratch tile), when the pass planned in m
+// runs two groups per CTA; with one group per SM the stand-alone scatter kernel runs beside the decoder CTAs instead
+static bool tc_bwd_fuses(const wb_nef_desc* nef, const WbTc& m, int planes)
+{
+    return nef->grid_kind == 0 && nef->feature_dim == 2 && nef->multiscale == 0 && planes <= 16 && m.groups > 1;
+}
+
+// The padded decoders and their parameter blob in *m, with the forward's shared-memory plan, or (bwd) with none and the backward's plan
+// in *bwd.  Returns WB_OK, or WB_ERR_INVALID with a message when that direction does not fit the tensor-core path.
+int wb_tc_make(const wb_nef_desc* d, WbTc* m, TcBwdPlan* bwd = nullptr)
 {
     WbDecoders dec; const int rc = wb_make_decoders(d, 128, "tensor-core path: layer widths must be <= 128", &dec); if (rc) return rc;
     const int dout = dec.O[dec.nl_d - 1];
@@ -112,55 +157,41 @@ int wb_tc_make(const wb_nef_desc* d, bool backward, WbTc* m)
     m->blob_bytes = wb_round_up(off, 16);
     m->has_bias = d->has_bias ? 1 : 0;
     m->maxw = maxw;
-    if (!backward) {
-        // every layer's input tile is overwritten in place by its output (the layer's MMAs have completed before the epilogue writes)
-        for (int l = 0; l < nl; ++l) m->tile_off[l] = 0;
-        m->scr_off = (maxw / 8) * TC_SLAB;
-        m->group_bytes = m->scr_off + TC_SCR_BYTES;
-        m->groups = TC_FWD_GROUPS;
-        m->w_smem_off = m->groups * m->group_bytes;
-        m->smem_bytes = m->w_smem_off + m->blob_bytes;
-        WB_CHECK_ARG(m->smem_bytes <= TC_SMEM_MAX, "tensor-core path: decoder does not fit in shared memory (use precision 0)");
+    if (bwd) {
+        bwd->npass = tc_bwd_passes(*m, bwd->mask, bwd->groups);
+        WB_CHECK_ARG(bwd->npass > 0, "tensor-core path: decoder backward does not fit in shared memory (use precision 0)");
+        bwd->fuses = tc_bwd_fuses(d, tc_bwd_pass(*m, *bwd, bwd->npass - 1), tc_dfeat(d, *m, 0).planes);
         return WB_OK;
     }
-    // backward: decoders whose whole backward fits two groups per CTA in one pass, and decoders of the app/nerf depth (one hidden
-    // density layer, two hidden colour layers) up to width 128, whose weight gradients may take several passes (every layer's
-    // accumulator must fit beside the tiles of one group); deeper, wider decoders train on the fp32 kernels
-    const bool one_pass = tc_bwd_layout(m, (1u << nl) - 1u, 2);
-    bool passes = m->nl_d <= 2 && m->nl_c <= 3;
-    for (int l = 0; l < nl && passes; ++l) passes = tc_bwd_layout(m, 1u << l, 1);
-    WB_CHECK_ARG(one_pass || passes, "tensor-core path: decoder backward does not fit in shared memory (use precision 0)");
-    tc_bwd_layout(m, (1u << nl) - 1u, 1);       // the plan of the first pass is left in *m
+    // every layer's input tile is overwritten in place by its output (the layer's MMAs have completed before the epilogue writes)
+    for (int l = 0; l < nl; ++l) m->tile_off[l] = 0;
+    m->scr_off = (maxw / 8) * TC_SLAB;
+    m->group_bytes = m->scr_off + TC_SCR_BYTES;
+    m->groups = TC_FWD_GROUPS;
+    m->w_smem_off = m->groups * m->group_bytes;
+    m->smem_bytes = m->w_smem_off + m->blob_bytes;
+    WB_CHECK_ARG(m->smem_bytes <= TC_SMEM_MAX, "tensor-core path: decoder does not fit in shared memory (use precision 0)");
     return WB_OK;
 }
 
-// number of dL/dfeat planes and halfs per (plane, sample): 'cat' -> one plane per live LOD, 'sum' -> a single plane
-static void tc_dfeat_shape(const wb_nef_desc* d, int* planes, int* width)
-{
-    *width = d->feature_dim;
-    *planes = d->multiscale == 0 ? (d->lod_idx < d->num_lods ? d->lod_idx : d->num_lods) : 1;
-    if (*planes < 0) *planes = 0;
-}
-
-// workspace layout (bytes): [ray_embed: R * Kc * 2][dfeat: planes * S * F * 2 (backward only)]
 int64_t wb_tc_workspace_bytes(const wb_nef_desc* nef, int64_t R, int64_t S, int backward)
 {
-    WbTc m; if (wb_tc_make(nef, false, &m)) return -1;
-    int planes, width; tc_dfeat_shape(nef, &planes, &width);
-    int64_t b = wb_align256(R * m.Kp[m.nl_d] * 2);
-    if (backward) b += wb_align256((int64_t)planes * S * width * 2);
+    WbTc m; if (wb_tc_make(nef, &m)) return -1;
+    const TcDfeat df = tc_dfeat(nef, m, R);
+    int64_t b = df.off;
+    if (backward) b += wb_align256((int64_t)df.planes * S * df.width * 2);
     return b + 256;
 }
 int wb_tc_supported(const wb_nef_desc* nef, int backward)
 {
-    WbTc m; if (wb_tc_make(nef, false, &m)) return 0;
-    if (backward && wb_tc_make(nef, true, &m)) return 0;
+    WbTc m; TcBwdPlan plan; if (wb_tc_make(nef, &m)) return 0;
+    if (backward && wb_tc_make(nef, &m, &plan)) return 0;
     return 1;
 }
 // the features are only saved for a backward pass: refuse here (at forward time) if that pass cannot run
 int64_t wb_tc_feat_bytes(const wb_nef_desc* nef, int64_t S)
 {
-    WbTc m; if (wb_tc_make(nef, true, &m) || wb_tc_make(nef, false, &m)) return -1;
+    WbTc m; TcBwdPlan plan; if (wb_tc_make(nef, &m, &plan) || wb_tc_make(nef, &m)) return -1;
     return (int64_t)m.Kp[0] * 2 * S + 256;
 }
 
@@ -186,11 +217,11 @@ __global__ void wb_tc_pack_kernel(WbTc m, const float* __restrict__ dens, const 
     }
 }
 
-int wb_tc_blob_floats(const wb_nef_desc* nef) { WbTc m; if (wb_tc_make(nef, false, &m)) return -1; return m.blob_bytes / 4; }
+int wb_tc_blob_floats(const wb_nef_desc* nef) { WbTc m; if (wb_tc_make(nef, &m)) return -1; return m.blob_bytes / 4; }
 
 int wb_tc_pack(const wb_nef_desc* nef, float* blob, cudaStream_t st)
 {
-    WbTc m; int rc = wb_tc_make(nef, false, &m); if (rc) return rc;
+    WbTc m; int rc = wb_tc_make(nef, &m); if (rc) return rc;
     wb_tc_pack_kernel<<<16, 256, 0, st>>>(m, nef->dens_params, nef->col_params, reinterpret_cast<uint8_t*>(blob));
     WB_LAUNCH_CHECK();
     return WB_OK;
@@ -575,18 +606,28 @@ static int tc_launch_ray_embed(const WbTc& m, const wb_rays* rays, void* workspa
     return WB_OK;
 }
 
-// CTAs per SM of the forward: more groups in flight hide the gather and chain latencies
-static int tc_fwd_per_sm(const WbTc& m, int grid_kind)
-{
-    const bool wide = m.maxw > 64;
-    int per_sm = max(1, min(3, TC_SMEM_MAX / (m.smem_bytes + 1024)));
-    if (grid_kind == 2) per_sm = min(per_sm, 2);        // the octree gather keeps more state per thread (up to 32 accumulators)
-    return wide ? min(per_sm, 2) : max(per_sm, 2);
-}
 // the app/nerf decoder on the hash grid: the forward instance compiled for its geometry
 static bool tc_fwd_nerf64(const WbTc& m, int grid_kind, int per_sm)
 {
     return m.maxw <= 64 && grid_kind == 0 && per_sm == 3 && TcShapeNerf64::matches(m);
+}
+
+using TcFwdKernel = decltype(&wb_shade_fwd_tc_kernel<2, false, 64>);
+// The forward instance of decoders m on grid kind `grid_kind` (the descriptor's, which wb_make_gridx copies into WbGridX::kind), and
+// its CTAs per SM: more groups in flight hide the gather and chain latencies, and the register bound of the instance must match them,
+// or the hardware silently runs fewer.  Decoders up to 64 wide: 2 or 3 CTAs (85 registers per thread); wider ones: 1 or 2 (a 128-wide
+// accumulator is 64 registers).
+static TcFwdKernel tc_fwd_kernel(const WbTc& m, int grid_kind, int& per_sm)
+{
+    const bool wide = m.maxw > 64, gx = grid_kind != 0;
+    per_sm = max(1, min(3, TC_SMEM_MAX / (m.smem_bytes + 1024)));
+    if (grid_kind == 2) per_sm = min(per_sm, 2);        // the octree gather keeps more state per thread (up to 32 accumulators)
+    per_sm = wide ? min(per_sm, 2) : max(per_sm, 2);
+    return tc_fwd_nerf64(m, grid_kind, per_sm) ? wb_shade_fwd_tc_kernel<3, false, 64, TcShapeNerf64>
+         : wide ? (gx ? (per_sm == 2 ? wb_shade_fwd_tc_kernel<2, true, 128> : wb_shade_fwd_tc_kernel<1, true, 128>)
+                      : (per_sm == 2 ? wb_shade_fwd_tc_kernel<2, false, 128> : wb_shade_fwd_tc_kernel<1, false, 128>))
+                : (gx ? (per_sm == 3 ? wb_shade_fwd_tc_kernel<3, true, 64> : wb_shade_fwd_tc_kernel<2, true, 64>)
+                      : (per_sm == 3 ? wb_shade_fwd_tc_kernel<3, false, 64> : wb_shade_fwd_tc_kernel<2, false, 64>));
 }
 
 int wb_tc_shade_fwd(const wb_nef_desc* nef, const float* blob, const wb_rays* rays, const float* rec_t, const int32_t* rec_ray,
@@ -594,20 +635,12 @@ int wb_tc_shade_fwd(const wb_nef_desc* nef, const float* blob, const wb_rays* ra
 {
     WbGrid g; int rc = wb_make_grid(nef, &g); if (rc) return rc;
     WbGridX gx; rc = wb_make_gridx(nef, false, &gx); if (rc) return rc;
-    WbTc m; rc = wb_tc_make(nef, false, &m); if (rc) return rc;
+    WbTc m; rc = wb_tc_make(nef, &m); if (rc) return rc;
     WB_CHECK_ARG(workspace != nullptr, "precision 1 needs the workspace (wb_rf_workspace_bytes)");
     rc = tc_launch_ray_embed(m, rays, workspace, st); if (rc) return rc;
     TcIn in = { rays->origins, rays->dirs, rec_t, rec_ray, S, reinterpret_cast<const uint4*>(workspace), reinterpret_cast<uint4*>(feat_save), nullptr };
-    // CTAs per SM (tc_fwd_per_sm): the register bound of the instantiation must match, or the hardware silently runs fewer.
-    // Decoders up to 64 wide: 2 or 3 CTAs (85 registers per thread); wider ones: 1 or 2 (a 128-wide accumulator is 64 registers).
-    const bool wide = m.maxw > 64;
-    const int per_sm = tc_fwd_per_sm(m, gx.kind);
-    const bool nerf64 = tc_fwd_nerf64(m, gx.kind, per_sm);
-    auto kern = nerf64 ? wb_shade_fwd_tc_kernel<3, false, 64, TcShapeNerf64>
-              : wide ? (gx.kind != 0 ? (per_sm == 2 ? wb_shade_fwd_tc_kernel<2, true, 128> : wb_shade_fwd_tc_kernel<1, true, 128>)
-                                     : (per_sm == 2 ? wb_shade_fwd_tc_kernel<2, false, 128> : wb_shade_fwd_tc_kernel<1, false, 128>))
-                     : (gx.kind != 0 ? (per_sm == 3 ? wb_shade_fwd_tc_kernel<3, true, 64> : wb_shade_fwd_tc_kernel<2, true, 64>)
-                                     : (per_sm == 3 ? wb_shade_fwd_tc_kernel<3, false, 64> : wb_shade_fwd_tc_kernel<2, false, 64>));
+    int per_sm;
+    const TcFwdKernel kern = tc_fwd_kernel(m, nef->grid_kind, per_sm);
     WB_CUDA(wb_allow_smem(kern, m.smem_bytes));
     const int64_t ntiles = (S + TC_ROWS - 1) / TC_ROWS, nctas = (ntiles + TC_FWD_GROUPS - 1) / TC_FWD_GROUPS;
     int64_t grid = (int64_t)wb_num_sms() * per_sm; if (grid > nctas) grid = nctas;
@@ -1008,24 +1041,13 @@ wb_featx_scatter_kernel(WbGridX gx, TcIn in, const __half* __restrict__ dfeat, i
     }
 }
 
-// the launches of one decoder backward: layer masks of the weight-grad accumulators that fit beside the tiles, and the group count
-static int tc_bwd_passes(WbTc* m, unsigned masks[TC_ML])
+using TcBwdKernel = decltype(&wb_mlp_bwd_tc_kernel<1, false>);
+// pass p's instance, and `fuse`: it runs the table scatter (the last pass, where the plan fuses, given a table gradient)
+static TcBwdKernel tc_bwd_kernel(const WbTc& m, const TcBwdPlan& b, int p, bool table, bool& fuse)
 {
-    const int nl = m->nl_d + m->nl_c;
-    int n = 0; unsigned cur = 0;
-    for (int l = 0; l < nl; ++l) {
-        if (cur && !tc_bwd_layout(m, cur | (1u << l), 1)) { masks[n++] = cur; cur = 0; }
-        cur |= 1u << l;
-    }
-    masks[n++] = cur;
-    return n;
-}
-
-// fused table scatter: F == 2 'cat' hash grids with <= 16 live LODs (32 features: the scratch tile), when the pass planned in *m
-// runs two groups per CTA
-static bool tc_bwd_fuses(const wb_nef_desc* nef, const WbTc& m, int planes)
-{
-    return nef->grid_kind == 0 && nef->feature_dim == 2 && nef->multiscale == 0 && planes <= 16 && m.groups > 1;
+    fuse = table && p == b.npass - 1 && b.fuses;
+    if (fuse && TcShapeNerf64::matches(m)) return wb_mlp_bwd_tc_kernel<2, true, TcShapeNerf64>;       // compiled for its geometry
+    return b.groups[p] == 2 ? (fuse ? wb_mlp_bwd_tc_kernel<2, true> : wb_mlp_bwd_tc_kernel<2, false>) : wb_mlp_bwd_tc_kernel<1, false>;
 }
 
 // decoder backward: dL/d(shaded) -> weight gradients + dL/dfeat planes in the workspace (or, fused, the hash-table scatter)
@@ -1035,38 +1057,26 @@ int wb_tc_decoder_bwd_ex(const wb_nef_desc* nef, const float* blob, const wb_ray
                          cudaStream_t st)
 {
     if (fused_out) *fused_out = 0;
-    WbTc m; int rc = wb_tc_make(nef, true, &m); if (rc) return rc;
+    WbTc m; TcBwdPlan plan; int rc = wb_tc_make(nef, &m, &plan); if (rc) return rc;
     WB_CHECK_ARG(scale != nullptr, "precision 1 needs the device loss-scale pointer");
     WB_CHECK_ARG(feat_saved != nullptr && workspace != nullptr, "precision 1 backward needs the saved features and the workspace");
     if (!ray_rows_ready) { rc = tc_launch_ray_embed(m, rays, workspace, st); if (rc) return rc; }
-    int planes, width; tc_dfeat_shape(nef, &planes, &width);
-    const int64_t R = rays->num_rays;
-    __half* dfeat = reinterpret_cast<__half*>(reinterpret_cast<uint8_t*>(workspace) + wb_align256(R * m.Kp[m.nl_d] * 2));
+    const TcDfeat df = tc_dfeat(nef, m, rays->num_rays);
     TcIn in = { rays->origins, rays->dirs, rec_t, rec_ray, S, reinterpret_cast<const uint4*>(workspace), nullptr, reinterpret_cast<const uint4*>(feat_saved),
                 s_begin, s_end };
     if (s_end <= s_begin) return WB_OK;
-    TcGrads G = { grad_dens, grad_col, scale, dfeat, planes, width };
-    unsigned masks[TC_ML];
-    const int npass = tc_bwd_passes(&m, masks);
-    for (int p = 0; p < npass; ++p) {
-        tc_bwd_layout(&m, masks[p], 1);
-        // two groups per CTA where they fit (the groups overlap each other's barrier and MMA latencies)
-        { WbTc m2 = m; if (tc_bwd_layout(&m2, masks[p], 2)) m = m2; }
-        const bool emit = p == npass - 1;
-        // fused table scatter: F == 2 'cat' hash grids with <= 16 live LODs (32 features: the scratch tile), when the pass runs two
-        // groups per CTA; with one group per SM the stand-alone scatter kernel runs beside the decoder CTAs instead
-        const bool fuse = emit && grad_table != nullptr && tc_bwd_fuses(nef, m, planes);
+    TcGrads G = { grad_dens, grad_col, scale, reinterpret_cast<__half*>(static_cast<uint8_t*>(workspace) + df.off), df.planes, df.width };
+    for (int p = 0; p < plan.npass; ++p) {
+        const WbTc mp = tc_bwd_pass(m, plan, p);
+        bool fuse;
+        const TcBwdKernel kern = tc_bwd_kernel(m, plan, p, grad_table != nullptr, fuse);
         WbGrid g; memset(&g, 0, sizeof(g));
         if (fuse) { rc = wb_make_grid(nef, &g); if (rc) return rc; }
-        // the app/nerf decoder: the instance compiled for its geometry
-        const bool nerf64 = fuse && TcShapeNerf64::matches(m);
-        auto kern = nerf64 ? wb_mlp_bwd_tc_kernel<2, true, TcShapeNerf64>
-                  : m.groups == 2 ? (fuse ? wb_mlp_bwd_tc_kernel<2, true> : wb_mlp_bwd_tc_kernel<2, false>) : wb_mlp_bwd_tc_kernel<1, false>;
         WB_CUDA(wb_allow_smem(kern, TC_SMEM_MAX));         // the passes of one call differ in size: allow the largest once
-        const int64_t nctas = ((s_end - s_begin + s_begin % TC_ROWS + TC_ROWS - 1) / TC_ROWS + m.groups - 1) / m.groups;
+        const int64_t nctas = ((s_end - s_begin + s_begin % TC_ROWS + TC_ROWS - 1) / TC_ROWS + mp.groups - 1) / mp.groups;
         int64_t grid = (int64_t)wb_num_sms(); if (grid > nctas) grid = nctas;         // 1 CTA / SM: shared memory holds the tiles and accumulators
-        kern<<<(unsigned)grid, m.groups * TC_GROUP, m.smem_bytes, st>>>(m, reinterpret_cast<const uint8_t*>(blob), in,
-                                                                        reinterpret_cast<const float4*>(g_shaded), G, masks[p], emit ? 1 : 0, g, grad_table);
+        kern<<<(unsigned)grid, mp.groups * TC_GROUP, mp.smem_bytes, st>>>(mp, reinterpret_cast<const uint8_t*>(blob), in, reinterpret_cast<const float4*>(g_shaded),
+                                                                          G, plan.mask[p], p == plan.npass - 1 ? 1 : 0, g, grad_table);
         WB_LAUNCH_CHECK();
         if (fuse && fused_out) *fused_out = 1;
     }
@@ -1080,19 +1090,19 @@ int wb_tc_table_scatter(const wb_nef_desc* nef, const wb_rays* rays, const float
 {
     WbGrid g; int rc = wb_make_grid(nef, &g); if (rc) return rc;
     WbGridX gx; rc = wb_make_gridx(nef, true, &gx); if (rc) return rc;
-    WbTc m; rc = wb_tc_make(nef, true, &m); if (rc) return rc;
+    // refuse the decoders whose backward does not fit: no decoder backward wrote their planes
+    WbTc m; TcBwdPlan plan; rc = wb_tc_make(nef, &m, &plan); if (rc) return rc;
     WB_CHECK_ARG(scale != nullptr && workspace != nullptr && (grad_table != nullptr || gx.kind != 0), "null pointer");
-    int planes, width; tc_dfeat_shape(nef, &planes, &width);
-    const int64_t R = rays->num_rays;
-    const __half* dfeat = reinterpret_cast<const __half*>(reinterpret_cast<const uint8_t*>(workspace) + wb_align256(R * m.Kp[m.nl_d] * 2));
+    const TcDfeat df = tc_dfeat(nef, m, rays->num_rays);
+    const __half* dfeat = reinterpret_cast<const __half*>(static_cast<const uint8_t*>(workspace) + df.off);
     TcIn in = { rays->origins, rays->dirs, rec_t, rec_ray, S, nullptr, nullptr, nullptr, s_begin, s_end };
     if (gx.kind != 0) {
         int64_t bx = (S + 255) / 256; const int64_t cap = (int64_t)wb_num_sms() * 16; if (bx > cap) bx = cap;
-        wb_featx_scatter_kernel<<<(unsigned)bx, 256, 0, st>>>(gx, in, dfeat, width, scale);
+        wb_featx_scatter_kernel<<<(unsigned)bx, 256, 0, st>>>(gx, in, dfeat, df.width, scale);
         WB_LAUNCH_CHECK();
         return WB_OK;
     }
-    const int levels = g.multiscale == 0 ? planes : g.L;
+    const int levels = g.multiscale == 0 ? df.planes : g.L;
     if (levels > 0 && s_end > s_begin) {
         int64_t bx = (s_end - s_begin + 255) / 256; const int64_t cap = (int64_t)wb_num_sms() * TC_SCATTER_CTAS_PER_SM; if (bx > cap) bx = cap;
         dim3 grid2((unsigned)bx, (unsigned)((levels + TC_SCATTER_LODS - 1) / TC_SCATTER_LODS));
@@ -1104,19 +1114,15 @@ int wb_tc_table_scatter(const wb_nef_desc* nef, const wb_rays* rays, const float
 }
 
 // *shaped = 1 when the forward (backward == 0) or the decoder backward with the fused table scatter (backward == 1) of this decoder
-// runs an instance compiled for its geometry, as wb_tc_shade_fwd / wb_tc_decoder_bwd_ex choose it; 0 when it runs the run-time one
+// runs an instance compiled for its geometry (the launches' own choice: tc_fwd_kernel, tc_bwd_kernel); 0 when it runs a run-time one
 int wb_tc_shaped(const wb_nef_desc* nef, int backward, int* shaped)
 {
     WB_CHECK_ARG(shaped != nullptr, "null pointer");
     *shaped = 0;
-    WbTc m; int rc = wb_tc_make(nef, backward != 0, &m); if (rc) return rc;
-    if (!backward) { *shaped = tc_fwd_nerf64(m, nef->grid_kind, tc_fwd_per_sm(m, nef->grid_kind)) ? 1 : 0; return WB_OK; }
-    int planes, width; tc_dfeat_shape(nef, &planes, &width);
-    unsigned masks[TC_ML];
-    const int npass = tc_bwd_passes(&m, masks);
-    tc_bwd_layout(&m, masks[npass - 1], 1);
-    { WbTc m2 = m; if (tc_bwd_layout(&m2, masks[npass - 1], 2)) m = m2; }
-    *shaped = tc_bwd_fuses(nef, m, planes) && TcShapeNerf64::matches(m) ? 1 : 0;
+    WbTc m; TcBwdPlan plan; int rc = wb_tc_make(nef, &m, backward ? &plan : nullptr); if (rc) return rc;
+    int per_sm; bool fuse;
+    if (!backward) *shaped = tc_fwd_kernel(m, nef->grid_kind, per_sm) ==wb_shade_fwd_tc_kernel<3, false, 64, TcShapeNerf64>;
+    else *shaped = tc_bwd_kernel(m, plan, plan.npass - 1, true, fuse) == wb_mlp_bwd_tc_kernel<2, true, TcShapeNerf64>;
     return WB_OK;
 }
 
@@ -1150,23 +1156,16 @@ int wb_tc_shade_bwd(const wb_nef_desc* nef, const float* blob, const wb_rays* ra
                     int64_t S, const float* g_shaded, const float* scale, const void* feat_saved, void* workspace, bool ray_rows_ready,
                     float* grad_table, float* grad_dens, float* grad_col, cudaStream_t st)
 {
-    {
-        WbTc m; unsigned masks[TC_ML];
-        TcSide* side = nullptr;
-        bool wide = false;         // one group per SM (wide decoders): the decoder backward leaves most warp slots idle
-        if (S >= TC_CHUNKED_MIN_S && nef->grid_kind == 0 && grad_table && wb_tc_make(nef, true, &m) == WB_OK) {
-            tc_bwd_passes(&m, masks);
-            tc_bwd_layout(&m, masks[0], 1);
-            wide = !tc_bwd_layout(&m, masks[0], 2);
-        }
-        // A call being captured into a graph runs the one-stream schedule (the same sums up to the order of the atomic additions): the
-        // shared side stream would otherwise join the capture, and another thread's eager call on it would be mixed into the graph.
-        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-        if (wide && cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap != cudaStreamCaptureStatusNone) wide = false;
-        TcSide* slot = wide ? tc_side_slot() : nullptr;
-        std::unique_lock<std::mutex> lock;
-        if (slot) { lock = std::unique_lock<std::mutex>(slot->mu); side = tc_side_stream_locked(*slot); }
-        if (side != nullptr) {
+    // one group per SM in the first pass (wide decoders): the decoder backward leaves most warp slots idle
+    WbTc m; TcBwdPlan plan;
+    bool wide = S >= TC_CHUNKED_MIN_S && nef->grid_kind == 0 && grad_table && wb_tc_make(nef, &m, &plan) == WB_OK && plan.groups[0] == 1;
+    // A call being captured into a graph runs the one-stream schedule (the same sums up to the order of the atomic additions): the
+    // shared side stream would otherwise join the capture, and another thread's eager call on it would be mixed into the graph.
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    if (wide && cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap != cudaStreamCaptureStatusNone) wide = false;
+    if (TcSide* slot = wide ? tc_side_slot() : nullptr) {
+        std::lock_guard<std::mutex> lock(slot->mu);
+        if (TcSide* side = tc_side_stream_locked(*slot)) {
             const int64_t per = ((S + TC_CHUNKS - 1) / TC_CHUNKS + TC_ROWS - 1) / TC_ROWS * TC_ROWS;
             int rc = WB_OK, c = 0;
             for (int64_t s0 = 0; s0 < S && rc == WB_OK; s0 += per, ++c) {

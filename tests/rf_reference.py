@@ -20,7 +20,7 @@ Rounding points
   scatters   one fp32 product fl(g * w) per texel / corner (precision 1: g = fl(h * inv_scale) of the fp16 dL/dfeat plane, exact:
              the scale is a power of two), added by atomics in any order, after at most 5 levels of the segmented warp scan at
              precision 1: gamma(n_terms + levels) * sum|terms| per entry, plus the propagated radius of g.  dL/dfeat feature f lives
-             in plane f / width at column f % width (tc_dfeat_shape).
+             in plane f / width at column f % width (tc_dfeat).
   decoders   (precision 0, wb_shade.cu) wb_layer_fwd: per unit an fp32 fma chain seeded with the bias over the inputs in
              ascending order, emulated on the centres (sdf_reference._chain); sinf / cosf of the view embedding within 2 ulp;
              rgb = 1 / (1 + expf(-c)) within tc_decoders.SIGMOID_REL; sigma = max(df0, 0).  Backward: gout = (go * r) * (1 - r)

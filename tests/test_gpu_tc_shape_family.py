@@ -56,7 +56,7 @@ def tc_refuses(case):
 
 
 def fwd_per_sm(Kp, Np):
-    """tc_fwd_per_sm for a hash grid: from the forward's shared memory, which only the padded widths set."""
+    """The CTAs per SM that tc_fwd_kernel picks for a hash grid: from the forward's shared memory, which only the padded widths set."""
     maxw = max(Kp + Np)
     blob = _r16(sum(k * n * 2 + n * 32 for k, n in zip(Kp, Np)))
     smem = 2 * (maxw // 8 * TC_SLAB + TC_SCR_BYTES) + blob
@@ -65,7 +65,7 @@ def fwd_per_sm(Kp, Np):
 
 
 def live_planes(case):
-    """tc_dfeat_shape: one plane per live LOD ('cat'), one plane ('sum')."""
+    """tc_dfeat's planes: one plane per live LOD ('cat'), one plane ('sum')."""
     if case.multiscale != "cat":
         return 1
     return case.L if case.lod_idx < 0 else max(0, min(case.lod_idx, case.L))
@@ -73,7 +73,7 @@ def live_planes(case):
 
 def nerf64_expected(case, backward):
     """What wb_rf_tc_shaped(desc, backward) reports: TcShapeNerf64::matches, plus tc_fwd_nerf64 (forward) or tc_bwd_fuses (backward,
-    the last pass as bwd_plan / tc_bwd_layout plan it).  A descriptor the library refuses is not shaped."""
+    the last pass as bwd_plan / tc_bwd_passes plan it).  A descriptor the library refuses is not shaped."""
     if tc_refuses(case):
         return 0
     nd, nc, Kp, Np = padded_dims(case)
